@@ -166,7 +166,10 @@ XGB_DLL int XGB200BuildRootHistogram(BoosterHandle handle, DMatrixHandle dmat, c
 /* same with a kernel choice and an optional row subset: mode 0 = production choice (TMA-staged root kernel), 1 = gather
  * kernel, 2 = G-only TMA root kernel (constant-hessian fast path: the H plane of out_hist stays zero).  With row_ids
  * (n_ids entries, ascending or not) the histogram covers that subset and gpair is given by POSITION (gpair[i] belongs to
- * row row_ids[i]) -- the deeper tree levels' access pattern.  out_kernel: name of the kernel variant that ran. */
+ * row row_ids[i]) -- the deeper tree levels' access pattern.  Added to the mode: 4 = the tail bytes come from where the
+ * training path takes them (by position for a 4-wide tail the line-aligned row copy does not hold; that copy's line when it
+ * does), 8 = G-only payload of the constant-hessian levels (only g of gpair is used, h == 1.0f for every row).
+ * out_kernel: name of the kernel variant that ran. */
 XGB_DLL int XGB200BuildHistogramEx(BoosterHandle handle, DMatrixHandle dmat, const float* gpair, int repeats, int mode,
                              const unsigned* row_ids, bst_ulong n_ids, int64_t* out_hist, float* scales, float* out_ms,
                              const char** out_kernel);
@@ -179,8 +182,9 @@ XGB_DLL int XGB200TimerStart(void);
 XGB_DLL int XGB200TimerStop(float* out_ms);
 /* per-kernel profile of the tree builder (CUDA events around each launch group of the rounds run while enabled): enable,
  * run rounds, then read {"root_hist_ms","root_hist_launches","root_hist_rows","deep_hist_ms","deep_hist_launches",
- * "deep_hist_rows","part_ms","part_launches","part_rows" (rows of split nodes),"part_rows_written","margin_ms",
- * "margin_launches","margin_rows"} */
+ * "deep_hist_rows","part_ms","part_launches","part_rows" (rows of split nodes),"part_rows_written","part_row_bytes_in_root",
+ * "part_row_bytes_in","part_row_bytes_out" (the partition's bytes per row read at the root level, read at deeper levels and
+ * written),"margin_ms","margin_launches","margin_rows"} */
 XGB_DLL int XGB200BoosterSetProfile(BoosterHandle handle, int enable);
 XGB_DLL int XGB200BoosterGetProfile(BoosterHandle handle, const char** out_json);
 /* number of CUDA kernels this library has launched so far in this process */

@@ -4,8 +4,12 @@ update, timed with CUDA events around each launch group (Booster profile mode) o
     python microbench/partition_profile.py --rows 50000000 --cols 100 [--out partition_profile.json]
 The round time is taken over graph-replayed rounds (as bench.py times them); the profiled rounds that follow are issued
 directly so that every launch group can be bracketed.
-Partition byte model per split level: rows * (4 [row id, 0 at the root] + 8 [(g,h)] + tail + 1 [split-feature byte]) read,
-plus (4 + 8 + tail) per row written; tail = 4 when the rows' 4 tail bin bytes travel with their ids, else 0."""
+Partition byte model per row, as the library reports it for the profiled trees (profile keys part_row_bytes_*):
+  read at the root level:   8 [the float2 gpair, also when only g is kept] + tail + 1 [split-feature byte]
+  read at deeper levels:    4 [row id] + payload + tail + 1
+  written:                  4 + payload + tail
+payload = 4 (g alone, constant-hessian objectives) or 8 ((g,h)); tail = 4 when the rows' 4 tail bin bytes travel with their
+ids (a 4-wide tail that the line-aligned row copy does not hold), else 0."""
 import argparse
 import json
 import os
@@ -15,16 +19,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def tail_width(F):
-    a, rem = divmod(F, 32)
-    return 4 if a >= 1 and 1 <= rem <= 4 else 0
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=50_000_000)
     ap.add_argument("--cols", type=int, default=100)
     ap.add_argument("--max-depth", type=int, default=6)
+    ap.add_argument("--objective", default="reg:squarederror")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--timed", type=int, default=10)
     ap.add_argument("--profiled", type=int, default=3)
@@ -35,12 +35,12 @@ def main():
     import sagemaker_xgboost_container_b200 as xgb
     be = xgb.get_backend()
     dev = torch.device("cuda", 0)
-    ba = argparse.Namespace(rows=a.rows, cols=a.cols, seed=43, objective="reg:squarederror", num_class=0)
+    ba = argparse.Namespace(rows=a.rows, cols=a.cols, seed=43, objective=a.objective, num_class=0)
     X, y = bench.gen_shard(ba, 0, a.rows, dev)
     d = xgb.DMatrix(X, label=y.cpu().numpy())
     del X
     torch.cuda.empty_cache()
-    params = bench.params_of(argparse.Namespace(objective="reg:squarederror", max_depth=a.max_depth, max_bin=256, num_class=0))
+    params = bench.params_of(argparse.Namespace(objective=a.objective, max_depth=a.max_depth, max_bin=256, num_class=0))
     b = xgb.Booster(params, [d])
     it = 0
     for _ in range(a.warmup):
@@ -56,9 +56,9 @@ def main():
     p = be.booster_get_profile(b.handle)
     be.booster_set_profile(b.handle, False)
     R = a.profiled
-    tw = tail_width(a.cols)
     root_rows = a.rows * R                        # the root split reads all rows without row ids (every profiled tree splits its root)
-    part_bytes = p["part_rows"] * (8 + tw + 1) + (p["part_rows"] - root_rows) * 4 + p["part_rows_written"] * (4 + 8 + tw)
+    part_bytes = (root_rows * p["part_row_bytes_in_root"] + (p["part_rows"] - root_rows) * p["part_row_bytes_in"] +
+                  p["part_rows_written"] * p["part_row_bytes_out"])
     peak = bench.hbm_peak()[0]
     part_gbs = part_bytes / (p["part_ms"] * 1e-3) / 1e9 if p["part_ms"] > 0 else 0.0
     name = torch.cuda.get_device_name(dev)
@@ -68,7 +68,7 @@ def main():
         power_w = pynvml.nvmlDeviceGetPowerManagementLimit(pynvml.nvmlDeviceGetHandleByIndex(0)) / 1000.0
     except Exception:
         power_w = None
-    out = {"gpu": name, "power_limit_w": power_w, "rows": a.rows, "cols": a.cols, "max_depth": a.max_depth, "profiled_rounds": R,
+    out = {"gpu": name, "power_limit_w": power_w, "rows": a.rows, "cols": a.cols, "objective": a.objective, "max_depth": a.max_depth, "profiled_rounds": R,
            "round_ms": round_ms,
            "per_round_ms": {"root_hist": p["root_hist_ms"] / R, "deep_hist": p["deep_hist_ms"] / R, "partition": p["part_ms"] / R,
                             "update_margin": p["margin_ms"] / R},
@@ -76,6 +76,7 @@ def main():
                                   "partition": p["part_launches"] / R, "update_margin": p["margin_launches"] / R},
            "partition_share_of_round": p["part_ms"] / R / round_ms,
            "partition_rows_per_round": p["part_rows"] / R, "partition_rows_written_per_round": p["part_rows_written"] / R,
+           "partition_row_bytes": {"in_root": p["part_row_bytes_in_root"], "in": p["part_row_bytes_in"], "out": p["part_row_bytes_out"]},
            "partition_bytes_per_round": part_bytes / R, "partition_gbs": part_gbs, "partition_frac_of_peak": part_gbs / peak,
            "peak_gbs": peak, "profile": p}
     print(json.dumps(out), flush=True)

@@ -158,9 +158,12 @@ void DMatrix::bin_with_cuts() {
   bins_gather.release();
   static const bool no_aligned = getenv("B200XGB_NO_ALIGNED_ROWS") != nullptr;
   if (ngroups * kSlots == 96 && !no_aligned) {           // 96 B rows straddle 128 B DRAM lines half of the time: the gathered levels read an aligned copy
+    // An 8-wide tail goes into the pad of the line (offset 96): the gathered levels then take it from the line they fetch
+    // anyway instead of gathering 8 B from bins_tail by row id.  A 4-wide tail stays out: it travels with the row ids, and a
+    // second request per gathered row into the line cost more in the histograms than it saved in the partition (DESIGN §6).
     gather_stride = 128;
     bins_gather.alloc((size_t)n * 128 + 128);
-    launch_pad_rows(bins.p, n, 96, bins_gather.p, 128, s);
+    launch_pad_rows(bins.p, bins_tail.p, tw == 8 ? 8 : 0, n, 96, bins_gather.p, 128, s);
   }
   bins_col.alloc((size_t)std::max(F, 1) * n);
   launch_transpose_bins(bins.p, bins_tail.p, n, F, ngroups, tw, bins_col.p, s);
@@ -281,7 +284,7 @@ struct TreeGraph {
 };
 
 struct GrowerImpl {
-  int64_t n = 0; int ngroups = 0, tw = 0, max_depth = 0, max_nodes = 0, cap_nodes = 0, max_level_nodes = 0, region = 0;
+  int64_t n = 0; int ngroups = 0, tw = 0, max_depth = 0, max_nodes = 0, cap_nodes = 0, max_level_nodes = 0, region = 0; bool tail_pos = false;
   int lg_iters = 0;                        // grow_policy=lossguide: expansions per tree (0 = depthwise)
   size_t slot_stride = 0;                  // GH64 entries per histogram slot
   int64_t gp_stride = 0;                   // rows reserved per class in gpair
@@ -292,6 +295,7 @@ struct GrowerImpl {
   DevBuf<unsigned char> tree_block;        // header + TreeArrays, copied to the host in one piece
   size_t tree_block_bytes = 0;
   DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx0, ridx1, scratch;
+  // gp0 / gp1: the gradients in partition (position) order; float g alone in the first n floats for constant-hessian objectives
   DevBuf<float2> gpair, gp0, gp1; DevBuf<unsigned> tl0, tl1; DevBuf<int> err, tree_index_dev, monotone_dev; DevBuf<unsigned char> feat_mask, ic_path, ic_allowed, ic_sets;
   std::vector<unsigned char> ic_sets_host; // what ic_sets holds
   std::vector<int> monotone_host;          // what monotone_dev holds (re-uploaded when the constraints or the feature count change)
@@ -300,11 +304,12 @@ struct GrowerImpl {
   DevBuf<DevNode> packed; std::vector<TreeGraph> graphs; std::vector<char> eager_done;
   TreeGraph* capturing = nullptr;          // set while enqueue_tree runs under stream capture: collectives cut the capture
 
-  void ensure(int64_t n_, int ngroups_, int tw_, int max_depth_, int K, int lg_iters_ = 0) {
+  // tail_pos: the rows' 4 tail bytes travel with their ids through the partition (a 4-wide tail that is not in bins_gather)
+  void ensure(int64_t n_, int ngroups_, int tw_, bool tail_pos_, int max_depth_, int K, int lg_iters_ = 0) {
     const int64_t stride_ = (n_ + 63) & ~(int64_t)63;
-    if (n == n_ && ngroups == ngroups_ && tw == tw_ && max_depth == max_depth_ && lg_iters == lg_iters_ && gpair.n >= (size_t)stride_ * K + 512) return;
+    if (n == n_ && ngroups == ngroups_ && tw == tw_ && tail_pos == tail_pos_ && max_depth == max_depth_ && lg_iters == lg_iters_ && gpair.n >= (size_t)stride_ * K + 512) return;
     if (lg_iters_ == 0) B200_CHECK(max_depth_ >= 1 && max_depth_ <= kMaxDepth, "max_depth must be in [1, 16] for the B200 depth-wise hist builder");
-    n = n_; ngroups = ngroups_; tw = tw_; max_depth = max_depth_; lg_iters = lg_iters_; gp_stride = stride_; root_h_valid = false;
+    n = n_; ngroups = ngroups_; tw = tw_; tail_pos = tail_pos_; max_depth = max_depth_; lg_iters = lg_iters_; gp_stride = stride_; root_h_valid = false;
     if (peer_reduce_active()) {                     // peers still map the buffers that are about to be freed: unmap everywhere first
       peer_reduce_close();
       DevBuf<unsigned> bar; bar.alloc(1); bar.zero(engine_stream());
@@ -329,7 +334,7 @@ struct GrowerImpl {
     ridx0.alloc(n); ridx1.alloc(n);
     gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(engine_stream()); gp0.alloc(n); gp1.alloc(n); err.alloc(1); dsum.alloc(4);
     root_h_cache.alloc(slot_stride);
-    tl0.alloc(tw == 4 ? n : 0); tl1.alloc(tw == 4 ? n : 0);
+    tl0.alloc(tail_pos ? n : 0); tl1.alloc(tail_pos ? n : 0);
     const unsigned max_tiles = (unsigned)((n + kPartTile - 1) / kPartTile) + max_level_nodes + 1;
     scratch.alloc(3 * (size_t)max_level_nodes + 8);
     // ---- GrowState block
@@ -379,6 +384,9 @@ struct GrowerImpl {
     }
   }
 };
+
+// a 4-wide tail rides with the row ids through the partition unless the aligned row copy already holds it
+static bool tail_by_position(const BinnedMatrix& bm) { return bm.tw == 4 && !bm.tail_in_gather; }
 
 // ranks must agree on the fixed-point grid: it follows the GLOBAL row count of the job (GrowerImpl::global_n, all-reduced
 // once), so that N ranks and one GPU train bit-identical models on the same data
@@ -695,7 +703,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   const int K = param_.num_class;
   if (!grower_) grower_ = new GrowerImpl();
   GrowerImpl& g = *grower_;
-  g.ensure(dtrain->n, dtrain->ngroups, dtrain->tw, param_.max_depth, K, lossguide_iters(param_));
+  g.ensure(dtrain->n, dtrain->ngroups, dtrain->tw, tail_by_position(dtrain->binned_view()), param_.max_depth, K, lossguide_iters(param_));
   if (!labels_checked_) {
     // label-range errors must surface from update() (the container maps them to UserError, train.py:461-467)
     const std::vector<float>& y = dtrain->labels;
@@ -744,8 +752,18 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
   if (root_mode == 2) { slot_from_cache_kernel<<<num_sms, 256, 0, s>>>(g.hist_pool.p, g.root_h_cache.p, g.slot_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
   else CUDA_OK(cudaMemsetAsync(g.hist_pool.p, 0, g.slot_stride * sizeof(GH64), s));
 
+  // What travels with the row ids through the partition: g alone when the hessian is constant (h == 1 for every row, the
+  // histograms add the constant h_q), else (g,h); plus the 4 tail bytes when the aligned row copy does not hold them.
+  const bool g_only = root_mode != 0;
+  const bool carry_tail = tail_by_position(bm);
+  if (profile_) {                                  // partition byte model per row (microbench/partition_profile.py)
+    prof_part_row_bytes_[0] = 8 + (carry_tail ? 4 : 0) + 1;                        // root level: the float2 gpair, tail, split byte
+    prof_part_row_bytes_[2] = 4 + (g_only ? 4 : 8) + (carry_tail ? 4 : 0);         // written: id + payload
+    prof_part_row_bytes_[1] = prof_part_row_bytes_[2] + 1;                         // deeper levels: id + payload + split byte
+  }
+
   HistArgs ha{}; ha.bins = bm.bins; ha.bins_tail = bm.bins_tail; ha.n = bm.n; ha.row_stride = bm.ngroups * kSlots; ha.tw = bm.tw;
-  ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride;
+  ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride; ha.tail_in_gather = bm.tail_in_gather;
   ha.gpair = g.gpair.p + (size_t)k * g.gp_stride; ha.ridx = nullptr;
   ha.build_count = g.gs.build_count; ha.build_nid = g.gs.build_nid; ha.build_prefix = g.gs.build_prefix; ha.seg_begin = g.gs.seg_begin;
   ha.hist_slot = g.gs.hist_slot; ha.scales = g.gs.scales; ha.hist_pool = g.hist_pool.p; ha.node_sum = g.gs.node_sum; ha.ngroups = bm.ngroups;
@@ -799,10 +817,10 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     if (ic_on) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = (int)interaction_.size(); aa.F = bm.F; }
     launch_apply_lossguide(aa, it, s);
     // live row segments always sit in buffer set 0; the partition writes the children into set 1 and they are copied straight back
-    const bool carry_tail = bm.tw == 4;
     PartArgs pa{}; pa.gs = g.gs; pa.tree = g.ta; pa.bins_col = bm.bins_col; pa.n = bm.n;
     pa.ridx_cur = it == 0 ? nullptr : g.ridx0.p; pa.ridx_next = g.ridx1.p;
-    pa.gp_cur = it == 0 ? g.gpair.p + (size_t)k * g.gp_stride : g.gp0.p; pa.gp_next = g.gp1.p;
+    pa.gp_cur = it == 0 ? static_cast<const void*>(g.gpair.p + (size_t)k * g.gp_stride) : g.gp0.p; pa.gp_next = g.gp1.p;
+    pa.gp_cur_stride = it == 0 ? 2 : 1; pa.g_only = g_only ? 1 : 0;
     pa.tl_cur = !carry_tail ? nullptr : (it == 0 ? reinterpret_cast<const unsigned*>(bm.bins_tail) : g.tl0.p); pa.tl_next = !carry_tail ? nullptr : g.tl1.p;
     pa.has_missing = bm.has_missing; pa.level = 0; pa.max_level_nodes = g.max_level_nodes; pa.rows_counter = profile_ ? prof_rows_.p + 2 : nullptr;
     prof_begin(kProfPartition);
@@ -810,7 +828,8 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     prof_end();
     launch_lg_copy_back(pa, g.ridx0.p, g.gp0.p, g.tl0.p, max_tiles, s);
     launch_zero_build_slots(g.gs, g.hist_pool.p, g.slot_stride, 1, s);
-    ha.ridx = g.ridx0.p; ha.gpair = g.gp0.p; ha.tail_pos = carry_tail ? g.tl0.p : nullptr; ha.accumulate_sum = 0;
+    ha.ridx = g.ridx0.p; ha.tail_pos = carry_tail ? g.tl0.p : nullptr; ha.accumulate_sum = 0;
+    ha.gpair = g_only ? nullptr : g.gp0.p; ha.gpos = g_only ? reinterpret_cast<const float*>(g.gp0.p) : nullptr;
     ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
     prof_begin(kProfDeepHist);
     launch_hist_build(ha, num_sms, s);
@@ -838,7 +857,7 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     pa.ridx_next = (L & 1) ? g.ridx1.p : g.ridx0.p;
     pa.gp_cur = L == 0 ? g.gpair.p + (size_t)k * g.gp_stride : ((L & 1) ? g.gp0.p : g.gp1.p);
     pa.gp_next = (L & 1) ? g.gp1.p : g.gp0.p;
-    const bool carry_tail = bm.tw == 4;                     // the 4 tail bytes of a row ride along with its id instead of being gathered
+    pa.gp_cur_stride = L == 0 ? 2 : 1; pa.g_only = g_only ? 1 : 0;
     pa.tl_cur = !carry_tail ? nullptr : (L == 0 ? reinterpret_cast<const unsigned*>(bm.bins_tail) : ((L & 1) ? g.tl0.p : g.tl1.p));
     pa.tl_next = !carry_tail ? nullptr : ((L & 1) ? g.tl1.p : g.tl0.p);
     pa.has_missing = bm.has_missing; pa.level = L; pa.max_level_nodes = g.max_level_nodes;
@@ -849,7 +868,8 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     prof_end();
     // histograms of the next level: build the smaller children, all-reduce, subtract for the siblings
     CUDA_OK(cudaMemsetAsync(g.hist_pool.p + (size_t)next_base * g.slot_stride, 0, (size_t)next_half * g.slot_stride * sizeof(GH64), s));
-    ha.ridx = pa.ridx_next; ha.gpair = pa.gp_next; ha.tail_pos = pa.tl_next; ha.accumulate_sum = 0;
+    ha.ridx = pa.ridx_next; ha.tail_pos = pa.tl_next; ha.accumulate_sum = 0;
+    ha.gpair = g_only ? nullptr : static_cast<const float2*>(pa.gp_next); ha.gpos = g_only ? static_cast<const float*>(pa.gp_next) : nullptr;
     ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
     prof_begin(kProfDeepHist);
     launch_hist_build(ha, num_sms, s);
@@ -1151,7 +1171,7 @@ void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::v
   dm->ensure_binned(param_.max_bin);
   if (!grower_) grower_ = new GrowerImpl();
   GrowerImpl& g = *grower_;
-  g.ensure(dm->n, dm->ngroups, dm->tw, param_.max_depth, param_.num_class, lossguide_iters(param_));
+  g.ensure(dm->n, dm->ngroups, dm->tw, tail_by_position(dm->binned_view()), param_.max_depth, param_.num_class, lossguide_iters(param_));
   hist_configure();
   const int64_t rows = row_ids ? n_ids : dm->n;
   B200_CHECK(rows <= dm->n, "debug_build_root_hist: more row ids than rows");
@@ -1167,10 +1187,19 @@ void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::v
   HistArgs ha{}; ha.bins = bm.bins; ha.bins_tail = bm.bins_tail; ha.n = bm.n; ha.row_stride = bm.ngroups * kSlots; ha.tw = bm.tw; ha.gpair = g.gpair.p;
   ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride;
   ha.ridx = row_ids ? g.ridx0.p : nullptr;
+  if (mode & 8) {                               // G-only payload: g alone by position, h == 1.0f for every row (the supplied h is ignored)
+    std::vector<float> gh((size_t)rows);
+    for (int64_t i = 0; i < rows; ++i) gh[i] = gpair_host[2 * i];
+    float* gpos = reinterpret_cast<float*>(g.gp0.p);
+    if (rows) CUDA_OK(cudaMemcpyAsync(gpos, gh.data(), sizeof(float) * rows, cudaMemcpyHostToDevice, s));
+    Comm::get().sync_stream(s);
+    ha.gpos = gpos; ha.gpair = nullptr;
+  }
   ha.build_count = g.gs.build_count; ha.build_nid = g.gs.build_nid; ha.build_prefix = g.gs.build_prefix; ha.seg_begin = g.gs.seg_begin;
   ha.hist_slot = g.gs.hist_slot; ha.scales = g.gs.scales; ha.hist_pool = g.hist_pool.p; ha.node_sum = g.gs.node_sum; ha.ngroups = bm.ngroups; ha.accumulate_sum = 1;
   ha.force_gather = (mode & 3) == 1 ? 1 : 0; ha.g_only = (mode & 3) == 2 ? 1 : 0; ha.window_rows = job_window_rows(g.global_n);
-  if ((mode & 4) && row_ids && bm.tw == 4) {      // the training path's variant: the rows' tail words by POSITION (as after a partition)
+  ha.tail_in_gather = bm.tail_in_gather;          // gathered passes on the aligned copy always read the tail from the row's line
+  if ((mode & 4) && row_ids && tail_by_position(bm)) {     // the training path's variant: the rows' tail words by POSITION (as after a partition)
     gather_u32_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(reinterpret_cast<const unsigned*>(bm.bins_tail), g.ridx0.p, g.tl0.p, rows); ++g_kernel_launches;
     CUDA_OK(cudaGetLastError());
     ha.tail_pos = g.tl0.p;
@@ -1309,9 +1338,11 @@ std::string Booster::get_profile() {
   if (prof_rows_.p) CUDA_OK(cudaMemcpy(rows, prof_rows_.p, sizeof rows, cudaMemcpyDeviceToHost));
   char buf[1024];
   snprintf(buf, sizeof buf, "{\"root_hist_ms\":%.6f,\"root_hist_launches\":%lld,\"root_hist_rows\":%llu,\"deep_hist_ms\":%.6f,\"deep_hist_launches\":%lld,\"deep_hist_rows\":%llu,"
-           "\"part_ms\":%.6f,\"part_launches\":%lld,\"part_rows\":%llu,\"part_rows_written\":%llu,\"margin_ms\":%.6f,\"margin_launches\":%lld,\"margin_rows\":%lld}",
+           "\"part_ms\":%.6f,\"part_launches\":%lld,\"part_rows\":%llu,\"part_rows_written\":%llu,"
+           "\"part_row_bytes_in_root\":%d,\"part_row_bytes_in\":%d,\"part_row_bytes_out\":%d,\"margin_ms\":%.6f,\"margin_launches\":%lld,\"margin_rows\":%lld}",
            ms[kProfRootHist], launches[kProfRootHist], rows[0], ms[kProfDeepHist], launches[kProfDeepHist], rows[1],
-           ms[kProfPartition], launches[kProfPartition], rows[2], rows[3], ms[kProfMargin], launches[kProfMargin], prof_margin_rows_);
+           ms[kProfPartition], launches[kProfPartition], rows[2], rows[3], prof_part_row_bytes_[0], prof_part_row_bytes_[1], prof_part_row_bytes_[2],
+           ms[kProfMargin], launches[kProfMargin], prof_margin_rows_);
   return buf;
 }
 

@@ -52,7 +52,7 @@ class DMatrix {
   void ensure_binned(int max_bin);
   void set_cuts(const HostCuts& c);                   // external cuts (shared with the oracle in tests)
   BinnedMatrix binned_view() const { BinnedMatrix b; b.bins = bins.p; b.bins_tail = tw ? bins_tail.p : nullptr; b.bins_col = bins_col.p; b.n = n; b.F = F;
-    b.bins_gather = bins_gather.p ? bins_gather.p : bins.p; b.gather_stride = gather_stride;
+    b.bins_gather = bins_gather.p ? bins_gather.p : bins.p; b.gather_stride = gather_stride; b.tail_in_gather = bins_gather.p && tw == 8 ? 1 : 0;
     b.ngroups = ngroups; b.tw = tw; b.ntail = ntail; b.has_missing = has_missing; return b; }
   void finish_upload(float missing);
  private:
@@ -119,7 +119,8 @@ class Booster {
   void set_profile(bool on);
   std::string get_profile();                      // JSON, see include/b200xgb.h
   // histogram of one node for kernel-level parity tests / the roofline bench
-  // mode: 0 = production choice (TMA root kernel), 1 = gather kernel, 2 = G-only TMA root kernel (H plane stays zero).
+  // mode: 0 = production choice (TMA root kernel), 1 = gather kernel, 2 = G-only TMA root kernel (H plane stays zero);
+  // + 4 = the training path's tail source, + 8 = G-only payload (g by position, h == 1.0f for every row).
   // row_ids (optional, n_ids entries): histogram of that row subset, gpair given by POSITION -> exercises the gathered path.
   void debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::vector<long long>* hist_out, float* scales_out,
                              int repeats, float* ms_out, int mode = 0, const unsigned* row_ids = nullptr, int64_t n_ids = 0);
@@ -155,6 +156,9 @@ class Booster {
   // [3] rows the partition wrote
   DevBuf<unsigned long long> prof_rows_;
   long long prof_margin_rows_ = 0;
+  // partition byte model per row of the last profiled tree: [0] read at the root level (no row id), [1] read at deeper levels,
+  // [2] written (row id + gradient payload + tail bytes when they travel with the ids)
+  int prof_part_row_bytes_[3] = {0, 0, 0};
 
   void configure();
   float base_margin() const;

@@ -67,6 +67,7 @@ struct BinnedMatrix {
   const uint8_t* bins_col = nullptr;
   const uint8_t* bins_gather = nullptr;   // main block with rows padded to whole 128 B lines when ngroups * 32 == 96 (else == bins)
   int gather_stride = 0;                  // DRAM serves gathered rows in whole 128 B lines: an aligned 96 B row costs one, a packed one 1.5
+  int tail_in_gather = 0;                 // the aligned copy also holds each row's 8 tail bytes (tw == 8), at offset ngroups * 32 (in the pad)
   int64_t n = 0;
   int F = 0, ngroups = 0, tw = 0, ntail = 0;
   int has_missing = 0;

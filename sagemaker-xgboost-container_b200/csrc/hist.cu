@@ -18,7 +18,8 @@
 //                          accumulated (1 atomic per update instead of 2).
 //      hist_gather_kernel  the deeper levels: rows gathered by row id (LDG.128 per 16 B chunk straight to registers, a
 //                          rolling one-super-tile-ahead prefetch), (g,h) read by POSITION (they travel with the row
-//                          ids through the partition).
+//                          ids through the partition; g alone for constant-hessian objectives, whose h_q is a constant),
+//                          tail bytes from the pad of the row's line-aligned copy where there is one.
 //  * Gradients are rounded to a power-of-two fixed-point grid (|g_q| <= 2^18, h_q <= 2^19) so a window of 8064 rows per
 //    CTA cannot overflow int32; between windows, accumulators above 2^24 are spilled to the global int64 histogram with
 //    RED.ADD.64 (sparse), and everything is flushed at the end of the CTA's portion.  Sums are exact integers =>
@@ -477,8 +478,9 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
 // ---------------------------------------------------------------------------------------------
 // Deeper levels (and the fallback for the root): rows gathered by row id, register-staged.
 // ---------------------------------------------------------------------------------------------
-template <int TW> struct Stage { unsigned id; float2 gh; unsigned t0; };
-template <> struct Stage<8> { unsigned id; float2 gh; unsigned t0, t1; };
+// one position per lane: row id, gradients (g alone with a G-only payload, else (g,h)) and the tail words
+template <int TW, bool GPAY> struct Stage { unsigned id; typename std::conditional<GPAY, float, float2>::type gr; unsigned t0; };
+template <bool GPAY> struct Stage<8, GPAY> { unsigned id; typename std::conditional<GPAY, float, float2>::type gr; unsigned t0, t1; };
 
 // tail planes [bin][trep][tw] of the gather kernel: 32 KB (G + H, trep * tw = 16) fit next to three groups, 64 KB otherwise
 __host__ __device__ constexpr int gather_tail_replicas(int ng) { return ng >= 3 ? 4 : 8; }
@@ -489,7 +491,9 @@ __host__ __device__ constexpr int gather_tail_bytes(int ng) { return ng >= 3 ? 3
 // cost ~2.6 bursts), i.e. 16 / 8 / 5 rows per instruction for NG = 1 / 2 / 3 (NG = 3 leaves lanes 30, 31 idle).  Lane (row q,
 // chunk c) owns group c >> 1, half c & 1 and the slot rotation NG * q + (c >> 1): the <= 16 lanes that share a half have
 // distinct rotations, so every ATOMS instruction is still bank-conflict free.
-template <int NG, int TW, int NTHREADS>       // TW: tail width this instantiation handles (0 = none, 4, 8)
+// GPAY (constant-hessian objectives): g alone by position from a.gpos; every valid row adds the constant h_q = rint(1.0f * sh)
+// to the H plane, which is what the (g,h) path computes from h == 1.0f, so both planes come out bit-identical.
+template <int NG, int TW, int NTHREADS, bool GPAY>       // TW: tail width this instantiation handles (0 = none, 4, 8)
 __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gather_kernel(HistArgs a) {
   constexpr bool TAIL = TW != 0;
   constexpr int NWARPS = NTHREADS / 32;
@@ -520,6 +524,10 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
   const unsigned smem_g = (unsigned)__cvta_generic_to_shared(smem);
   // gathered passes read the line-aligned copy of the rows; the contiguous pass (ridx == nullptr) the packed one
   const bool aligned = a.ridx != nullptr && a.bins_gather != nullptr;
+  // tail bytes in the pad of the row's own aligned line: only 3 groups + an 8-wide tail have that layout, and the code must
+  // not cost the other instantiations registers
+  constexpr bool kLineTail = NG == 3 && TW == 8;
+  const bool tail_line = kLineTail && aligned && a.tail_in_gather;
   const int64_t row_stride = aligned ? (int64_t)a.gather_stride : (int64_t)a.row_stride;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int q = lane / LPR, c = lane - q * LPR;                            // row inside a unit, 16 B chunk inside the row
@@ -543,7 +551,8 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
   { int lo = 0, hi = nb; while (lo < hi) { int mid = (lo + hi) >> 1; if (a.build_prefix[mid + 1] > r0) hi = mid; else lo = mid + 1; } b = lo; }
 
   const size_t slot_entries = (size_t)a.ngroups * kGroupEntries + (size_t)256 * a.tw;
-  typedef Stage<TW> StageT;
+  typedef Stage<TW, GPAY> StageT;
+  const unsigned hq_one = (unsigned)__float2int_rn(1.0f * sh);              // GPAY: h_q of every row
   while (r0 < r1) {
     const unsigned nbeg = a.build_prefix[b], nend_node = a.build_prefix[b + 1];
     const unsigned nend = nend_node < r1 ? nend_node : r1;
@@ -558,17 +567,20 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
     const unsigned iters = (nsuper + NWARPS - 1) / NWARPS;          // same for every warp: barriers stay aligned
 
     // Software pipeline per warp over super-tiles of SUP positions; it runs THROUGH the overflow-check barriers:
-    //   row ids + (g,h) + tail bytes two super-tiles ahead (coalesced, one position per lane);
+    //   row ids + gradients + tail bytes two super-tiles ahead (coalesced, one position per lane);
     //   bin chunks (one LDG.128 per lane and unit) one super-tile ahead, ROLLING: the register of unit k is refilled with
-    //   unit k of the next super-tile right after it has been consumed (U loads in flight per lane at all times);
+    //   unit k of the next super-tile right after it has been consumed (U loads in flight per lane at all times); on the
+    //   aligned copy the tail bytes are requested right behind the bin chunks of the same lines (a request of its own two
+    //   super-tiles earlier would fetch every line twice, and hang a dependent gather on the row-id load);
     //   conflict-free ATOMS pairs now.
     auto load_ids = [&](unsigned st) -> StageT {
-      StageT s_; s_.id = 0xffffffffu; s_.gh = make_float2(0.f, 0.f); s_.t0 = 0u;
+      StageT s_; s_.id = 0xffffffffu; s_.gr = {}; s_.t0 = 0u;
       if constexpr (TW == 8) s_.t1 = 0u;
       unsigned p = pa + st * SUP + lane;
       if (lane < SUP && st < nsuper && p < pb) {
-        s_.id = a.ridx ? __ldg(a.ridx + p) : p; s_.gh = ldg_nc_f2(a.gpair + p);
-        if (TAIL && has_tail) {
+        s_.id = a.ridx ? __ldg(a.ridx + p) : p;
+        if constexpr (GPAY) s_.gr = __uint_as_float(ldg_nc_u32(a.gpos + p)); else s_.gr = ldg_nc_f2(a.gpair + p);
+        if (TAIL && has_tail && !tail_line) {
           if constexpr (TW == 8) { const uint2 v = ldg_nc_v2(a.bins_tail + (int64_t)s_.id * 8); s_.t0 = v.x; s_.t1 = v.y; }
           else if (a.tail_pos) s_.t0 = ldg_nc_u32(a.tail_pos + p);                  // tail bytes travel with the row ids (tw == 4)
           else s_.t0 = ldg_nc_u32(a.bins_tail + (int64_t)s_.id * 4);
@@ -580,17 +592,27 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
       const unsigned rid = __shfl_sync(0xffffffffu, ids, q < RPI ? k * RPI + q : 0);
       return (lane_on && rid != 0xffffffffu) ? ldg_nc_v4(gbins + (int64_t)rid * row_stride) : make_uint4(0, 0, 0, 0);
     };
+    auto load_line_tail = [&](StageT& s_) {
+      if constexpr (TAIL) {
+        if (tail_line && has_tail && s_.id != 0xffffffffu) {
+          const uint8_t* t = a.bins_gather + (int64_t)s_.id * row_stride + a.ngroups * kSlots;
+          if constexpr (TW == 8) { const uint2 v = ldg_nc_v2(t); s_.t0 = v.x; s_.t1 = v.y; } else s_.t0 = ldg_nc_u32(t);
+        }
+      }
+    };
     StageT cur = load_ids(warp);
     StageT nxt = load_ids(warp + NWARPS);
     uint4 w[U];
 #pragma unroll
     for (int k = 0; k < U; ++k) w[k] = load_unit(cur.id, k);
+    load_line_tail(cur);
     for (unsigned it = 0; it < iters; ++it) {
       const unsigned s = warp + it * NWARPS;
       StageT nn = load_ids(s + 2 * NWARPS);
       const bool active = s < nsuper;
-      const int gq_l = __float2int_rn(cur.gh.x * sg);
-      const unsigned hq_l = (unsigned)__float2int_rn(cur.gh.y * sh);
+      int gq_l; unsigned hq_l;
+      if constexpr (GPAY) { gq_l = __float2int_rn(cur.gr * sg); hq_l = cur.id != 0xffffffffu ? hq_one : 0u; }      // no row: adds nothing
+      else { gq_l = __float2int_rn(cur.gr.x * sg); hq_l = (unsigned)__float2int_rn(cur.gr.y * sh); }
       accG += gq_l; accH += hq_l;
 #pragma unroll
       for (int k = 0; k < U; ++k) {
@@ -605,6 +627,7 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
         w[k] = load_unit(nxt.id, k);
       }
       if constexpr (TAIL) { if (active && has_tail) { unsigned t1 = 0; if constexpr (TW == 8) t1 = cur.t1; tail_accumulate_ct<TWC, trep>(tail_base_rep, lane, cur.t0, t1, gq_l, hq_l); } }
+      load_line_tail(nxt);
       cur = nxt; nxt = nn;
       if ((it + 1) % iters_per_window == 0 && it + 1 < iters) {       // overflow check: at most kWindowRows rows since the last one
         if (a.accumulate_sum && blockIdx.y == 0) { flush_node_sum(a.node_sum + nid, accG, accH, lane); accG = 0; accH = 0; }
@@ -695,7 +718,9 @@ static bool get_tensor_map(const uint8_t* bins, int64_t n, int row_stride, int b
 }
 
 template <int NG, int TW, int NT> static void set_gather_attr() {
-  CUDA_OK(cudaFuncSetAttribute(hist_gather_kernel<NG, TW, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, NG * 2 * kPlaneBytes + (TW ? gather_tail_bytes(NG) : 0)));
+  const int smem = NG * 2 * kPlaneBytes + (TW ? gather_tail_bytes(NG) : 0);
+  CUDA_OK(cudaFuncSetAttribute(hist_gather_kernel<NG, TW, NT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  CUDA_OK(cudaFuncSetAttribute(hist_gather_kernel<NG, TW, NT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
 }
 
 void hist_configure() {
@@ -709,12 +734,16 @@ void hist_configure() {
   configured = true;
 }
 
+template <int NG, int NT, bool GPAY>
+static void launch_gather_tw(const HistArgs& a, int gx, int nchunks, cudaStream_t stream) {
+  const int smem = NG * 2 * kPlaneBytes + (a.tw ? gather_tail_bytes(NG) : 0);
+  if (a.tw == 0) hist_gather_kernel<NG, 0, NT, GPAY><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
+  else if (a.tw == 4) hist_gather_kernel<NG, 4, NT, GPAY><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
+  else hist_gather_kernel<NG, 8, NT, GPAY><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
+}
 template <int NG, int NT>
 static void launch_gather(const HistArgs& a, int gx, int nchunks, cudaStream_t stream) {
-  const int smem = NG * 2 * kPlaneBytes + (a.tw ? gather_tail_bytes(NG) : 0);
-  if (a.tw == 0) hist_gather_kernel<NG, 0, NT><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
-  else if (a.tw == 4) hist_gather_kernel<NG, 4, NT><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
-  else hist_gather_kernel<NG, 8, NT><<<dim3(gx, nchunks), NT, smem, stream>>>(a);
+  if (a.gpos) launch_gather_tw<NG, NT, true>(a, gx, nchunks, stream); else launch_gather_tw<NG, NT, false>(a, gx, nchunks, stream);
 }
 
 void launch_hist_build(const HistArgs& a_in, int num_sms, cudaStream_t stream) {
@@ -722,7 +751,7 @@ void launch_hist_build(const HistArgs& a_in, int num_sms, cudaStream_t stream) {
   const int nchunks = chunks_for(a.ngroups);
   a.ng_chunk = groups_per_chunk(a.ngroups);
   static const bool no_tma = getenv("B200XGB_NO_TMA") != nullptr;
-  if (a.ridx == nullptr && !no_tma && !a.force_gather) {
+  if (a.ridx == nullptr && !no_tma && !a.force_gather && a.gpos == nullptr) {     // the root kernel streams (g,h) pairs
     RootCfg c; CUtensorMap tm;
     const bool gonly = a.g_only != 0;
     if (root_plan(a.ng_chunk, a.tw, gonly, &c) && get_tensor_map(a.bins, a.n, a.row_stride, c.box_groups, kRootRows, &tm)) {

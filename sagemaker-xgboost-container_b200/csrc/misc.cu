@@ -145,19 +145,25 @@ __global__ void __launch_bounds__(256) bin_kernel(const float* X, int64_t n, int
   }
 }
 
-// rows re-laid at `dst_stride` bytes (whole 128 B lines for 96 B rows): 16 B per thread
-__global__ void __launch_bounds__(256) pad_rows_kernel(const uint8_t* src, int64_t n, int src_stride, uint8_t* dst, int dst_stride) {
+// rows re-laid at `dst_stride` bytes (whole 128 B lines for 96 B rows): 16 B per thread.  The row's tw tail bytes go right
+// behind its main bytes (offset src_stride), the rest of the pad is zero.
+__global__ void __launch_bounds__(256) pad_rows_kernel(const uint8_t* src, const uint8_t* tail, int tw, int64_t n, int src_stride, uint8_t* dst, int dst_stride) {
   const int cpr = dst_stride / 16, spr = src_stride / 16;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n * cpr; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / cpr; const int c = (int)(i - r * cpr);
     uint4 v = make_uint4(0, 0, 0, 0);
     if (c < spr) v = reinterpret_cast<const uint4*>(src + r * src_stride)[c];
+    else if (c == spr && tw > 0) {
+      v.x = reinterpret_cast<const unsigned*>(tail + r * tw)[0];
+      if (tw == 8) v.y = reinterpret_cast<const unsigned*>(tail + r * tw)[1];
+    }
     reinterpret_cast<uint4*>(dst + r * dst_stride)[c] = v;
   }
 }
-void launch_pad_rows(const uint8_t* src, int64_t n, int src_stride, uint8_t* dst, int dst_stride, cudaStream_t s) {
+void launch_pad_rows(const uint8_t* src, const uint8_t* tail, int tw, int64_t n, int src_stride, uint8_t* dst, int dst_stride, cudaStream_t s) {
   if (n == 0) return;
-  pad_rows_kernel<<<engine_num_sms() * 16, 256, 0, s>>>(src, n, src_stride, dst, dst_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  B200_CHECK(tw == 0 || (tw <= dst_stride - src_stride && src_stride % 16 == 0), "pad_rows: the tail does not fit in the row's pad");
+  pad_rows_kernel<<<engine_num_sms() * 16, 256, 0, s>>>(src, tail, tw, n, src_stride, dst, dst_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 
 // column-major copy [F][n] of the binned matrix (used by the 1-byte-per-row consumers: partition, cache update)

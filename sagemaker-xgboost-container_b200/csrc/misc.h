@@ -59,7 +59,7 @@ void launch_gradient(const GradArgs& a, cudaStream_t s);
 void launch_sum_gpair(const float2* gp, int64_t n, double* out, cudaStream_t s);
 void launch_bin(const float* X, int64_t n, int F, int ngroups, int tw, const int* cut_ptrs, const float* cut_vals, uint8_t* bins, uint8_t* bins_tail, cudaStream_t s);
 void launch_transpose_bins(const uint8_t* bins, const uint8_t* bins_tail, int64_t n, int F, int ngroups, int tw, uint8_t* bins_col, cudaStream_t s);
-void launch_pad_rows(const uint8_t* src, int64_t n, int src_stride, uint8_t* dst, int dst_stride, cudaStream_t s);
+void launch_pad_rows(const uint8_t* src, const uint8_t* tail, int tw, int64_t n, int src_stride, uint8_t* dst, int dst_stride, cudaStream_t s);
 void launch_count_nan(const float* X, int64_t count, float missing, int use_missing, unsigned long long* out, cudaStream_t s);
 void launch_replace_missing(float* X, int64_t count, float missing, cudaStream_t s);
 void launch_predict(const PredictArgs& a, cudaStream_t s);

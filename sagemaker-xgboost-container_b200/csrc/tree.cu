@@ -2,6 +2,7 @@
 // depth-wise hist tree builder (SURVEY.md section 8a rows A9, A10, A11).  Mirrors the behaviour of upstream
 // xgboost's src/tree/hist/evaluate_splits.h, src/tree/driver.h, src/tree/updater_quantile_hist.cc and
 // src/common/partition_builder.h as restated in oracle/gbt_oracle.c; all control flow stays on the device.
+#include <type_traits>
 #include "engine.h"
 #include "tree.h"
 
@@ -463,13 +464,15 @@ __global__ void __launch_bounds__(256) apply_lossguide_kernel(ApplyArgs a, int i
 }
 
 // lossguide keeps every live row segment in ONE buffer set: the children written by the partition go straight back
-__global__ void __launch_bounds__(256) lg_copy_back_kernel(PartArgs a, unsigned* ridx_dst, float2* gp_dst, unsigned* tl_dst) {
+template <typename Pay>       // the partition's payload: float2 (g,h) or float g
+__global__ void __launch_bounds__(256) lg_copy_back_kernel(PartArgs a, unsigned* ridx_dst, Pay* gp_dst, unsigned* tl_dst) {
   const GrowState& gs = a.gs;
   if (gs.level_count[0] <= 0 || !gs.part_action[0]) return;
   const int nid = gs.level_nodes[0];
   const unsigned b = gs.seg_begin[nid], c = gs.seg_count[nid];
+  const Pay* gp_src = static_cast<const Pay*>(a.gp_next);
   for (unsigned p = b + blockIdx.x * blockDim.x + threadIdx.x; p < b + c; p += gridDim.x * blockDim.x) {
-    ridx_dst[p] = a.ridx_next[p]; gp_dst[p] = a.gp_next[p];
+    ridx_dst[p] = a.ridx_next[p]; gp_dst[p] = gp_src[p];
     if (a.tl_next) tl_dst[p] = a.tl_next[p];
   }
 }
@@ -536,14 +539,19 @@ __device__ unsigned lookback_lefts(const unsigned long long* d, unsigned lt) {
   return acc;
 }
 
-// One CTA per tile, taken from an atomic ticket.  Per tile: ids, (g,h), tail word and the split byte in; the left count
-// published; the tile compacted in shared memory ([lefts | rights], position order) while warp 0 looks back; 16 B per row out.
+// One CTA per tile, taken from an atomic ticket.  Per tile: ids, payload and the split byte in; the left count published; the
+// tile compacted in shared memory ([lefts | rights], position order) while warp 0 looks back; id + payload per row out.
 // The node's last tile writes the children's segments; the last CTA of the grid computes the build list's prefix.
-__global__ void __launch_bounds__(256) part_kernel(PartArgs a) {
+// Payload: GONLY (constant hessian) carries g alone, else (g,h); TL adds the row's 4 tail bytes.  8, 12 or 16 B per row out.
+// The tile is latency bound (a dependent split-byte gather per row): the G-only variants fit 6 / 5 CTAs per SM in 40 / 48
+// registers without spilling, and each CTA more per SM measured faster; the (g,h) variants keep 4 (64 registers).
+template <bool GONLY, bool TL>
+__global__ void __launch_bounds__(256, GONLY ? (TL ? 5 : 6) : 4) part_kernel(PartArgs a) {
+  typedef typename std::conditional<GONLY, float, float2>::type Pay;
   GrowState& gs = a.gs;
   __shared__ unsigned s_rid[kPartTile];
-  __shared__ float2 s_gp[kPartTile];
-  __shared__ unsigned s_tl[kPartTile];
+  __shared__ Pay s_gp[kPartTile];
+  __shared__ unsigned s_tl[TL ? kPartTile : 1];
   __shared__ unsigned s_w[8];
   const int cnt = gs.level_count[a.level];
   const unsigned total = cnt > 0 ? gs.tile_prefix[cnt] : 0u;
@@ -561,14 +569,20 @@ __global__ void __launch_bounds__(256) part_kernel(PartArgs a) {
     const int f = a.tree.split_index[nid];
     const int sb = a.tree.split_bin[nid], dl = a.tree.default_left[nid];
     const uint8_t* col = a.bins_col + (int64_t)f * a.n;        // column-major copy: one byte per row
-    const bool has_tl = a.tl_cur != nullptr;
+    const Pay* gp_cur = static_cast<const Pay*>(a.gp_cur);
+    Pay* gp_next = static_cast<Pay*>(a.gp_next);
     const unsigned pt = p0 + threadIdx.x * 8;
-    unsigned rows[8]; float2 gp[8]; unsigned tl[8]; unsigned char fl[8]; unsigned mine = 0;
+    unsigned rows[8]; Pay gp[8]; unsigned tl[8]; unsigned char fl[8]; unsigned mine = 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const unsigned p = pt + j;
-      if (p < p1) { rows[j] = a.ridx_cur ? a.ridx_cur[p] : p; gp[j] = a.gp_cur[p]; tl[j] = has_tl ? a.tl_cur[p] : 0u; }
-      else { rows[j] = 0; gp[j] = make_float2(0.f, 0.f); tl[j] = 0u; }
+      rows[j] = 0; gp[j] = Pay{}; tl[j] = 0u;
+      if (p < p1) {
+        rows[j] = a.ridx_cur ? a.ridx_cur[p] : p;
+        if constexpr (GONLY) gp[j] = static_cast<const float*>(a.gp_cur)[(size_t)p * a.gp_cur_stride];
+        else gp[j] = gp_cur[p];
+        if constexpr (TL) tl[j] = a.tl_cur[p];
+      }
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -594,7 +608,7 @@ __global__ void __launch_bounds__(256) part_kernel(PartArgs a) {
       if (fl[j] == 2) continue;
       const unsigned jj = threadIdx.x * 8 + j;
       const unsigned slot = fl[j] ? lbefore++ : tile_left + (jj - lbefore);
-      s_rid[slot] = rows[j]; s_gp[slot] = gp[j]; if (has_tl) s_tl[slot] = tl[j];
+      s_rid[slot] = rows[j]; s_gp[slot] = gp[j]; if constexpr (TL) s_tl[slot] = tl[j];
     }
     unsigned lefts_before = 0;
     if (warp == 0 && lt > 0) {
@@ -615,8 +629,8 @@ __global__ void __launch_bounds__(256) part_kernel(PartArgs a) {
     for (unsigned k = k0 + threadIdx.x; k < k1; k += blockDim.x) {
       const unsigned dest = k < tile_left ? dl0 + k : dr0 - k;
       a.ridx_next[dest] = s_rid[k];
-      a.gp_next[dest] = s_gp[k];
-      if (has_tl) a.tl_next[dest] = s_tl[k];
+      gp_next[dest] = s_gp[k];
+      if constexpr (TL) a.tl_next[dest] = s_tl[k];
     }
     if (threadIdx.x == 0) {
       if (lt == gs.tile_prefix[i + 1] - t0 - 1) {       // the node's last tile knows its left total
@@ -719,8 +733,11 @@ void launch_eval(const EvalArgs& a, int max_nodes_level, cudaStream_t s) {
   dim3 grid(max_nodes_level, a.ngroups + (a.tw > 0 ? 1 : 0)); eval_kernel<<<grid, 32 * kEvalSegs, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_apply_lossguide(const ApplyArgs& a, int iter, cudaStream_t s) { apply_lossguide_kernel<<<1, 256, 0, s>>>(a, iter); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
-void launch_lg_copy_back(const PartArgs& a, unsigned* ridx_dst, float2* gp_dst, unsigned* tl_dst, unsigned max_tiles, cudaStream_t s) {
-  lg_copy_back_kernel<<<max_tiles < 1184u ? max_tiles : 1184u, 256, 0, s>>>(a, ridx_dst, gp_dst, tl_dst); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+void launch_lg_copy_back(const PartArgs& a, unsigned* ridx_dst, void* gp_dst, unsigned* tl_dst, unsigned max_tiles, cudaStream_t s) {
+  const unsigned grid = max_tiles < 1184u ? max_tiles : 1184u;
+  if (a.g_only) lg_copy_back_kernel<float><<<grid, 256, 0, s>>>(a, ridx_dst, static_cast<float*>(gp_dst), tl_dst);
+  else lg_copy_back_kernel<float2><<<grid, 256, 0, s>>>(a, ridx_dst, static_cast<float2*>(gp_dst), tl_dst);
+  ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_zero_build_slots(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s) {
   dim3 grid(max_build, (unsigned)((slot_entries + 1023) / 1024)); zero_build_slots_kernel<<<grid, 256, 0, s>>>(gs, pool, slot_entries); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
@@ -731,7 +748,10 @@ void launch_lg_stage(const GrowState& gs, GH64* pool, size_t slot_entries, int t
 void launch_apply(const ApplyArgs& a, cudaStream_t s) { apply_kernel<<<1, 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
 void launch_partition(const PartArgs& a, unsigned max_tiles, cudaStream_t s) {
   CUDA_OK(cudaMemsetAsync(a.gs.tile_desc, 0, sizeof(unsigned long long) * ((size_t)max_tiles + 1), s));   // descriptors + part_ctl
-  part_kernel<<<max_tiles, 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  const bool tl = a.tl_cur != nullptr;
+  if (a.g_only) { if (tl) part_kernel<true, true><<<max_tiles, 256, 0, s>>>(a); else part_kernel<true, false><<<max_tiles, 256, 0, s>>>(a); }
+  else { if (tl) part_kernel<false, true><<<max_tiles, 256, 0, s>>>(a); else part_kernel<false, false><<<max_tiles, 256, 0, s>>>(a); }
+  ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k, cudaStream_t s) {
   if (n == 0) return;

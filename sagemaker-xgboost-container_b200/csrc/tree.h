@@ -30,8 +30,11 @@ struct ApplyArgs {
 
 struct PartArgs {
   GrowState gs; TreeArrays tree; const uint8_t* bins_col; int64_t n; const unsigned* ridx_cur; unsigned* ridx_next;
-  const float2* gp_cur; float2* gp_next;      // (g,h) pairs travel with the row ids (position order)
-  const unsigned* tl_cur; unsigned* tl_next;  // ... and so do the 4 tail bin bytes of a row (nullptr when there is no 4-wide tail)
+  // the gradients travel with the row ids (position order): float2 (g,h) pairs, or with g_only (constant hessian, h == 1 for
+  // every row) float g alone.  gp_cur_stride: floats between two positions' g in gp_cur (2 while it is the float2 gpair of the
+  // root, 1 after); not used without g_only.
+  const void* gp_cur; void* gp_next; int gp_cur_stride; int g_only;
+  const unsigned* tl_cur; unsigned* tl_next;  // ... and so do the 4 tail bin bytes of a row (nullptr: no 4-wide tail, or it is in bins_gather)
   int has_missing, level, max_level_nodes;
   int build_only;                             // write only the child whose histogram is built (its rows are never read again otherwise)
   unsigned long long* rows_counter;           // optional (profiling): [0] += rows of split nodes read, [1] += rows written
@@ -45,8 +48,10 @@ struct HistArgs {
   int row_stride;               // ngroups * 32
   const uint8_t* bins_gather;   // rows for the gathered passes (BinnedMatrix::bins_gather) and their stride
   int gather_stride;
+  int tail_in_gather;           // gathered passes read the tail bytes from the row's own line of bins_gather (tail_pos unused)
   int tw;                       // tail width in bytes (0, 4, 8)
   const float2* gpair;          // (g, h) by POSITION in the row-id buffer (== by row at the root)
+  const float* gpos;            // constant hessian: g alone by POSITION, h == 1.0f for every row (gpair unused); nullptr = gpair
   const unsigned* ridx;         // row ids by segment position; nullptr = identity (root)
   const int* build_count;       // number of nodes to build
   const int* build_nid;         // their node ids
@@ -68,7 +73,7 @@ struct HistArgs {
 // grow_policy=lossguide (one expansion per iteration; tree.cu)
 constexpr int kLgRootSlot = 0, kLgStageSlot = 1, kLgFirstFreeSlot = 2;     // histogram pool slots: root, all-reduce staging, then one per expansion
 void launch_apply_lossguide(const ApplyArgs& a, int iter, cudaStream_t s);
-void launch_lg_copy_back(const PartArgs& a, unsigned* ridx_dst, float2* gp_dst, unsigned* tl_dst, unsigned max_tiles, cudaStream_t s);
+void launch_lg_copy_back(const PartArgs& a, unsigned* ridx_dst, void* gp_dst, unsigned* tl_dst, unsigned max_tiles, cudaStream_t s);
 void launch_zero_build_slots(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s);
 void launch_lg_stage(const GrowState& gs, GH64* pool, size_t slot_entries, int to_stage, cudaStream_t s);
 void launch_hist_build(const HistArgs& a, int num_sms, cudaStream_t stream);
