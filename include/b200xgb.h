@@ -175,6 +175,10 @@ XGB_DLL int XGB200BuildHistogramEx(BoosterHandle handle, DMatrixHandle dmat, con
                              const char** out_kernel);
 /* mean device time (CUDA events) of the predictor kernel alone over `repeats` launches on `dmat` */
 XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dmat, int repeats, float* out_ms);
+/* the predictor's plan for `dmat` and the rounds [iter_begin, iter_end) (iter_end == 0: all), without running it: JSON
+ * {"kernel": "predict_tiled_kernel" | "predict_kernel", "reason" (why thread-per-row), "has_nan", "tree_begin", "tree_end",
+ * "pitch", "chunks": [{"begin","end","node_bytes","rows","threads","smem"}]} (see csrc/predict_plan.h) */
+XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_begin, int iter_end, const char** out_json);
 /* raw margins of the prediction cache the trainer keeps for `dmat` (n x num_class), brought up to date first */
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
 /* CUDA-event stopwatch on the engine's stream: Start records an event, Stop records another, waits, returns ms */

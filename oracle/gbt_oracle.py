@@ -316,13 +316,18 @@ def base_margin_of(model):
 
 
 def predict_margin(model, X, tree_begin=0, tree_end=None, base_margin=None):
+    """fp32 margins (n, K): the leaf values of trees [tree_begin, tree_end) added in tree order to the base margin, a scalar
+    (default: the model's) or per row, (n,) or (n, K) like DMatrix base_margin."""
     X = np.ascontiguousarray(X, np.float32)
     n, F = X.shape
     K = int(model.get("num_class", 1))
     nt = model.num_trees if isinstance(model, Model) else len(model["tree_info"])
     tree_end = nt if tree_end is None else tree_end
     bm = base_margin_of(model) if base_margin is None else base_margin
-    out = np.full((n, K), bm, np.float32)
+    if np.ndim(bm) == 0:
+        out = np.full((n, K), bm, np.float32)
+    else:
+        out = np.array(bm, np.float32).reshape(n, K)
     lib().orc_predict(_p(X), n, F, K, nt, tree_begin, tree_end, _p(model["tree_offset"]), _p(model["tree_info"]),
                       _p(model["left"]), _p(model["right"]), _p(model["split_index"]), _p(model["default_left"]),
                       _p(model["split_cond"]), _p(out), None)

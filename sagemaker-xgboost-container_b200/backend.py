@@ -406,6 +406,12 @@ class CudaBackend:
         self._check(self.lib.XGB200BoosterPredictKernelMs(bh, dh, C.c_int(repeats), C.byref(ms)))
         return float(ms.value)
 
+    def booster_predict_plan(self, bh, dh, iteration_range=(0, 0)):
+        """The predictor's plan for this matrix and rounds, as a dict (include/b200xgb.h XGB200BoosterPredictPlan)."""
+        out = C.c_char_p()
+        self._check(self.lib.XGB200BoosterPredictPlan(bh, dh, C.c_int(iteration_range[0]), C.c_int(iteration_range[1]), C.byref(out)))
+        return json.loads(out.value.decode())
+
     def booster_cached_margin(self, bh, dh, K):
         n = self.dmatrix_num_row(dh)
         out = np.zeros((n, K), np.float32)

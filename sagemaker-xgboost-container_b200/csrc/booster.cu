@@ -677,9 +677,8 @@ void Booster::bring_cache_up_to_date(DMatrix* dm, PredCache& c) {
   }
   if (c.trees_applied < nt) {
     upload_model();
-    PredictArgs pa{}; pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
-    pa.tree_begin = c.trees_applied; pa.tree_end = nt; pa.K = K; pa.margin = c.margin.p; pa.leaf = nullptr;
-    pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
+    PredictArgs pa = predict_args(dm, c.trees_applied, nt);
+    pa.margin = c.margin.p;
     launch_predict(pa, s);
     c.trees_applied = nt;
   }
@@ -1120,9 +1119,7 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
   upload_model();
   const int tb = iter_begin * K, te = iter_end * K;
   const int64_t n = dm->n;
-  PredictArgs pa{}; pa.X = dm->X.p; pa.n = n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
-  pa.tree_begin = tb; pa.tree_end = te; pa.K = K;
-  pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
+  PredictArgs pa = predict_args(dm, tb, te);
   if (type == 6) {
     const int nt = te - tb;
     DevBuf<int>& leaf = pred_leaf_; leaf.ensure((size_t)n * std::max(nt, 1));
@@ -1275,6 +1272,25 @@ void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* 
   if (K > 1) shape->assign({(uint64_t)n, (uint64_t)K, (uint64_t)(F + 1)}); else shape->assign({(uint64_t)n, (uint64_t)(F + 1)});
 }
 
+PredictArgs Booster::predict_args(DMatrix* dm, int tree_begin, int tree_end) {
+  PredictArgs pa{}; pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
+  pa.tree_begin = tree_begin; pa.tree_end = tree_end; pa.K = param_.num_class; pa.margin = nullptr; pa.leaf = nullptr;
+  pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
+  pa.model_F = num_feature_;
+  return pa;
+}
+
+// the plan predict(dm, iteration_range = [iter_begin, iter_end)) executes (iter_end == 0: every round)
+std::string Booster::debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end) {
+  configure();
+  upload_model();
+  const int K = param_.num_class;
+  if (iter_end == 0) iter_end = (int)trees_.size() / K;
+  B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end * K <= (int)trees_.size(), "debug_predict_plan: invalid iteration range");
+  const PredictArgs pa = predict_args(dm, iter_begin * K, iter_end * K);
+  return predict_plan_json(plan_for(pa), pa.tree_begin, pa.tree_end, pa.has_nan != 0);
+}
+
 // device time of the predictor kernel alone (margins of all trees into the scratch buffer), for the roofline line of bench.py
 float Booster::debug_predict_kernel_ms(DMatrix* dm, int repeats) {
   configure();
@@ -1282,9 +1298,8 @@ float Booster::debug_predict_kernel_ms(DMatrix* dm, int repeats) {
   upload_model();
   const int K = param_.num_class;
   pred_margin_.ensure((size_t)dm->n * K);
-  PredictArgs pa{}; pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
-  pa.tree_begin = 0; pa.tree_end = (int)trees_.size(); pa.K = K; pa.margin = pred_margin_.p; pa.leaf = nullptr;
-  pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
+  PredictArgs pa = predict_args(dm, 0, (int)trees_.size());
+  pa.margin = pred_margin_.p;
   cudaEvent_t e0, e1; CUDA_OK(cudaEventCreate(&e0)); CUDA_OK(cudaEventCreate(&e1));
   float total = 0.f;
   for (int r = 0; r < std::max(1, repeats); ++r) {

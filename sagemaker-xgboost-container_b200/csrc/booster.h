@@ -111,6 +111,7 @@ class Booster {
   void sync_model();                              // materialise pending trees on the host
   void cached_margin(DMatrix* dm, std::vector<float>* out);   // the trainer's prediction cache for dm
   float debug_predict_kernel_ms(DMatrix* dm, int repeats);
+  std::string debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end);   // JSON of the plan predict() would run
   const std::vector<HostTree>& trees() { sync_model(); return trees_; }
   const std::vector<int>& tree_info() const { return tree_info_; }
   float base_score() const { return base_score_; }
@@ -127,6 +128,7 @@ class Booster {
 
  private:
   friend struct GrowerImpl;
+  PredictArgs predict_args(DMatrix* dm, int tree_begin, int tree_end);   // the device model on dm (outputs left unset)
   std::map<std::string, std::string> raw_params_;
   std::vector<std::string> eval_metrics_;
   std::vector<int> monotone_;              // parsed monotone_constraints (empty = none)

@@ -519,6 +519,10 @@ int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dmat, int r
   *out_ms = BST(handle)->debug_predict_kernel_ms(DM(dmat), repeats);
   API_END();
 }
+int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_begin, int iter_end, const char** out_json) {
+  API_BEGIN(); BoosterBox* box = static_cast<BoosterBox*>(handle); box->ret_str = BST(handle)->debug_predict_plan(DM(dmat), iter_begin, iter_end);
+  *out_json = box->ret_str.c_str(); API_END();
+}
 int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out) {
   API_BEGIN();
   std::vector<float> v;

@@ -415,58 +415,37 @@ void launch_replace_missing(float* X, int64_t count, float missing, cudaStream_t
   if (count == 0) return;
   replace_missing_kernel<<<grid_for(count), 256, 0, s>>>(X, count, missing); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
-// host-side plan of the tiled predictor: trees are cut into chunks that fit in shared memory next to a row tile
+// the plan (predict_plan.h) of these arguments: B200XGB_PREDICT_LEGACY (read once per process) forces thread-per-row
+PredictPlan plan_for(const PredictArgs& a) {
+  static const bool legacy = getenv("B200XGB_PREDICT_LEGACY") != nullptr;
+  return plan_predict(a.h_tree_offset, a.tree_begin, a.tree_end, a.F, a.model_F, a.children_adjacent != 0, legacy);
+}
+
+// executes plan_for(a): one tiled launch per tree chunk, or the thread-per-row kernel
 void launch_predict(const PredictArgs& a, cudaStream_t s) {
   if (a.n == 0 || a.tree_end <= a.tree_begin) return;
-  static const bool legacy = getenv("B200XGB_PREDICT_LEGACY") != nullptr;
-  const bool ok = !legacy && a.h_tree_offset != nullptr && a.F <= 32767 && a.children_adjacent;
-  const int pitch = a.F | 1;                                       // odd pitch: threads of a warp (rows) hit different banks for the same feature
-  const size_t kSmem = 220 * 1024;
-  if (ok && (size_t)pitch * 4 * 32 + 64 * 1024 <= kSmem) {
+  const PredictPlan plan = plan_for(a);
+  if (plan.kernel == PredictKernel::kTiled) {
     static bool attr = false;
     if (!attr) {
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
+      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
+      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
+      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
       attr = true;
     }
-    const size_t node_budget = 96 * 1024;                          // bytes of packed nodes per chunk
-    int lo = a.tree_begin;
-    bool fits = true;
-    std::vector<std::pair<int, int>> chunks;
-    while (lo < a.tree_end) {
-      int hi = lo; size_t bytes = 0;
-      while (hi < a.tree_end) {
-        const int64_t nn = a.h_tree_offset[hi + 1] - a.h_tree_offset[hi];
-        if (nn > 65534) { fits = false; break; }
-        if (bytes + (size_t)nn * 8 > node_budget && hi > lo) break;
-        if ((size_t)nn * 8 > node_budget) { fits = false; break; }
-        bytes += (size_t)nn * 8; ++hi;
-      }
-      if (!fits) break;
-      chunks.emplace_back(lo, hi); lo = hi;
+    const int pitch = plan.pitch;
+    for (const PredictChunk& ch : plan.chunks) {
+      const int rows = ch.rows, threads = ch.threads;
+      const int64_t tiles = (a.n + rows - 1) / rows;
+      const int grid = (int)std::min<int64_t>(tiles, engine_num_sms() * (threads == 1024 ? 1 : 2048 / threads));
+      if (a.leaf) { if (a.has_nan) predict_tiled_kernel<true, true><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles);
+                    else predict_tiled_kernel<false, true><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles); }
+      else { if (a.has_nan) predict_tiled_kernel<true, false><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles);
+             else predict_tiled_kernel<false, false><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles); }
+      ++g_kernel_launches; CUDA_OK(cudaGetLastError());
     }
-    if (fits) {
-      for (auto& ch : chunks) {
-        size_t node_bytes = 0;
-        for (int t = ch.first; t < ch.second; ++t) node_bytes += (size_t)(a.h_tree_offset[t + 1] - a.h_tree_offset[t]) * 8;
-        const size_t head = (((size_t)(ch.second - ch.first + 1) * 4 + 15) & ~(size_t)15) + node_bytes;
-        int rows = (int)((kSmem - head) / ((size_t)pitch * 4));
-        rows = rows > 1024 ? 1024 : (rows / 32) * 32;
-        const int threads = rows >= 1024 ? 1024 : (rows >= 512 ? 512 : 256);
-        if (rows > threads) rows = threads;                        // one row per thread and tile
-        const int64_t tiles = (a.n + rows - 1) / rows;
-        const int grid = (int)std::min<int64_t>(tiles, engine_num_sms() * (threads == 1024 ? 1 : 2048 / threads));
-        const size_t smem = head + (size_t)rows * pitch * 4;
-        if (a.leaf) { if (a.has_nan) predict_tiled_kernel<true, true><<<grid, threads, smem, s>>>(a, ch.first, ch.second, pitch, rows, tiles);
-                      else predict_tiled_kernel<false, true><<<grid, threads, smem, s>>>(a, ch.first, ch.second, pitch, rows, tiles); }
-        else { if (a.has_nan) predict_tiled_kernel<true, false><<<grid, threads, smem, s>>>(a, ch.first, ch.second, pitch, rows, tiles);
-               else predict_tiled_kernel<false, false><<<grid, threads, smem, s>>>(a, ch.first, ch.second, pitch, rows, tiles); }
-        ++g_kernel_launches; CUDA_OK(cudaGetLastError());
-      }
-      return;
-    }
+    return;
   }
   predict_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }

@@ -1,6 +1,7 @@
 // misc.h -- argument blocks and launchers for misc.cu / quantile.cu
 #pragma once
 #include "engine.h"
+#include "predict_plan.h"
 
 namespace b200 {
 
@@ -30,6 +31,7 @@ struct PredictArgs {
   const int64_t* h_tree_offset;   // host copy of tree_offset (plans the shared-memory tree chunks); nullptr = thread-per-row kernel
   int has_nan;              // the matrix contains missing values
   int children_adjacent;    // right child == left child + 1 in every tree (true for every tree this engine trains)
+  int model_F;              // features of the model: a matrix with F < model_F reads the features it lacks as missing
 };
 
 enum Metric : int { kMetricRmse = 0, kMetricMae = 1, kMetricLogloss = 2, kMetricError = 3, kMetricMerror = 4, kMetricMlogloss = 5,
@@ -62,6 +64,7 @@ void launch_transpose_bins(const uint8_t* bins, const uint8_t* bins_tail, int64_
 void launch_pad_rows(const uint8_t* src, const uint8_t* tail, int tw, int64_t n, int src_stride, uint8_t* dst, int dst_stride, cudaStream_t s);
 void launch_count_nan(const float* X, int64_t count, float missing, int use_missing, unsigned long long* out, cudaStream_t s);
 void launch_replace_missing(float* X, int64_t count, float missing, cudaStream_t s);
+PredictPlan plan_for(const PredictArgs& a);             // what launch_predict(a) runs
 void launch_predict(const PredictArgs& a, cudaStream_t s);
 void launch_transform(float* m, int64_t n, int K, int objective, float* out_class, cudaStream_t s);
 void launch_fill(float* p, int64_t n, float v, cudaStream_t s);

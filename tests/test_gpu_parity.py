@@ -166,6 +166,10 @@ def test_training_matches_oracle(xgb, oracle, objective, kind, K, hp, n, F, roun
     np.testing.assert_array_equal(leaves.astype(np.int32), oracle.predict_leaf(mr, X))
     margin = bst.predict(d, output_margin=True).reshape(n, -1)
     np.testing.assert_allclose(margin, oracle.predict_margin(mr, X), rtol=0, atol=MARGIN_TOL)
+    # the predictor alone: bit-exact against the oracle walking the model the device exported (MARGIN_TOL above covers
+    # the leaf values the two trainers round differently)
+    m["objective"] = objective
+    np.testing.assert_array_equal(margin.view(np.uint32), oracle.predict_margin(m, X).view(np.uint32))
 
 
 @pytest.mark.parametrize("hp", [dict(colsample_bytree=0.5), dict(colsample_bylevel=0.5), dict(colsample_bynode=0.3),
@@ -457,6 +461,8 @@ def test_lossguide_growth_matches_oracle(xgb, oracle, hp, objective, kind, n, F)
         assert max(leaves) <= hp["max_leaves"]
     np.testing.assert_array_equal(bst.predict(d, pred_leaf=True).astype(np.int32), oracle.predict_leaf(mr, X))
     np.testing.assert_allclose(bst.predict(d, output_margin=True), oracle.predict_margin(mr, X).ravel(), rtol=0, atol=MARGIN_TOL)
+    m["objective"] = objective
+    np.testing.assert_array_equal(bst.predict(d, output_margin=True).view(np.uint32), oracle.predict_margin(m, X).ravel().view(np.uint32))
     if hp["max_leaves"] == 40:          # best-first growth stops at 40 leaves: not a level-complete tree
         assert max(leaves) == 40
         t0 = slice(m["tree_offset"][0], m["tree_offset"][1])
