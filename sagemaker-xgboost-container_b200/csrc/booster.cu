@@ -9,6 +9,7 @@
 #include <cstring>
 #include <functional>
 #include "comm.h"
+#include "rng.h"
 
 namespace b200 {
 
@@ -294,9 +295,10 @@ struct GrowerImpl {
   DevBuf<unsigned char> state_block;       // all GrowState arrays
   DevBuf<unsigned char> tree_block;        // header + TreeArrays, copied to the host in one piece
   size_t tree_block_bytes = 0;
-  DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx0, ridx1, scratch;
-  // gp0 / gp1: the gradients in partition (position) order; float g alone in the first n floats for constant-hessian objectives
-  DevBuf<float2> gpair, gp0, gp1; DevBuf<unsigned> tl0, tl1; DevBuf<int> err, tree_index_dev, monotone_dev; DevBuf<unsigned char> feat_mask, ic_path, ic_allowed, ic_sets;
+  // the partition's two buffer sets: row ids, the gradients (float g alone in the first n floats for constant-hessian objectives)
+  // and the 4 tail bytes of each row, by position
+  DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx[2], scratch;
+  DevBuf<float2> gpair, gp[2]; DevBuf<unsigned> tl[2]; DevBuf<int> err, tree_index_dev, monotone_dev; DevBuf<unsigned char> feat_mask, ic_path, ic_allowed, ic_sets;
   std::vector<unsigned char> ic_sets_host; // what ic_sets holds
   std::vector<int> monotone_host;          // what monotone_dev holds (re-uploaded when the constraints or the feature count change)
   DevBuf<double> dsum;
@@ -331,10 +333,9 @@ struct GrowerImpl {
     size_t free_b = 0, total_b = 0; cudaMemGetInfo(&free_b, &total_b);
     B200_CHECK(pool_bytes < free_b / 2 + hist_pool.n * sizeof(GH64), "histogram pool for this max_depth / max_leaves / feature count does not fit in device memory");
     hist_pool.alloc(pool_slots * slot_stride);
-    ridx0.alloc(n); ridx1.alloc(n);
-    gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(engine_stream()); gp0.alloc(n); gp1.alloc(n); err.alloc(1); dsum.alloc(4);
+    gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(engine_stream()); err.alloc(1); dsum.alloc(4);
     root_h_cache.alloc(slot_stride);
-    tl0.alloc(tail_pos ? n : 0); tl1.alloc(tail_pos ? n : 0);
+    for (int i = 0; i < 2; ++i) { ridx[i].alloc(n); gp[i].alloc(n); tl[i].alloc(tail_pos ? n : 0); }
     const unsigned max_tiles = (unsigned)((n + kPartTile - 1) / kPartTile) + max_level_nodes + 1;
     scratch.alloc(3 * (size_t)max_level_nodes + 8);
     // ---- GrowState block
@@ -405,14 +406,21 @@ static TrainParamDev to_dev(const TrainParam& p) {
   d.max_delta_step = p.max_delta_step; d.max_depth = p.max_depth; d.max_leaves = p.max_leaves; return d;
 }
 
-// counter-based RNG shared with the oracle (splitmix64 on (seed, stream, index))
-static inline uint64_t splitmix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ULL; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL; x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL; return x ^ (x >> 31);
+// The histogram pass of the root: every row in order, (g,h) of class k by row.  The deeper levels (enqueue_tree) and the
+// kernel-level entry point (Booster::debug_build_root_hist) override only the row source and their mode fields.
+static HistArgs hist_args(const GrowerImpl& g, const BinnedMatrix& bm, int k) {
+  HistArgs ha{}; ha.bins = bm.bins; ha.bins_tail = bm.bins_tail; ha.n = bm.n; ha.row_stride = bm.ngroups * kSlots; ha.tw = bm.tw;
+  ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride;
+  ha.tail_in_gather = bm.tail_in_gather;          // gathered passes on the aligned copy always read the tail from the row's line
+  ha.gpair = g.gpair.p + (size_t)k * g.gp_stride;
+  ha.build_count = g.gs.build_count; ha.build_nid = g.gs.build_nid; ha.build_prefix = g.gs.build_prefix; ha.seg_begin = g.gs.seg_begin;
+  ha.hist_slot = g.gs.hist_slot; ha.scales = g.gs.scales; ha.hist_pool = g.hist_pool.p; ha.node_sum = g.gs.node_sum; ha.ngroups = bm.ngroups;
+  ha.accumulate_sum = 1; ha.window_rows = job_window_rows(g.global_n);
+  return ha;
 }
-static inline float rng_uniform(uint32_t seed, uint64_t stream, uint64_t idx) {
-  uint64_t h = splitmix64(splitmix64(((uint64_t)seed << 32) ^ stream) ^ idx);
-  return (float)(h >> 40) * (1.0f / 16777216.0f);
-}
+
+constexpr int kRootRows = -1;     // the partition's input at the root: every row in order, the float2 gpair and the tail words by row
+
 // Column sampling (upstream src/common/random.h ColumnSampler: bytree, then bylevel inside it, then bynode inside that; a
 // subset keeps max(1, floor(frac * |parent|)) features).  Upstream shuffles with a mt19937; product and oracle share a
 // counter-based rule instead: feature f of the parent set is kept iff fewer than `keep` parent features have a smaller
@@ -747,7 +755,7 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
   const int num_sms = engine_num_sms();
   const unsigned max_tiles = (unsigned)((dtrain->n + kPartTile - 1) / kPartTile) + g.max_level_nodes + 1;
 
-  launch_init_tree(g.gs, g.ta, (unsigned)dtrain->n, 0, g.max_level_nodes, s);
+  launch_init_tree(g.gs, g.ta, (unsigned)dtrain->n, s);
   if (root_mode == 2) { slot_from_cache_kernel<<<num_sms, 256, 0, s>>>(g.hist_pool.p, g.root_h_cache.p, g.slot_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
   else CUDA_OK(cudaMemsetAsync(g.hist_pool.p, 0, g.slot_stride * sizeof(GH64), s));
 
@@ -761,18 +769,12 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     prof_part_row_bytes_[1] = prof_part_row_bytes_[2] + 1;                         // deeper levels: id + payload + split byte
   }
 
-  HistArgs ha{}; ha.bins = bm.bins; ha.bins_tail = bm.bins_tail; ha.n = bm.n; ha.row_stride = bm.ngroups * kSlots; ha.tw = bm.tw;
-  ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride; ha.tail_in_gather = bm.tail_in_gather;
-  ha.gpair = g.gpair.p + (size_t)k * g.gp_stride; ha.ridx = nullptr;
-  ha.build_count = g.gs.build_count; ha.build_nid = g.gs.build_nid; ha.build_prefix = g.gs.build_prefix; ha.seg_begin = g.gs.seg_begin;
-  ha.hist_slot = g.gs.hist_slot; ha.scales = g.gs.scales; ha.hist_pool = g.hist_pool.p; ha.node_sum = g.gs.node_sum; ha.ngroups = bm.ngroups;
-  ha.accumulate_sum = 1; ha.g_only = root_mode == 2 ? 1 : 0; ha.window_rows = job_window_rows(g.global_n);
-  ha.rows_counter = profile_ ? prof_rows_.p : nullptr;
+  HistArgs root = hist_args(g, bm, k);
+  root.g_only = root_mode == 2 ? 1 : 0; root.rows_counter = profile_ ? prof_rows_.p : nullptr;
   prof_begin(kProfRootHist);
-  launch_hist_build(ha, num_sms, s);
+  launch_hist_build(root, num_sms, s);
   prof_end();
   if (root_mode == 1) { snapshot_h_kernel<<<num_sms, 256, 0, s>>>(g.hist_pool.p, g.root_h_cache.p, g.slot_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
-  ha.g_only = 0;
   // a collective: issued directly, or (under capture) closes the current graph segment and is remembered for the replay
   auto collective = [&](std::function<void()> f) {
     if (!comm.distributed()) return;
@@ -804,34 +806,51 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     CUDA_OK(cudaMemsetAsync(g.ic_path.p, 0, (size_t)bm.F, s));
     CUDA_OK(cudaMemsetAsync(g.ic_allowed.p, 1, (size_t)bm.F, s));
   }
-  EvalArgs ea{}; ea.hist_pool = g.hist_pool.p; ea.gs = g.gs; ea.cut_ptrs = dtrain->d_cut_ptrs.p; ea.feat_mask = mask; ea.p = pd; ea.F = bm.F;
-  ea.ngroups = bm.ngroups; ea.tw = bm.tw; ea.ntail = bm.ntail; ea.has_missing = bm.has_missing; ea.level = 0; ea.max_level_nodes = g.max_level_nodes;
-  ea.colsample_bynode = mask ? param_.colsample_bynode : 1.0f; ea.seed = param_.seed; ea.tree_index = g.tree_index_dev.p; ea.monotone = mono_dev; ea.node_allowed = ic_on ? g.ic_allowed.p : nullptr;
-  launch_eval(ea, 1, s);
+  // The argument blocks of this tree's kernels, each filled in one place.  The two growth policies below pass only their own data:
+  // the level, the buffer sets and the feature mask.
+  auto eval_args = [&](int level, const unsigned char* feat_mask) {
+    EvalArgs ea{}; ea.hist_pool = g.hist_pool.p; ea.gs = g.gs; ea.cut_ptrs = dtrain->d_cut_ptrs.p; ea.feat_mask = feat_mask; ea.p = pd; ea.F = bm.F;
+    ea.ngroups = bm.ngroups; ea.tw = bm.tw; ea.ntail = bm.ntail; ea.has_missing = bm.has_missing; ea.level = level; ea.max_level_nodes = g.max_level_nodes;
+    ea.colsample_bynode = mask ? param_.colsample_bynode : 1.0f; ea.seed = param_.seed; ea.tree_index = g.tree_index_dev.p; ea.monotone = mono_dev; ea.node_allowed = ic_on ? g.ic_allowed.p : nullptr;
+    return ea;
+  };
+  auto apply_args = [&](int level, int next_base, int next_half) {     // next_base, next_half: the children's histogram slots (depth-wise)
+    ApplyArgs aa{}; aa.gs = g.gs; aa.tree = g.ta; aa.cut_ptrs = dtrain->d_cut_ptrs.p; aa.cut_vals = dtrain->d_cut_vals.p; aa.min_vals = dtrain->d_min_vals.p;
+    aa.p = pd; aa.scratch = g.scratch.p; aa.nblocks = bm.ngroups + (bm.tw > 0 ? 1 : 0); aa.level = level; aa.max_level_nodes = g.max_level_nodes; aa.next_base = next_base; aa.next_half = next_half; aa.monotone = mono_dev;
+    if (ic_on) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = (int)interaction_.size(); aa.F = bm.F; }
+    return aa;
+  };
+  auto part_args = [&](int level, int cur, int next) {                  // the partition of `level` from buffer set `cur` into set `next`
+    const bool root = cur == kRootRows;
+    PartArgs pa{}; pa.gs = g.gs; pa.tree = g.ta; pa.bins_col = bm.bins_col; pa.n = bm.n;
+    pa.ridx_cur = root ? nullptr : g.ridx[cur].p; pa.ridx_next = g.ridx[next].p;
+    pa.gp_cur = root ? static_cast<const void*>(g.gpair.p + (size_t)k * g.gp_stride) : g.gp[cur].p; pa.gp_next = g.gp[next].p;
+    pa.gp_cur_stride = root ? 2 : 1; pa.g_only = g_only ? 1 : 0;
+    pa.tl_cur = !carry_tail ? nullptr : (root ? reinterpret_cast<const unsigned*>(bm.bins_tail) : g.tl[cur].p); pa.tl_next = carry_tail ? g.tl[next].p : nullptr;
+    pa.has_missing = bm.has_missing; pa.level = level; pa.max_level_nodes = g.max_level_nodes; pa.rows_counter = profile_ ? prof_rows_.p + 2 : nullptr;
+    return pa;
+  };
+  auto level_hist_args = [&](int set) {                                 // the build list's rows by position in buffer set `set`
+    HistArgs ha = hist_args(g, bm, k);
+    ha.ridx = g.ridx[set].p; ha.tail_pos = carry_tail ? g.tl[set].p : nullptr; ha.accumulate_sum = 0;
+    ha.gpair = g_only ? nullptr : g.gp[set].p; ha.gpos = g_only ? reinterpret_cast<const float*>(g.gp[set].p) : nullptr;
+    ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
+    return ha;
+  };
+  launch_eval(eval_args(0, mask), 1, s);
 
   const int lg_iters = lossguide_iters(param_);
   for (int it = 0; it < lg_iters; ++it) {                 // grow_policy=lossguide: one expansion per iteration (tree.cu apply_lossguide_kernel)
-    ApplyArgs aa{}; aa.gs = g.gs; aa.tree = g.ta; aa.cut_ptrs = dtrain->d_cut_ptrs.p; aa.cut_vals = dtrain->d_cut_vals.p; aa.min_vals = dtrain->d_min_vals.p;
-    aa.p = pd; aa.scratch = g.scratch.p; aa.ngroups = bm.ngroups + (bm.tw > 0 ? 1 : 0); aa.level = 0; aa.max_level_nodes = g.max_level_nodes; aa.monotone = mono_dev;
-    if (ic_on) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = (int)interaction_.size(); aa.F = bm.F; }
-    launch_apply_lossguide(aa, it, s);
+    launch_apply_lossguide(apply_args(0, 0, 0), it, s);
     // live row segments always sit in buffer set 0; the partition writes the children into set 1 and they are copied straight back
-    PartArgs pa{}; pa.gs = g.gs; pa.tree = g.ta; pa.bins_col = bm.bins_col; pa.n = bm.n;
-    pa.ridx_cur = it == 0 ? nullptr : g.ridx0.p; pa.ridx_next = g.ridx1.p;
-    pa.gp_cur = it == 0 ? static_cast<const void*>(g.gpair.p + (size_t)k * g.gp_stride) : g.gp0.p; pa.gp_next = g.gp1.p;
-    pa.gp_cur_stride = it == 0 ? 2 : 1; pa.g_only = g_only ? 1 : 0;
-    pa.tl_cur = !carry_tail ? nullptr : (it == 0 ? reinterpret_cast<const unsigned*>(bm.bins_tail) : g.tl0.p); pa.tl_next = !carry_tail ? nullptr : g.tl1.p;
-    pa.has_missing = bm.has_missing; pa.level = 0; pa.max_level_nodes = g.max_level_nodes; pa.rows_counter = profile_ ? prof_rows_.p + 2 : nullptr;
+    const PartArgs pa = part_args(0, it == 0 ? kRootRows : 0, 1);
     prof_begin(kProfPartition);
     launch_partition(pa, max_tiles, s);
     prof_end();
-    launch_lg_copy_back(pa, g.ridx0.p, g.gp0.p, g.tl0.p, max_tiles, s);
+    launch_lg_copy_back(pa, g.ridx[0].p, g.gp[0].p, g.tl[0].p, max_tiles, s);
     launch_zero_build_slots(g.gs, g.hist_pool.p, g.slot_stride, 1, s);
-    ha.ridx = g.ridx0.p; ha.tail_pos = carry_tail ? g.tl0.p : nullptr; ha.accumulate_sum = 0;
-    ha.gpair = g_only ? nullptr : g.gp0.p; ha.gpos = g_only ? reinterpret_cast<const float*>(g.gp0.p) : nullptr;
-    ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
     prof_begin(kProfDeepHist);
-    launch_hist_build(ha, num_sms, s);
+    launch_hist_build(level_hist_args(0), num_sms, s);
     prof_end();
     if (comm.distributed()) {                              // the collective needs a fixed address: go through the staging slot
       launch_lg_stage(g.gs, g.hist_pool.p, g.slot_stride, 1, s);
@@ -839,45 +858,27 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
       launch_lg_stage(g.gs, g.hist_pool.p, g.slot_stride, 0, s);
     }
     launch_subtract(g.gs, g.hist_pool.p, g.slot_stride, 1, s);
-    ea.level = 1; ea.feat_mask = nullptr;
-    launch_eval(ea, 2, s);
+    launch_eval(eval_args(1, nullptr), 2, s);
   }
 
   for (int L = 0; L < D && lg_iters == 0; ++L) {
     const bool final_level = (L == D - 1);
     const int next_base = ((L + 1) & 1) * g.region, next_half = 1 << L;
-    ApplyArgs aa{}; aa.gs = g.gs; aa.tree = g.ta; aa.cut_ptrs = dtrain->d_cut_ptrs.p; aa.cut_vals = dtrain->d_cut_vals.p; aa.min_vals = dtrain->d_min_vals.p;
-    aa.p = pd; aa.scratch = g.scratch.p; aa.ngroups = bm.ngroups + (bm.tw > 0 ? 1 : 0); aa.level = L; aa.max_level_nodes = g.max_level_nodes; aa.next_base = next_base; aa.next_half = next_half; aa.monotone = mono_dev;
-    if (ic_on) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = (int)interaction_.size(); aa.F = bm.F; }
-    launch_apply(aa, s);
+    launch_apply(apply_args(L, next_base, next_half), s);
     if (final_level) break;                  // children of the last level are leaves: no partition, no histograms
-    PartArgs pa{}; pa.gs = g.gs; pa.tree = g.ta; pa.bins_col = bm.bins_col; pa.n = bm.n;
-    pa.ridx_cur = L == 0 ? nullptr : ((L & 1) ? g.ridx0.p : g.ridx1.p);
-    pa.ridx_next = (L & 1) ? g.ridx1.p : g.ridx0.p;
-    pa.gp_cur = L == 0 ? g.gpair.p + (size_t)k * g.gp_stride : ((L & 1) ? g.gp0.p : g.gp1.p);
-    pa.gp_next = (L & 1) ? g.gp1.p : g.gp0.p;
-    pa.gp_cur_stride = L == 0 ? 2 : 1; pa.g_only = g_only ? 1 : 0;
-    pa.tl_cur = !carry_tail ? nullptr : (L == 0 ? reinterpret_cast<const unsigned*>(bm.bins_tail) : ((L & 1) ? g.tl0.p : g.tl1.p));
-    pa.tl_next = !carry_tail ? nullptr : ((L & 1) ? g.tl1.p : g.tl0.p);
-    pa.has_missing = bm.has_missing; pa.level = L; pa.max_level_nodes = g.max_level_nodes;
+    PartArgs pa = part_args(L, L == 0 ? kRootRows : (L & 1) ^ 1, L & 1);     // the buffer sets alternate
     pa.build_only = L == D - 2 ? 1 : 0;                    // the next level is the last one: only the built children are read again
-    pa.rows_counter = profile_ ? prof_rows_.p + 2 : nullptr;
     prof_begin(kProfPartition);
     launch_partition(pa, max_tiles, s);
     prof_end();
     // histograms of the next level: build the smaller children, all-reduce, subtract for the siblings
     CUDA_OK(cudaMemsetAsync(g.hist_pool.p + (size_t)next_base * g.slot_stride, 0, (size_t)next_half * g.slot_stride * sizeof(GH64), s));
-    ha.ridx = pa.ridx_next; ha.tail_pos = pa.tl_next; ha.accumulate_sum = 0;
-    ha.gpair = g_only ? nullptr : static_cast<const float2*>(pa.gp_next); ha.gpos = g_only ? static_cast<const float*>(pa.gp_next) : nullptr;
-    ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
     prof_begin(kProfDeepHist);
-    launch_hist_build(ha, num_sms, s);
+    launch_hist_build(level_hist_args(L & 1), num_sms, s);
     prof_end();
     allreduce_hist(g.hist_pool.p + (size_t)next_base * g.slot_stride, (size_t)next_half * g.slot_stride * 2);
     launch_subtract(g.gs, g.hist_pool.p, g.slot_stride, next_half, s);
-    ea.level = L + 1;
-    ea.feat_mask = mask ? mask + (size_t)(L + 1) * bm.F : nullptr;
-    launch_eval(ea, 1 << (L + 1), s);
+    launch_eval(eval_args(L + 1, mask ? mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
   }
 
   // prediction cache += leaf values of this tree: one row-order pass over the column-major bins
@@ -1173,7 +1174,7 @@ void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::v
   const int64_t rows = row_ids ? n_ids : dm->n;
   B200_CHECK(rows <= dm->n, "debug_build_root_hist: more row ids than rows");
   CUDA_OK(cudaMemcpyAsync(g.gpair.p, gpair_host, sizeof(float2) * rows, cudaMemcpyHostToDevice, s));
-  if (row_ids) CUDA_OK(cudaMemcpyAsync(g.ridx0.p, row_ids, sizeof(unsigned) * rows, cudaMemcpyHostToDevice, s));
+  if (row_ids) CUDA_OK(cudaMemcpyAsync(g.ridx[0].p, row_ids, sizeof(unsigned) * rows, cudaMemcpyHostToDevice, s));
   // scales from max|g|, max h of the supplied pairs
   float mg = 0.f, mh = 0.f;
   for (int64_t i = 0; i < rows; ++i) { mg = std::max(mg, std::fabs(gpair_host[2 * i])); mh = std::max(mh, gpair_host[2 * i + 1]); }
@@ -1181,31 +1182,27 @@ void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::v
   CUDA_OK(cudaMemcpyAsync(g.gs.absmax, am, 8, cudaMemcpyHostToDevice, s));
   launch_scales(g.gs, job_grad_bits(g.global_n), s);
   const BinnedMatrix bm = dm->binned_view();
-  HistArgs ha{}; ha.bins = bm.bins; ha.bins_tail = bm.bins_tail; ha.n = bm.n; ha.row_stride = bm.ngroups * kSlots; ha.tw = bm.tw; ha.gpair = g.gpair.p;
-  ha.bins_gather = bm.bins_gather; ha.gather_stride = bm.gather_stride;
-  ha.ridx = row_ids ? g.ridx0.p : nullptr;
+  HistArgs ha = hist_args(g, bm, 0);              // the training path's arguments; the row ids and the mode bits override
+  ha.ridx = row_ids ? g.ridx[0].p : nullptr;
+  ha.force_gather = (mode & 3) == 1 ? 1 : 0; ha.g_only = (mode & 3) == 2 ? 1 : 0;
   if (mode & 8) {                               // G-only payload: g alone by position, h == 1.0f for every row (the supplied h is ignored)
     std::vector<float> gh((size_t)rows);
     for (int64_t i = 0; i < rows; ++i) gh[i] = gpair_host[2 * i];
-    float* gpos = reinterpret_cast<float*>(g.gp0.p);
+    float* gpos = reinterpret_cast<float*>(g.gp[0].p);
     if (rows) CUDA_OK(cudaMemcpyAsync(gpos, gh.data(), sizeof(float) * rows, cudaMemcpyHostToDevice, s));
     Comm::get().sync_stream(s);
     ha.gpos = gpos; ha.gpair = nullptr;
   }
-  ha.build_count = g.gs.build_count; ha.build_nid = g.gs.build_nid; ha.build_prefix = g.gs.build_prefix; ha.seg_begin = g.gs.seg_begin;
-  ha.hist_slot = g.gs.hist_slot; ha.scales = g.gs.scales; ha.hist_pool = g.hist_pool.p; ha.node_sum = g.gs.node_sum; ha.ngroups = bm.ngroups; ha.accumulate_sum = 1;
-  ha.force_gather = (mode & 3) == 1 ? 1 : 0; ha.g_only = (mode & 3) == 2 ? 1 : 0; ha.window_rows = job_window_rows(g.global_n);
-  ha.tail_in_gather = bm.tail_in_gather;          // gathered passes on the aligned copy always read the tail from the row's line
   if ((mode & 4) && row_ids && tail_by_position(bm)) {     // the training path's variant: the rows' tail words by POSITION (as after a partition)
-    gather_u32_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(reinterpret_cast<const unsigned*>(bm.bins_tail), g.ridx0.p, g.tl0.p, rows); ++g_kernel_launches;
+    gather_u32_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(reinterpret_cast<const unsigned*>(bm.bins_tail), g.ridx[0].p, g.tl[0].p, rows); ++g_kernel_launches;
     CUDA_OK(cudaGetLastError());
-    ha.tail_pos = g.tl0.p;
+    ha.tail_pos = g.tl[0].p;
   }
   g.root_h_valid = false;                       // the debug entry point overwrites gpair and the root slot
   cudaEvent_t e0, e1; CUDA_OK(cudaEventCreate(&e0)); CUDA_OK(cudaEventCreate(&e1));
   float total = 0.f;
   for (int r = 0; r < std::max(1, repeats); ++r) {
-    launch_init_tree(g.gs, g.ta, (unsigned)rows, 0, g.max_level_nodes, s);
+    launch_init_tree(g.gs, g.ta, (unsigned)rows, s);
     CUDA_OK(cudaMemsetAsync(g.hist_pool.p, 0, g.slot_stride * sizeof(GH64), s));
     CUDA_OK(cudaEventRecord(e0, s));
     launch_hist_build(ha, engine_num_sms(), s);

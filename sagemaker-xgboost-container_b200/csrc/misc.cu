@@ -7,6 +7,7 @@
 #include <utility>
 #include "engine.h"
 #include "misc.h"
+#include "rng.h"
 
 namespace b200 {
 
@@ -15,15 +16,6 @@ __device__ __forceinline__ float sigmoidf_xgb(float x) {
   x = fminf(-x, 88.7f);
   float denom = expf(x) + 1.0f + kEps;
   return 1.0f / denom;
-}
-
-__device__ __forceinline__ unsigned long long splitmix64_dev(unsigned long long x) {
-  x += 0x9E3779B97F4A7C15ULL; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL; return x ^ (x >> 31);
-}
-__device__ __forceinline__ float rng_uniform_dev(unsigned seed, unsigned long long stream, unsigned long long idx) {
-  unsigned long long h = splitmix64_dev(splitmix64_dev(((unsigned long long)seed << 32) ^ stream) ^ idx);
-  return (float)(h >> 40) * (1.0f / 16777216.0f);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -35,7 +27,7 @@ __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
     const float y = a.label[r];
     float w = a.weight ? a.weight[r] : 1.0f;
     bool dropped = false;
-    if (a.subsample < 1.0f) dropped = !(rng_uniform_dev(a.seed, 0x2000ull + a.iter, (unsigned long long)(r + a.row_offset)) < a.subsample);
+    if (a.subsample < 1.0f) dropped = !(rng_uniform(a.seed, 0x2000ull + a.iter, (unsigned long long)(r + a.row_offset)) < a.subsample);
     if (a.objective == kSoftprob || a.objective == kSoftmax) {
       const int K = a.K;
       const float* m = a.margin ? a.margin + r * K : nullptr;

@@ -4,6 +4,7 @@
 // src/common/partition_builder.h as restated in oracle/gbt_oracle.c; all control flow stays on the device.
 #include <type_traits>
 #include "engine.h"
+#include "rng.h"
 #include "tree.h"
 
 namespace b200 {
@@ -71,16 +72,6 @@ __device__ __forceinline__ bool constrained_split_gain(const TrainParamDev& p, d
   return c == 0 || (c > 0 ? wl <= wr : wl >= wr);
 }
 
-// counter-based RNG shared with the host and the oracle (splitmix64 on (seed, stream, index)); booster.cu subset_mask
-__device__ __forceinline__ unsigned long long splitmix64_tree(unsigned long long x) {
-  x += 0x9E3779B97F4A7C15ULL; x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBULL; return x ^ (x >> 31);
-}
-__device__ __forceinline__ float rng_uniform_tree(unsigned seed, unsigned long long stream, unsigned long long idx) {
-  unsigned long long h = splitmix64_tree(splitmix64_tree(((unsigned long long)seed << 32) ^ stream) ^ idx);
-  return (float)(h >> 40) * (1.0f / 16777216.0f);
-}
-
 // Total order of candidates == upstream SplitEntry::NeedReplace: larger loss_chg, then lower feature,
 // then earlier position in scan order (forward bins ascending, then backward bins descending).
 __device__ __forceinline__ unsigned long long cand_key(float loss, int f, int ord) {
@@ -90,20 +81,19 @@ __device__ __forceinline__ unsigned long long cand_key(float loss, int f, int or
 }
 
 // ---------------------------------------------------------------------------------------------
-__global__ void init_tree_kernel(GrowState gs, TreeArrays t, unsigned n, int root_slot, int max_level_nodes) {
+__global__ void init_tree_kernel(GrowState gs, TreeArrays t, unsigned n) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   *gs.n_nodes = 1; *gs.n_leaves = 1;
   *gs.n_slots = kLgFirstFreeSlot; *gs.lg_done = 0; gs.depth[0] = 0; gs.open[0] = 0;
   gs.lower[0] = -INFINITY; gs.upper[0] = INFINITY;
   for (int d = 0; d < kMaxDepth + 2; ++d) gs.level_count[d] = 0;
   gs.level_count[0] = 1; gs.level_nodes[0] = 0;
-  gs.seg_begin[0] = 0; gs.seg_count[0] = n; gs.hist_slot[0] = root_slot;
+  gs.seg_begin[0] = 0; gs.seg_count[0] = n; gs.hist_slot[0] = kLgRootSlot;
   gs.node_sum[0].g = 0; gs.node_sum[0].h = 0;
   *gs.build_count = 1; gs.build_nid[0] = 0; gs.build_sub_nid[0] = -1; gs.build_parent_slot[0] = -1;
   gs.build_prefix[0] = 0; gs.build_prefix[1] = n;
   t.left[0] = -1; t.right[0] = -1; t.parent[0] = 2147483647; t.split_index[0] = 0; t.split_bin[0] = -1;
   t.default_left[0] = 0; t.split_cond[0] = 0.f; t.base_weight[0] = 0.f; t.loss_chg[0] = 0.f; t.sum_hess[0] = 0.f;
-  (void)max_level_nodes;
 }
 
 // Fixed-point scales from the all-reduced max|g|, max h of this round: power-of-two so that
@@ -145,10 +135,10 @@ __global__ void __launch_bounds__(32 * kEvalSegs) eval_kernel(EvalArgs a) {
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
     const unsigned long long stream = 0x80000000ull + ((unsigned long long)(unsigned)*a.tree_index << 20) + (unsigned long long)nid;
-    const float uf = rng_uniform_tree(a.seed, stream, (unsigned long long)f);
+    const float uf = rng_uniform(a.seed, stream, (unsigned long long)f);
     int rank = 0, cnt = 0;
     for (int g = seg; g < a.F; g += kEvalSegs) {
-      if (a.feat_mask[g]) { ++cnt; const float ug = rng_uniform_tree(a.seed, stream, (unsigned long long)g); rank += (ug < uf || (ug == uf && g < f)) ? 1 : 0; }
+      if (a.feat_mask[g]) { ++cnt; const float ug = rng_uniform(a.seed, stream, (unsigned long long)g); rank += (ug < uf || (ug == uf && g < f)) ? 1 : 0; }
     }
     if (rank) atomicAdd(&s_rank[slot], rank);
     if (slot == 0 && cnt) atomicAdd(&s_cnt, cnt);
@@ -264,11 +254,82 @@ __device__ unsigned block_exclusive_scan(const unsigned* in, unsigned* out, int 
 }
 
 // ---------------------------------------------------------------------------------------------
-// node expansion for one level (single block): validity, child ids, tree arrays, build list, partition plan
+// node expansion, shared by the depth-wise (apply_kernel) and the loss-guided (apply_lossguide_kernel) policy
+// ---------------------------------------------------------------------------------------------
+// best split of nid over its candidate blocks (eval_kernel writes one per feature group and one for the tail); kept in gs.best
+__device__ __forceinline__ SplitCand best_of_blocks(const ApplyArgs& a, int nid) {
+  SplitCand best = a.gs.best_group[(size_t)nid * a.nblocks];
+  unsigned long long bk = cand_key(best.loss_chg, best.feature, best.ord);
+  for (int g = 1; g < a.nblocks; ++g) {
+    SplitCand c = a.gs.best_group[(size_t)nid * a.nblocks + g];
+    unsigned long long k = cand_key(c.loss_chg, c.feature, c.ord);
+    if (k > bk) { bk = k; best = c; }
+  }
+  a.gs.best[nid] = best;
+  return best;
+}
+
+// ExpandEntry::IsValid for a node at `depth` (max_leaves is the policy's: level order or queue order)
+__device__ __forceinline__ bool split_is_valid(const TrainParamDev& p, const SplitCand& best, const GH64& tot, int depth) {
+  bool ok = best.loss_chg > 1e-6f;
+  if (ok && (best.HL == 0 || tot.h - best.HL == 0)) ok = false;
+  if (ok && best.loss_chg < p.gamma) ok = false;
+  if (ok && p.max_depth > 0 && depth >= p.max_depth) ok = false;
+  return ok;
+}
+
+// the root was created without a parent: finish it once eval_kernel has its weight
+__device__ __forceinline__ void finish_root(const ApplyArgs& a, double ish) {
+  const GrowState& gs = a.gs; const TreeArrays& t = a.tree;
+  t.base_weight[0] = gs.weight[0]; t.sum_hess[0] = (float)((double)gs.node_sum[0].h * ish); t.split_cond[0] = a.p.eta * gs.weight[0];
+}
+
+// Split nid by `best` into the new leaves Lc, Rc: tree arrays, the children's weight bounds and allowed features, their sums.
+// Their row segments are set by part_kernel.
+__device__ __forceinline__ void expand_node(const ApplyArgs& a, int nid, const SplitCand& best, const GH64& tot, int Lc, int Rc, double isg, double ish) {
+  const GrowState& gs = a.gs; const TreeArrays& t = a.tree;
+  const long long GLq = best.GL, HLq = best.HL, GRq = tot.g - best.GL, HRq = tot.h - best.HL;
+  const double GL = (double)GLq * isg, HL = (double)HLq * ish, GR = (double)GRq * isg, HR = (double)HRq * ish;
+  float wl = calc_weight(a.p, GL, HL), wr = calc_weight(a.p, GR, HR);
+  if (a.monotone) {            // TreeEvaluator::AddSplit: children inherit the interval, mid bounds the constrained side
+    const float lo = gs.lower[nid], hi = gs.upper[nid];
+    wl = clamp_weight(wl, lo, hi); wr = clamp_weight(wr, lo, hi);
+    const float mid = (wl + wr) / 2.0f; const int mc = a.monotone[best.feature];
+    gs.lower[Lc] = lo; gs.upper[Lc] = hi; gs.lower[Rc] = lo; gs.upper[Rc] = hi;
+    if (mc < 0) { gs.lower[Lc] = mid; gs.upper[Rc] = mid; } else if (mc > 0) { gs.upper[Lc] = mid; gs.lower[Rc] = mid; }
+  }
+  interaction_children(a, nid, best.feature, Lc, Rc);
+  const int cb = a.cut_ptrs[best.feature];
+  const float thr = best.dleft ? (best.bin < 0 ? a.min_vals[best.feature] : a.cut_vals[cb + best.bin]) : a.cut_vals[cb + best.bin];
+  t.left[nid] = Lc; t.right[nid] = Rc; t.split_index[nid] = best.feature; t.split_cond[nid] = thr;
+  t.split_bin[nid] = best.bin; t.default_left[nid] = (unsigned char)best.dleft;
+  t.base_weight[nid] = gs.weight[nid]; t.loss_chg[nid] = best.loss_chg; t.sum_hess[nid] = (float)((double)tot.h * ish);
+  const int ch[2] = {Lc, Rc}; const float cw[2] = {wl, wr}; const double chh[2] = {HL, HR};
+  for (int s = 0; s < 2; ++s) {
+    const int c = ch[s];
+    t.left[c] = -1; t.right[c] = -1; t.parent[c] = nid; t.split_index[c] = 0; t.split_bin[c] = -1; t.default_left[c] = 0;
+    t.split_cond[c] = a.p.eta * cw[s]; t.base_weight[c] = a.p.eta * cw[s]; t.loss_chg[c] = 0.f; t.sum_hess[c] = (float)chh[s];
+  }
+  gs.node_sum[Lc].g = GLq; gs.node_sum[Lc].h = HLq; gs.node_sum[Rc].g = GRq; gs.node_sum[Rc].h = HRq;
+  gs.seg_begin[Lc] = 0; gs.seg_count[Lc] = 0; gs.seg_begin[Rc] = 0; gs.seg_count[Rc] = 0;
+}
+
+// Build list entry r for the children of nid: the child with the smaller hessian sum gets its histogram built into bld_slot,
+// its sibling's (sub_slot) is the parent's minus it (subtract_kernel).
+__device__ __forceinline__ void plan_child_hists(const GrowState& gs, int r, int nid, const SplitCand& best, const GH64& tot, int Lc, int Rc,
+                                                 int bld_slot, int sub_slot) {
+  const bool fewer_right = tot.h - best.HL < best.HL;
+  const int bld = fewer_right ? Rc : Lc, sub = fewer_right ? Lc : Rc;
+  gs.hist_slot[bld] = bld_slot; gs.hist_slot[sub] = sub_slot;
+  gs.build_nid[r] = bld; gs.build_sub_nid[r] = sub; gs.build_parent_slot[r] = gs.hist_slot[nid];
+}
+
+// ---------------------------------------------------------------------------------------------
+// depth-wise: expansion of one level (single block): the max_leaves order, child ids, level-region histogram slots, partition plan
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) apply_kernel(ApplyArgs a) {
   __shared__ unsigned s_tmp[33];
-  GrowState& gs = a.gs; TreeArrays& t = a.tree;
+  GrowState& gs = a.gs;
   const int L = a.level;
   const int cnt = gs.level_count[L];
   const int* nodes = gs.level_nodes + (size_t)L * a.max_level_nodes;
@@ -276,26 +337,11 @@ __global__ void __launch_bounds__(256) apply_kernel(ApplyArgs a) {
   unsigned* rank = a.scratch + a.max_level_nodes;    // [max_level_nodes]
   unsigned* tiles = a.scratch + 2 * (size_t)a.max_level_nodes;
   const double isg = (double)gs.scales[2], ish = (double)gs.scales[3];
-  if (L == 0 && threadIdx.x == 0 && cnt > 0) {      // the root was created without a parent: finish it here
-    t.base_weight[0] = gs.weight[0]; t.sum_hess[0] = (float)((double)gs.node_sum[0].h * ish);
-    t.split_cond[0] = a.p.eta * gs.weight[0];
-  }
+  if (L == 0 && threadIdx.x == 0 && cnt > 0) finish_root(a, ish);
   for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
     const int nid = nodes[i];
-    SplitCand best = gs.best_group[(size_t)nid * a.ngroups];
-    unsigned long long bk = cand_key(best.loss_chg, best.feature, best.ord);
-    for (int g = 1; g < a.ngroups; ++g) {
-      SplitCand c = gs.best_group[(size_t)nid * a.ngroups + g];
-      unsigned long long k = cand_key(c.loss_chg, c.feature, c.ord);
-      if (k > bk) { bk = k; best = c; }
-    }
-    gs.best[nid] = best;
-    const GH64 tot = gs.node_sum[nid];
-    bool ok = best.loss_chg > 1e-6f;
-    if (ok && (best.HL == 0 || tot.h - best.HL == 0)) ok = false;
-    if (ok && best.loss_chg < a.p.gamma) ok = false;
-    if (ok && a.p.max_depth > 0 && L >= a.p.max_depth) ok = false;
-    valid[i] = ok ? 1u : 0u;
+    const SplitCand best = best_of_blocks(a, nid);
+    valid[i] = split_is_valid(a.p, best, gs.node_sum[nid], L) ? 1u : 0u;
   }
   __syncthreads();
   if (a.p.max_leaves > 0 && threadIdx.x == 0) {     // Driver::Pop order: increasing nid, stop at max_leaves
@@ -315,37 +361,11 @@ __global__ void __launch_bounds__(256) apply_kernel(ApplyArgs a) {
     const GH64 tot = gs.node_sum[nid];
     const int r = (int)rank[i];
     const int Lc = n0 + 2 * r, Rc = Lc + 1;
-    const long long GLq = best.GL, HLq = best.HL, GRq = tot.g - best.GL, HRq = tot.h - best.HL;
-    const double GL = (double)GLq * isg, HL = (double)HLq * ish, GR = (double)GRq * isg, HR = (double)HRq * ish;
-    float wl = calc_weight(a.p, GL, HL), wr = calc_weight(a.p, GR, HR);
-    if (a.monotone) {            // TreeEvaluator::AddSplit: children inherit the interval, mid bounds the constrained side
-      const float lo = gs.lower[nid], hi = gs.upper[nid];
-      wl = clamp_weight(wl, lo, hi); wr = clamp_weight(wr, lo, hi);
-      const float mid = (wl + wr) / 2.0f; const int mc = a.monotone[best.feature];
-      gs.lower[Lc] = lo; gs.upper[Lc] = hi; gs.lower[Rc] = lo; gs.upper[Rc] = hi;
-      if (mc < 0) { gs.lower[Lc] = mid; gs.upper[Rc] = mid; } else if (mc > 0) { gs.upper[Lc] = mid; gs.lower[Rc] = mid; }
-    }
-    interaction_children(a, nid, best.feature, Lc, Rc);
-    const int cb = a.cut_ptrs[best.feature];
-    float thr = best.dleft ? (best.bin < 0 ? a.min_vals[best.feature] : a.cut_vals[cb + best.bin]) : a.cut_vals[cb + best.bin];
-    t.left[nid] = Lc; t.right[nid] = Rc; t.split_index[nid] = best.feature; t.split_cond[nid] = thr;
-    t.split_bin[nid] = best.bin; t.default_left[nid] = (unsigned char)best.dleft;
-    t.base_weight[nid] = gs.weight[nid]; t.loss_chg[nid] = best.loss_chg; t.sum_hess[nid] = (float)((double)tot.h * ish);
-    const int ch[2] = {Lc, Rc}; const float cw[2] = {wl, wr}; const double chh[2] = {HL, HR};
-    for (int s = 0; s < 2; ++s) {
-      int c = ch[s];
-      t.left[c] = -1; t.right[c] = -1; t.parent[c] = nid; t.split_index[c] = 0; t.split_bin[c] = -1; t.default_left[c] = 0;
-      t.split_cond[c] = a.p.eta * cw[s]; t.base_weight[c] = a.p.eta * cw[s]; t.loss_chg[c] = 0.f; t.sum_hess[c] = (float)chh[s];
-    }
-    gs.node_sum[Lc].g = GLq; gs.node_sum[Lc].h = HLq; gs.node_sum[Rc].g = GRq; gs.node_sum[Rc].h = HRq;
-    gs.seg_begin[Lc] = 0; gs.seg_count[Lc] = 0; gs.seg_begin[Rc] = 0; gs.seg_count[Rc] = 0;   // set by part_kernel
-    if (children_evaluated) {               // build the child with the smaller hessian sum, subtract the sibling
+    expand_node(a, nid, best, tot, Lc, Rc, isg, ish);
+    if (children_evaluated) {
       int* nxt = gs.level_nodes + (size_t)(L + 1) * a.max_level_nodes;
       nxt[2 * r] = Lc; nxt[2 * r + 1] = Rc;
-      const bool fewer_right = HRq < HLq;
-      const int bld = fewer_right ? Rc : Lc, sub = fewer_right ? Lc : Rc;
-      gs.hist_slot[bld] = a.next_base + r; gs.hist_slot[sub] = a.next_base + a.next_half + r;
-      gs.build_nid[r] = bld; gs.build_sub_nid[r] = sub; gs.build_parent_slot[r] = gs.hist_slot[nid];
+      plan_child_hists(gs, r, nid, best, tot, Lc, Rc, a.next_base + r, a.next_base + a.next_half + r);
     }
   }
   __syncthreads();
@@ -361,32 +381,22 @@ __global__ void __launch_bounds__(256) apply_kernel(ApplyArgs a) {
 
 // ---------------------------------------------------------------------------------------------
 // grow_policy=lossguide: one node per iteration (upstream Driver::Pop in loss-guided mode: the open candidate with the largest
-// loss_chg, ties to the smaller node id; an INVALID top candidate ends the tree).  The per-level machinery is reused with
-// "level" 0 = the node being split and "level" 1 = its two children: this kernel (a) registers the candidates evaluated by the
-// previous iteration, (b) picks and validates the best one, (c) expands it exactly like apply_kernel does for a whole level.
+// loss_chg, ties to the smaller node id; an INVALID top candidate ends the tree).  Node expansion is shared with apply_kernel,
+// with "level" 0 = the node being split and "level" 1 = its two children: this kernel (a) registers the candidates evaluated by
+// the previous iteration, (b) picks and validates the best one, (c) expands it.
 // Histogram slots: the built child gets a fresh slot, its sibling inherits the parent's (subtract_kernel works in place).
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) apply_lossguide_kernel(ApplyArgs a, int iter) {
   __shared__ unsigned long long s_key[8];
-  GrowState& gs = a.gs; TreeArrays& t = a.tree;
+  GrowState& gs = a.gs;
   const double isg = (double)gs.scales[2], ish = (double)gs.scales[3];
   const int src = iter == 0 ? 0 : 1;
   const int cnt = gs.level_count[src];
   const int* nodes = gs.level_nodes + (size_t)src * a.max_level_nodes;
-  if (iter == 0 && threadIdx.x == 0 && cnt > 0) {
-    t.base_weight[0] = gs.weight[0]; t.sum_hess[0] = (float)((double)gs.node_sum[0].h * ish); t.split_cond[0] = a.p.eta * gs.weight[0];
-  }
+  if (iter == 0 && threadIdx.x == 0 && cnt > 0) finish_root(a, ish);
   for (int i = threadIdx.x; i < cnt; i += blockDim.x) {        // (a) Driver::Push: candidates with loss_chg > eps enter the queue
     const int nid = nodes[i];
-    SplitCand best = gs.best_group[(size_t)nid * a.ngroups];
-    unsigned long long bk = cand_key(best.loss_chg, best.feature, best.ord);
-    for (int g = 1; g < a.ngroups; ++g) {
-      SplitCand c = gs.best_group[(size_t)nid * a.ngroups + g];
-      unsigned long long k = cand_key(c.loss_chg, c.feature, c.ord);
-      if (k > bk) { bk = k; best = c; }
-    }
-    gs.best[nid] = best;
-    gs.open[nid] = best.loss_chg > 1e-6f ? 1 : 0;
+    gs.open[nid] = best_of_blocks(a, nid).loss_chg > 1e-6f ? 1 : 0;
   }
   __syncthreads();
   const int n0 = *gs.n_nodes;
@@ -404,12 +414,7 @@ __global__ void __launch_bounds__(256) apply_lossguide_kernel(ApplyArgs a, int i
   if (!stop) {
     nid = (int)(0xffffffffu - (unsigned)(key & 0xffffffffull));
     best = gs.best[nid]; tot = gs.node_sum[nid];
-    bool ok = best.loss_chg > 1e-6f;                                            // ExpandEntry::IsValid
-    if (ok && (best.HL == 0 || tot.h - best.HL == 0)) ok = false;
-    if (ok && best.loss_chg < a.p.gamma) ok = false;
-    if (ok && a.p.max_depth > 0 && gs.depth[nid] == a.p.max_depth) ok = false;
-    if (ok && a.p.max_leaves > 0 && *gs.n_leaves == a.p.max_leaves) ok = false;
-    stop = !ok;
+    stop = !split_is_valid(a.p, best, tot, gs.depth[nid]) || (a.p.max_leaves > 0 && *gs.n_leaves == a.p.max_leaves);
   }
   if (stop) {
     *gs.lg_done = 1;
@@ -418,31 +423,8 @@ __global__ void __launch_bounds__(256) apply_lossguide_kernel(ApplyArgs a, int i
   }
   gs.open[nid] = 0;                                            // (c) expand
   const int Lc = n0, Rc = n0 + 1, d = gs.depth[nid];
-  const long long GLq = best.GL, HLq = best.HL, GRq = tot.g - best.GL, HRq = tot.h - best.HL;
-  const double GL = (double)GLq * isg, HL = (double)HLq * ish, GR = (double)GRq * isg, HR = (double)HRq * ish;
-  float wl = calc_weight(a.p, GL, HL), wr = calc_weight(a.p, GR, HR);
-  if (a.monotone) {
-    const float lo = gs.lower[nid], hi = gs.upper[nid];
-    wl = clamp_weight(wl, lo, hi); wr = clamp_weight(wr, lo, hi);
-    const float mid = (wl + wr) / 2.0f; const int mc = a.monotone[best.feature];
-    gs.lower[Lc] = lo; gs.upper[Lc] = hi; gs.lower[Rc] = lo; gs.upper[Rc] = hi;
-    if (mc < 0) { gs.lower[Lc] = mid; gs.upper[Rc] = mid; } else if (mc > 0) { gs.upper[Lc] = mid; gs.lower[Rc] = mid; }
-  }
-  interaction_children(a, nid, best.feature, Lc, Rc);
-  const int cb = a.cut_ptrs[best.feature];
-  const float thr = best.dleft ? (best.bin < 0 ? a.min_vals[best.feature] : a.cut_vals[cb + best.bin]) : a.cut_vals[cb + best.bin];
-  t.left[nid] = Lc; t.right[nid] = Rc; t.split_index[nid] = best.feature; t.split_cond[nid] = thr;
-  t.split_bin[nid] = best.bin; t.default_left[nid] = (unsigned char)best.dleft;
-  t.base_weight[nid] = gs.weight[nid]; t.loss_chg[nid] = best.loss_chg; t.sum_hess[nid] = (float)((double)tot.h * ish);
-  const int ch[2] = {Lc, Rc}; const float cw[2] = {wl, wr}; const double chh[2] = {HL, HR};
-  for (int s = 0; s < 2; ++s) {
-    const int c = ch[s];
-    t.left[c] = -1; t.right[c] = -1; t.parent[c] = nid; t.split_index[c] = 0; t.split_bin[c] = -1; t.default_left[c] = 0;
-    t.split_cond[c] = a.p.eta * cw[s]; t.base_weight[c] = a.p.eta * cw[s]; t.loss_chg[c] = 0.f; t.sum_hess[c] = (float)chh[s];
-    gs.depth[c] = d + 1; gs.open[c] = 0;
-  }
-  gs.node_sum[Lc].g = GLq; gs.node_sum[Lc].h = HLq; gs.node_sum[Rc].g = GRq; gs.node_sum[Rc].h = HRq;
-  gs.seg_begin[Lc] = 0; gs.seg_count[Lc] = 0; gs.seg_begin[Rc] = 0; gs.seg_count[Rc] = 0;      // set by part_kernel
+  expand_node(a, nid, best, tot, Lc, Rc, isg, ish);
+  gs.depth[Lc] = d + 1; gs.depth[Rc] = d + 1; gs.open[Lc] = 0; gs.open[Rc] = 0;
   *gs.n_nodes = n0 + 2;
   const int leaves = *gs.n_leaves + 1;
   *gs.n_leaves = leaves;
@@ -454,11 +436,8 @@ __global__ void __launch_bounds__(256) apply_lossguide_kernel(ApplyArgs a, int i
   if (children_evaluated) {
     int* nxt = gs.level_nodes + (size_t)a.max_level_nodes;
     nxt[0] = Lc; nxt[1] = Rc; gs.level_count[1] = 2;
-    const bool fewer_right = HRq < HLq;
-    const int bld = fewer_right ? Rc : Lc, sub = fewer_right ? Lc : Rc;
     const int slot = (*gs.n_slots)++;
-    gs.hist_slot[bld] = slot; gs.hist_slot[sub] = gs.hist_slot[nid];
-    gs.build_nid[0] = bld; gs.build_sub_nid[0] = sub; gs.build_parent_slot[0] = gs.hist_slot[nid];
+    plan_child_hists(gs, 0, nid, best, tot, Lc, Rc, slot, gs.hist_slot[nid]);
     *gs.build_count = 1;
   } else { gs.level_count[1] = 0; *gs.build_count = 0; }
 }
@@ -725,8 +704,8 @@ __global__ void __launch_bounds__(256) subtract_kernel(GrowState gs, GH64* pool,
 // ---------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------
-void launch_init_tree(const GrowState& gs, const TreeArrays& t, unsigned n, int root_slot, int max_level_nodes, cudaStream_t s) {
-  init_tree_kernel<<<1, 32, 0, s>>>(gs, t, n, root_slot, max_level_nodes); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+void launch_init_tree(const GrowState& gs, const TreeArrays& t, unsigned n, cudaStream_t s) {
+  init_tree_kernel<<<1, 32, 0, s>>>(gs, t, n); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_scales(const GrowState& gs, int grad_bits, cudaStream_t s) { scales_kernel<<<1, 32, 0, s>>>(gs, grad_bits); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
 void launch_eval(const EvalArgs& a, int max_nodes_level, cudaStream_t s) {

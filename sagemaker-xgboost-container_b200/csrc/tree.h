@@ -21,7 +21,7 @@ struct EvalArgs {
 
 struct ApplyArgs {
   GrowState gs; TreeArrays tree; const int* cut_ptrs; const float* cut_vals; const float* min_vals;
-  TrainParamDev p; unsigned* scratch; int ngroups /* candidate blocks per node: groups + tail */, level, max_level_nodes, next_base, next_half;
+  TrainParamDev p; unsigned* scratch; int nblocks /* candidate blocks per node: groups + tail */, level, max_level_nodes, next_base, next_half;
   const int* monotone;            // as in EvalArgs
   // interaction constraints (upstream FeatureInteractionConstraintHost): per node the features used on its path and the features
   // it may split on ([cap_nodes][F] each), the constraint sets as a membership matrix [n_sets][F]
@@ -79,7 +79,7 @@ void launch_lg_stage(const GrowState& gs, GH64* pool, size_t slot_entries, int t
 void launch_hist_build(const HistArgs& a, int num_sms, cudaStream_t stream);
 void hist_configure();     // one-time function attributes (must happen outside stream capture)
 const char* hist_last_kernel();   // name of the kernel variant the last launch used (profiling / tests)
-void launch_init_tree(const GrowState& gs, const TreeArrays& t, unsigned n, int root_slot, int max_level_nodes, cudaStream_t s);
+void launch_init_tree(const GrowState& gs, const TreeArrays& t, unsigned n, cudaStream_t s);   // the root's histogram: slot kLgRootSlot
 void launch_scales(const GrowState& gs, int grad_bits, cudaStream_t s);
 void launch_eval(const EvalArgs& a, int max_nodes_level, cudaStream_t s);
 void launch_apply(const ApplyArgs& a, cudaStream_t s);
