@@ -173,6 +173,15 @@ XGB_DLL int XGB200BuildRootHistogram(BoosterHandle handle, DMatrixHandle dmat, c
 XGB_DLL int XGB200BuildHistogramEx(BoosterHandle handle, DMatrixHandle dmat, const float* gpair, int repeats, int mode,
                              const unsigned* row_ids, bst_ulong n_ids, int64_t* out_hist, float* scales, float* out_ms,
                              const char** out_kernel);
+/* split evaluation of one root, with the training path's kernels and arguments: `hist` is int64 [F][256][2] fixed point (g, h)
+ * on the grid launch_scales derives from max_g = max|g| and max_h = max h for the row count of `dmat`, which supplies the layout
+ * and the cuts (XGB200DMatrixSetCuts); (G, H) are the node totals in grid units, [lower, upper] the root's weight bounds (only
+ * read under monotone constraints), feat_mask (F bytes, 1 = usable; NULL = all) the tree's column set.  Runs init_tree,
+ * eval_kernel at level 0 and the grow_policy's expansion.  *out_json: {"scales": [4], "root_gain", "weight", "best_group":
+ * [per candidate block], "best", "n_nodes", "expanded", "tree": {the arrays of nodes 0 .. n_nodes-1}, "children": [{"G", "H",
+ * "lower", "upper"}]}; a candidate is {"loss_chg", "feature", "bin", "dleft", "ord", "GL", "HL"}; every float is its uint32 bits. */
+XGB_DLL int XGB200BoosterEvalRootSplit(BoosterHandle handle, DMatrixHandle dmat, const int64_t* hist, int64_t G, int64_t H, float max_g,
+                               float max_h, float lower, float upper, const uint8_t* feat_mask, const char** out_json);
 /* mean device time (CUDA events) of the predictor kernel alone over `repeats` launches on `dmat` */
 XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dmat, int repeats, float* out_ms);
 /* the predictor's plan for `dmat` and the rounds [iter_begin, iter_end) (iter_end == 0: all), without running it: JSON

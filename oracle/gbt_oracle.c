@@ -843,7 +843,8 @@ int orc_update_one_iter(OrcTrainer* t) {
     float mg = 0, mh = 0;
     for (int64_t i = 0; i < t->n * K; ++i) { mg = fmaxf(mg, fabsf(t->gpair[2 * i])); mh = fmaxf(mh, t->gpair[2 * i + 1]); }
     int eg, eh; frexpf(mg, &eg); frexpf(mh, &eh);      /* m < 2^e */
-    float sg = ldexpf(1.0f, t->quant_bits - 1 - eg), sh = ldexpf(1.0f, t->quant_bits - 1 - eh);
+    /* the product's scales_kernel with grad_bits = quant_bits - 1: |g_q| <= 2^grad_bits, h_q <= 2^(grad_bits + 1) */
+    float sg = ldexpf(1.0f, t->quant_bits - 1 - eg), sh = ldexpf(1.0f, t->quant_bits - eh);
     for (int64_t i = 0; i < t->n * K; ++i) {
       t->gpair[2 * i] = rintf(t->gpair[2 * i] * sg) / sg;
       t->gpair[2 * i + 1] = rintf(t->gpair[2 * i + 1] * sh) / sh;

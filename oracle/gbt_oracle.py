@@ -24,8 +24,15 @@ OBJECTIVES = {
 def build(force=False):
     """Compile the oracle with gcc (recipe committed here; output is git-ignored)."""
     if force or not os.path.exists(_SO) or os.path.getmtime(_SO) < os.path.getmtime(_SRC):
-        subprocess.check_call(["gcc", "-O3", "-fopenmp", "-fPIC", "-shared", "-o", _SO, _SRC, "-lm"])
+        # -ffp-contract=off: the split gains round every product before the add, as upstream's CPU code (and the product) do;
+        # a compiler that fuses them (gcc on aarch64 does by default) would move loss_chg by an ulp
+        subprocess.check_call(["gcc", "-O3", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", "-o", _SO, _SRC, "-lm"])
     return _SO
+
+
+class OrcSplit(C.Structure):
+    _fields_ = [("loss_chg", C.c_float), ("findex", C.c_int32), ("split_value", C.c_float), ("split_bin", C.c_int32),
+                ("default_left", C.c_int32), ("GL", C.c_double), ("HL", C.c_double), ("GR", C.c_double), ("HR", C.c_double)]
 
 
 class OrcParams(C.Structure):
@@ -84,6 +91,8 @@ def lib():
         L.orc_set_monotone.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         L.orc_set_interaction.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         L.orc_set_margins.argtypes = [C.c_void_p, C.c_void_p]
+        L.orc_eval_split.argtypes = [C.POINTER(OrcParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                     C.c_double, C.c_double, C.c_float, C.POINTER(OrcSplit)]
         _lib = L
     return _lib
 
@@ -189,6 +198,21 @@ def build_hist_fixed(bins, gq, hq, rows=None):
     return hist
 
 
+def eval_split(params, hist, cut_ptrs, cut_vals, min_vals, G, H, root_gain, feat_mask=None):
+    """Best unconstrained split of one node (EnumerateSplit over every feature): hist is (total_bins, 2) float64 (g, h), G, H
+    the node totals, root_gain its float gain.  Returns the oracle's Split as a dict."""
+    p = make_params(params)
+    hist = np.ascontiguousarray(hist, np.float64)
+    ptrs = np.ascontiguousarray(cut_ptrs, np.int32)
+    vals = np.ascontiguousarray(cut_vals, np.float32)
+    mins = np.ascontiguousarray(min_vals, np.float32)
+    mask = None if feat_mask is None else np.ascontiguousarray(feat_mask, np.uint8)
+    out = OrcSplit()
+    lib().orc_eval_split(C.byref(p), _p(hist), _p(ptrs), _p(vals), _p(mins), len(ptrs) - 1, _p(mask), float(G), float(H),
+                         C.c_float(root_gain), C.byref(out))
+    return {k: getattr(out, k) for k, _ in OrcSplit._fields_}
+
+
 class Model(dict):
     """Flat tree arrays: tree_offset, tree_info, left, right, parent, split_index, split_bin,
     default_left, split_cond, base_weight, loss_chg, sum_hess + base_score, num_class, num_feature."""
@@ -256,8 +280,15 @@ class Trainer:
         return max(1, self.p.num_class)
 
     def set_quant_bits(self, bits):
-        """Study knob: emulate the product's fixed-point gradient grid (0 = reference behaviour)."""
+        """Study knob: emulate the product's fixed-point gradient grid with `bits` - 1 magnitude bits of g (0 = reference
+        behaviour): g is rounded to 2^(bits - 1 - eg), h to 2^(bits - eh), as the product's scales_kernel does."""
         lib().orc_set_quant_bits(self.h, int(bits))
+
+    def set_device_grid(self, n=None):
+        """The grid the product trains `n` rows (default: this trainer's) on: 21 magnitude bits up to 2^20 rows, 18 above
+        (csrc/engine.h grad_bits_for)."""
+        n = self.n if n is None else int(n)
+        self.set_quant_bits((21 if n <= (1 << 20) else 18) + 1)
 
     def set_margins(self, m):
         m = np.ascontiguousarray(m, np.float32).reshape(self.n, self.K)

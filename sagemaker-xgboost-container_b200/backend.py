@@ -401,6 +401,17 @@ class CudaBackend:
                                                     scales.ctypes.data_as(C.POINTER(C.c_float)), C.byref(ms), C.byref(name)))
         return hist, scales, float(ms.value), (name.value or b"").decode()
 
+    def eval_root_split(self, bh, dh, hist, G, H, max_g, max_h, lower=float("-inf"), upper=float("inf"), feat_mask=None):
+        """Split evaluation of one root from an int64 [F][256][2] histogram (include/b200xgb.h XGB200BoosterEvalRootSplit):
+        a dict whose floats are uint32 bit patterns."""
+        hist = np.ascontiguousarray(hist, np.int64)
+        mask = None if feat_mask is None else np.ascontiguousarray(feat_mask, np.uint8)
+        out = C.c_char_p()
+        self._check(self.lib.XGB200BoosterEvalRootSplit(bh, dh, hist.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int64(int(G)), C.c_int64(int(H)),
+                                                        C.c_float(max_g), C.c_float(max_h), C.c_float(lower), C.c_float(upper),
+                                                        None if mask is None else mask.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(out)))
+        return json.loads(out.value.decode())
+
     def booster_predict_kernel_ms(self, bh, dh, repeats=5):
         ms = C.c_float()
         self._check(self.lib.XGB200BoosterPredictKernelMs(bh, dh, C.c_int(repeats), C.byref(ms)))

@@ -419,6 +419,42 @@ static HistArgs hist_args(const GrowerImpl& g, const BinnedMatrix& bm, int k) {
   return ha;
 }
 
+// Split evaluation of the nodes of `level` (their histograms are in the pool).  feat_mask: the level's column set or nullptr;
+// sampling: the tree samples columns (colsample_bynode then picks each node's subset inside feat_mask); mono: the per-feature
+// monotone constraints on the device or nullptr; ic_on: interaction constraints (GrowerImpl::ic_allowed).  Training
+// (enqueue_tree) and the kernel-level entry point (Booster::debug_eval_root) both start from here.
+static EvalArgs eval_args(const GrowerImpl& g, const BinnedMatrix& bm, const DMatrix& dm, const TrainParam& p, const int* mono, bool ic_on,
+                          bool sampling, int level, const unsigned char* feat_mask) {
+  EvalArgs ea{}; ea.hist_pool = g.hist_pool.p; ea.gs = g.gs; ea.cut_ptrs = dm.d_cut_ptrs.p; ea.feat_mask = feat_mask; ea.p = to_dev(p); ea.F = bm.F;
+  ea.ngroups = bm.ngroups; ea.tw = bm.tw; ea.ntail = bm.ntail; ea.has_missing = bm.has_missing; ea.level = level; ea.max_level_nodes = g.max_level_nodes;
+  ea.colsample_bynode = sampling ? p.colsample_bynode : 1.0f; ea.seed = p.seed; ea.tree_index = g.tree_index_dev.p; ea.monotone = mono;
+  ea.node_allowed = ic_on ? g.ic_allowed.p : nullptr;
+  return ea;
+}
+// Expansion of the nodes of `level`; next_base, next_half: the children's histogram slots (depth-wise).  n_ic: interaction
+// constraint sets (0 = none).
+static ApplyArgs apply_args(const GrowerImpl& g, const BinnedMatrix& bm, const DMatrix& dm, const TrainParam& p, const int* mono, int n_ic,
+                            int level, int next_base, int next_half) {
+  ApplyArgs aa{}; aa.gs = g.gs; aa.tree = g.ta; aa.cut_ptrs = dm.d_cut_ptrs.p; aa.cut_vals = dm.d_cut_vals.p; aa.min_vals = dm.d_min_vals.p;
+  aa.p = to_dev(p); aa.scratch = g.scratch.p; aa.nblocks = bm.ngroups + (bm.tw > 0 ? 1 : 0); aa.level = level; aa.max_level_nodes = g.max_level_nodes;
+  aa.next_base = next_base; aa.next_half = next_half; aa.monotone = mono;
+  if (n_ic > 0) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = n_ic; aa.F = bm.F; }
+  return aa;
+}
+
+// the monotone constraints in device memory (padded with 0 to the feature count; re-uploaded when they or F change), or nullptr
+static const int* monotone_on_device(GrowerImpl& g, const std::vector<int>& mono, int F, cudaStream_t s) {
+  if (mono.empty()) return nullptr;
+  std::vector<int> mh(mono); mh.resize((size_t)std::max<int>(F, (int)mh.size()), 0);
+  if (mh != g.monotone_host || g.monotone_dev.n < mh.size()) {
+    g.monotone_dev.ensure(mh.size());
+    CUDA_OK(cudaMemcpyAsync(g.monotone_dev.p, mh.data(), sizeof(int) * mh.size(), cudaMemcpyHostToDevice, s));
+    Comm::get().sync_stream(s);
+    g.monotone_host = mh;
+  }
+  return g.monotone_dev.p;
+}
+
 constexpr int kRootRows = -1;     // the partition's input at the root: every row in order, the float2 gpair and the tail words by row
 
 // Column sampling (upstream src/common/random.h ColumnSampler: bytree, then bylevel inside it, then bynode inside that; a
@@ -696,6 +732,10 @@ static void check_labels(const DMatrix* dm) {
   B200_CHECK(dm->labels.size() == (size_t)dm->n, "Check failed: preds.size() == info.labels_.size() (" + std::to_string(dm->n) + " vs. " +
              std::to_string(dm->labels.size()) + ") : labels are not correctly provided");
 }
+static void check_train_width(const DMatrix* dm) {
+  B200_CHECK(dm->F <= kMaxTrainFeatures, "the CUDA hist builder trains on at most " + std::to_string(kMaxTrainFeatures) + " features (the data has " +
+             std::to_string(dm->F) + ")");
+}
 
 void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   configure();
@@ -706,6 +746,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
              " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
   B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
+  check_train_width(dtrain);
   dtrain->ensure_binned(param_.max_bin);
   const int K = param_.num_class;
   if (!grower_) grower_ = new GrowerImpl();
@@ -750,7 +791,6 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
   Comm& comm = Comm::get();
   const int K = param_.num_class;
   const int D = param_.max_depth;
-  const TrainParamDev pd = to_dev(param_);
   const BinnedMatrix bm = dtrain->binned_view();
   const int num_sms = engine_num_sms();
   const unsigned max_tiles = (unsigned)((dtrain->n + kPartTile - 1) / kPartTile) + g.max_level_nodes + 1;
@@ -808,17 +848,11 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
   }
   // The argument blocks of this tree's kernels, each filled in one place.  The two growth policies below pass only their own data:
   // the level, the buffer sets and the feature mask.
-  auto eval_args = [&](int level, const unsigned char* feat_mask) {
-    EvalArgs ea{}; ea.hist_pool = g.hist_pool.p; ea.gs = g.gs; ea.cut_ptrs = dtrain->d_cut_ptrs.p; ea.feat_mask = feat_mask; ea.p = pd; ea.F = bm.F;
-    ea.ngroups = bm.ngroups; ea.tw = bm.tw; ea.ntail = bm.ntail; ea.has_missing = bm.has_missing; ea.level = level; ea.max_level_nodes = g.max_level_nodes;
-    ea.colsample_bynode = mask ? param_.colsample_bynode : 1.0f; ea.seed = param_.seed; ea.tree_index = g.tree_index_dev.p; ea.monotone = mono_dev; ea.node_allowed = ic_on ? g.ic_allowed.p : nullptr;
-    return ea;
+  auto eval_at = [&](int level, const unsigned char* feat_mask) {
+    return eval_args(g, bm, *dtrain, param_, mono_dev, ic_on, mask != nullptr, level, feat_mask);
   };
-  auto apply_args = [&](int level, int next_base, int next_half) {     // next_base, next_half: the children's histogram slots (depth-wise)
-    ApplyArgs aa{}; aa.gs = g.gs; aa.tree = g.ta; aa.cut_ptrs = dtrain->d_cut_ptrs.p; aa.cut_vals = dtrain->d_cut_vals.p; aa.min_vals = dtrain->d_min_vals.p;
-    aa.p = pd; aa.scratch = g.scratch.p; aa.nblocks = bm.ngroups + (bm.tw > 0 ? 1 : 0); aa.level = level; aa.max_level_nodes = g.max_level_nodes; aa.next_base = next_base; aa.next_half = next_half; aa.monotone = mono_dev;
-    if (ic_on) { aa.node_path = g.ic_path.p; aa.node_allowed = g.ic_allowed.p; aa.ic_sets = g.ic_sets.p; aa.n_ic_sets = (int)interaction_.size(); aa.F = bm.F; }
-    return aa;
+  auto apply_at = [&](int level, int next_base, int next_half) {
+    return apply_args(g, bm, *dtrain, param_, mono_dev, (int)interaction_.size(), level, next_base, next_half);
   };
   auto part_args = [&](int level, int cur, int next) {                  // the partition of `level` from buffer set `cur` into set `next`
     const bool root = cur == kRootRows;
@@ -837,11 +871,11 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     ha.rows_counter = profile_ ? prof_rows_.p + 1 : nullptr;
     return ha;
   };
-  launch_eval(eval_args(0, mask), 1, s);
+  launch_eval(eval_at(0, mask), 1, s);
 
   const int lg_iters = lossguide_iters(param_);
   for (int it = 0; it < lg_iters; ++it) {                 // grow_policy=lossguide: one expansion per iteration (tree.cu apply_lossguide_kernel)
-    launch_apply_lossguide(apply_args(0, 0, 0), it, s);
+    launch_apply_lossguide(apply_at(0, 0, 0), it, s);
     // live row segments always sit in buffer set 0; the partition writes the children into set 1 and they are copied straight back
     const PartArgs pa = part_args(0, it == 0 ? kRootRows : 0, 1);
     prof_begin(kProfPartition);
@@ -858,13 +892,13 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
       launch_lg_stage(g.gs, g.hist_pool.p, g.slot_stride, 0, s);
     }
     launch_subtract(g.gs, g.hist_pool.p, g.slot_stride, 1, s);
-    launch_eval(eval_args(1, nullptr), 2, s);
+    launch_eval(eval_at(1, nullptr), 2, s);
   }
 
   for (int L = 0; L < D && lg_iters == 0; ++L) {
     const bool final_level = (L == D - 1);
     const int next_base = ((L + 1) & 1) * g.region, next_half = 1 << L;
-    launch_apply(apply_args(L, next_base, next_half), s);
+    launch_apply(apply_at(L, next_base, next_half), s);
     if (final_level) break;                  // children of the last level are leaves: no partition, no histograms
     PartArgs pa = part_args(L, L == 0 ? kRootRows : (L & 1) ^ 1, L & 1);     // the buffer sets alternate
     pa.build_only = L == D - 2 ? 1 : 0;                    // the next level is the last one: only the built children are read again
@@ -878,7 +912,7 @@ void Booster::enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned
     prof_end();
     allreduce_hist(g.hist_pool.p + (size_t)next_base * g.slot_stride, (size_t)next_half * g.slot_stride * 2);
     launch_subtract(g.gs, g.hist_pool.p, g.slot_stride, next_half, s);
-    launch_eval(eval_args(L + 1, mask ? mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
+    launch_eval(eval_at(L + 1, mask ? mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
   }
 
   // prediction cache += leaf values of this tree: one row-order pass over the column-major bins
@@ -908,15 +942,7 @@ void Booster::grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_i
     Comm::get().sync_stream(s);
     mask = g.feat_mask.p;
   }
-  if (!monotone_.empty()) {                     // per-feature constraints in device memory (padded with 0 to the feature count)
-    std::vector<int> mh(monotone_); mh.resize((size_t)std::max<int>(dtrain->F, (int)mh.size()), 0);
-    if (mh != g.monotone_host || g.monotone_dev.n < mh.size()) {
-      g.monotone_dev.ensure(mh.size());
-      CUDA_OK(cudaMemcpyAsync(g.monotone_dev.p, mh.data(), sizeof(int) * mh.size(), cudaMemcpyHostToDevice, s));
-      Comm::get().sync_stream(s);
-      g.monotone_host = mh;
-    }
-  }
+  monotone_on_device(g, monotone_, dtrain->F, s);
   if (!interaction_.empty()) {                  // constraint sets as a membership matrix, per-node path / allowed flags
     const size_t F = (size_t)dtrain->F;
     std::vector<unsigned char> sets(interaction_.size() * F, 0);
@@ -1216,6 +1242,93 @@ void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::v
   CUDA_OK(cudaMemcpyAsync(scales_out, g.gs.scales, 4 * sizeof(float), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
   cudaEventDestroy(e0); cudaEventDestroy(e1);
+}
+
+// Kernel-level entry point for split evaluation: the root of a tree whose histogram is hist_fm ([F][256]{g,h}, int64 fixed point)
+// with node totals (G, H) on the grid that launch_scales derives from max_g, max_h for dm's row count; lower / upper bound the
+// root's weight (monotone constraints); feat_mask (F bytes, nullptr = all) is the tree's column set.  Runs init_tree, eval_kernel
+// at level 0 and the booster's grow_policy expansion with the training path's arguments, and returns JSON (floats as uint32 bits).
+std::string Booster::debug_eval_root(DMatrix* dm, const long long* hist_fm, long long G, long long H, float max_g, float max_h,
+                                     float lower, float upper, const unsigned char* feat_mask) {
+  configure();
+  cudaStream_t s = engine_stream();
+  check_train_width(dm);
+  B200_CHECK(interaction_.empty(), "debug_eval_root: interaction constraints are not supported");
+  dm->ensure_binned(param_.max_bin);
+  if (!grower_) grower_ = new GrowerImpl();
+  GrowerImpl& g = *grower_;
+  g.ensure(dm->n, dm->ngroups, dm->tw, tail_by_position(dm->binned_view()), param_.max_depth, param_.num_class, lossguide_iters(param_));
+  g.root_h_valid = false;                       // the root slot is overwritten
+  const BinnedMatrix bm = dm->binned_view();
+  const int F = bm.F;
+  // the histogram in pool layout: [group][bin][slot] then the tail [bin][tw]
+  std::vector<GH64> slot(g.slot_stride, GH64{0, 0});
+  const size_t W = (size_t)bm.ngroups * kSlots, tail0 = (size_t)bm.ngroups * kGroupEntries;
+  for (int f = 0; f < F; ++f)
+    for (int b = 0; b < kBins; ++b) {
+      const size_t e = (size_t)f < W ? ((size_t)(f / kSlots) * kBins + b) * kSlots + f % kSlots : tail0 + (size_t)b * bm.tw + (f - W);
+      slot[e].g = hist_fm[((size_t)f * kBins + b) * 2]; slot[e].h = hist_fm[((size_t)f * kBins + b) * 2 + 1];
+    }
+  const bool sampling = feat_mask != nullptr || param_.colsample_bynode < 1.0f;
+  if (sampling) {
+    g.feat_mask.ensure((size_t)F); g.tree_index_dev.ensure(1);
+    std::vector<unsigned char> m((size_t)F, 1);
+    if (feat_mask) m.assign(feat_mask, feat_mask + F);
+    const int tree_index = 0;
+    CUDA_OK(cudaMemcpyAsync(g.feat_mask.p, m.data(), (size_t)F, cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(g.tree_index_dev.p, &tree_index, sizeof(int), cudaMemcpyHostToDevice, s));
+    Comm::get().sync_stream(s);
+  }
+  const int* mono = monotone_on_device(g, monotone_, F, s);
+  launch_init_tree(g.gs, g.ta, (unsigned)dm->n, s);
+  CUDA_OK(cudaMemcpyAsync(g.hist_pool.p, slot.data(), sizeof(GH64) * g.slot_stride, cudaMemcpyHostToDevice, s));
+  const GH64 tot{G, H};
+  CUDA_OK(cudaMemcpyAsync(g.gs.node_sum, &tot, sizeof tot, cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(g.gs.lower, &lower, 4, cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(g.gs.upper, &upper, 4, cudaMemcpyHostToDevice, s));
+  unsigned am[2]; memcpy(&am[0], &max_g, 4); memcpy(&am[1], &max_h, 4);
+  CUDA_OK(cudaMemcpyAsync(g.gs.absmax, am, 8, cudaMemcpyHostToDevice, s));
+  launch_scales(g.gs, job_grad_bits(g.global_n), s);
+  launch_eval(eval_args(g, bm, *dm, param_, mono, false, sampling, 0, sampling ? g.feat_mask.p : nullptr), 1, s);
+  const ApplyArgs aa = apply_args(g, bm, *dm, param_, mono, 0, 0, g.region, 1);
+  if (param_.lossguide) launch_apply_lossguide(aa, 0, s); else launch_apply(aa, s);
+  // read back
+  const int nblocks = bm.ngroups + (bm.tw > 0 ? 1 : 0);
+  float scales[4], root_gain, weight, lo[3], hi[3];
+  std::vector<SplitCand> groups((size_t)nblocks); SplitCand best; GH64 sums[3];
+  std::vector<unsigned char> tb(g.tree_block_bytes);
+  CUDA_OK(cudaMemcpyAsync(scales, g.gs.scales, sizeof scales, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(&root_gain, g.gs.root_gain, 4, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(&weight, g.gs.weight, 4, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(groups.data(), g.gs.best_group, sizeof(SplitCand) * nblocks, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(&best, g.gs.best, sizeof best, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(sums, g.gs.node_sum, sizeof sums, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(lo, g.gs.lower, sizeof lo, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(hi, g.gs.upper, sizeof hi, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(tb.data(), g.tree_block.p, tb.size(), cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
+  auto bits = [](float v) { unsigned u; memcpy(&u, &v, 4); return std::to_string(u); };
+  auto cand = [&](const SplitCand& c) {
+    return "{\"loss_chg\":" + bits(c.loss_chg) + ",\"feature\":" + std::to_string(c.feature) + ",\"bin\":" + std::to_string(c.bin) + ",\"dleft\":" +
+           std::to_string(c.dleft) + ",\"ord\":" + std::to_string(c.ord) + ",\"GL\":" + std::to_string(c.GL) + ",\"HL\":" + std::to_string(c.HL) + "}";
+  };
+  const int nn = *(const int*)tb.data(); const size_t N = (size_t)g.cap_nodes;
+  const int* ip = (const int*)(tb.data() + 64); const float* fp = (const float*)(ip + 5 * N); const unsigned char* up = (const unsigned char*)(fp + 4 * N);
+  std::string o = "{\"scales\":[";
+  for (int i = 0; i < 4; ++i) o += (i ? "," : "") + bits(scales[i]);
+  o += "],\"root_gain\":" + bits(root_gain) + ",\"weight\":" + bits(weight) + ",\"best_group\":[";
+  for (int i = 0; i < nblocks; ++i) o += (i ? "," : "") + cand(groups[i]);
+  o += "],\"best\":" + cand(best) + ",\"n_nodes\":" + std::to_string(nn) + ",\"expanded\":" + (nn == 3 ? "true" : "false") + ",\"tree\":{";
+  const char* iname[5] = {"left", "right", "parent", "split_index", "split_bin"};
+  const char* fname[4] = {"split_cond", "base_weight", "loss_chg", "sum_hess"};
+  for (int a = 0; a < 5; ++a) { o += std::string(a ? "," : "") + "\"" + iname[a] + "\":["; for (int i = 0; i < nn; ++i) o += (i ? "," : "") + std::to_string(ip[a * N + i]); o += "]"; }
+  for (int a = 0; a < 4; ++a) { o += std::string(",\"") + fname[a] + "\":["; for (int i = 0; i < nn; ++i) o += (i ? "," : "") + bits(fp[a * N + i]); o += "]"; }
+  o += ",\"default_left\":["; for (int i = 0; i < nn; ++i) o += (i ? "," : "") + std::to_string((int)up[i]); o += "]}";
+  o += ",\"children\":[";
+  for (int c = 1; c < nn && c < 3; ++c)
+    o += std::string(c > 1 ? "," : "") + "{\"G\":" + std::to_string(sums[c].g) + ",\"H\":" + std::to_string(sums[c].h) + ",\"lower\":" + bits(lo[c]) + ",\"upper\":" + bits(hi[c]) + "}";
+  o += "]}";
+  return o;
 }
 
 // pred_contribs: path-dependent Tree SHAP on the device (shap.cu); output [n][F + 1], or [n][K][F + 1] for multi-class models

@@ -125,6 +125,10 @@ class Booster {
   // row_ids (optional, n_ids entries): histogram of that row subset, gpair given by POSITION -> exercises the gathered path.
   void debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::vector<long long>* hist_out, float* scales_out,
                              int repeats, float* ms_out, int mode = 0, const unsigned* row_ids = nullptr, int64_t n_ids = 0);
+  // split evaluation and expansion of a root with the given histogram ([F][256]{g,h} int64) and totals, JSON of every result
+  // (include/b200xgb.h XGB200BoosterEvalRootSplit)
+  std::string debug_eval_root(DMatrix* dm, const long long* hist_fm, long long G, long long H, float max_g, float max_h,
+                              float lower, float upper, const unsigned char* feat_mask);
 
  private:
   friend struct GrowerImpl;

@@ -514,6 +514,12 @@ int XGB200BuildHistogramEx(BoosterHandle handle, DMatrixHandle dmat, const float
   if (out_kernel) *out_kernel = hist_last_kernel();
   API_END();
 }
+int XGB200BoosterEvalRootSplit(BoosterHandle handle, DMatrixHandle dmat, const int64_t* hist, int64_t G, int64_t H, float max_g, float max_h,
+                               float lower, float upper, const uint8_t* feat_mask, const char** out_json) {
+  API_BEGIN(); BoosterBox* box = static_cast<BoosterBox*>(handle);
+  box->ret_str = BST(handle)->debug_eval_root(DM(dmat), reinterpret_cast<const long long*>(hist), G, H, max_g, max_h, lower, upper, feat_mask);
+  *out_json = box->ret_str.c_str(); API_END();
+}
 int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dmat, int repeats, float* out_ms) {
   API_BEGIN();
   *out_ms = BST(handle)->debug_predict_kernel_ms(DM(dmat), repeats);

@@ -53,6 +53,10 @@ constexpr int64_t kSmallMatrixRows = 1 << 20;
 inline int grad_bits_for(int64_t n) { return n <= kSmallMatrixRows ? kGradBitsSmall : kGradBits; }
 inline int window_rows_for(int64_t n) { return n <= kSmallMatrixRows ? kWindowRowsSmall : kWindowRows; }
 constexpr int kMaxDepth = 16;
+// Widest training matrix: eval_kernel runs one block row per feature group (+ the tail block) in grid.y (<= 65535), and the
+// split key (tree.cu cand_key) holds 23 bits of feature id.
+constexpr int kMaxTrainFeatures = 65534 * 32;
+static_assert(kMaxTrainFeatures < (1 << 23), "cand_key holds 23 bits of feature id");
 
 struct GH64 { long long g, h; };      // exact fixed-point gradient/hessian sums
 

@@ -223,6 +223,9 @@ __global__ void __launch_bounds__(256) predict_kernel(PredictArgs a) {
 // against 4*F bytes: beyond T*D ~ 100 the kernel is issue-bound, not HBM-bound (DESIGN.md "predictor").
 struct PNode { float cond; unsigned w; };            // w = left child (16 bit, 0xffff = leaf) | feature << 16 | default_left << 31
 
+// PNode::w keeps 15 bits of feature id: the plan tiles only matrices of at most kPredictMaxPitch features
+static_assert(kPredictMaxPitch <= 0x7fff + 1, "the tiled predictor's feature field has 15 bits");
+
 template <bool HAS_NAN, bool LEAF_OUT>
 __global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, int tree_lo, int tree_hi, int pitch, int rows_per_tile, int64_t num_tiles) {
   extern __shared__ __align__(16) unsigned char psm[];

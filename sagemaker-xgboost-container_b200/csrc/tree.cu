@@ -23,11 +23,15 @@ __device__ __forceinline__ float calc_weight(const TrainParamDev& p, double G, d
   if (p.max_delta_step != 0.0f && fabs(dw) > p.max_delta_step) dw = copysign((double)p.max_delta_step, dw);
   return (float)dw;
 }
+// -(2 g w + (h + lambda) w^2) in float with every product rounded before the add, as upstream's CPU code evaluates it: a fused
+// multiply-add would change the last bits of loss_chg, and at near-ties which split wins
+__device__ __forceinline__ float gain_at_weight_f(float g, float h, float lambda, float w) {
+  return -__fadd_rn(__fmul_rn(__fmul_rn(2.0f, g), w), __fmul_rn(__fmul_rn(__fadd_rn(h, lambda), w), w));
+}
 __device__ __forceinline__ float calc_gain_given_weight(const TrainParamDev& p, double G, double H, float w) {
   if (H <= 0.0) return 0.0f;
   if (p.max_delta_step == 0.0f) { double t = threshold_l1(G, p.alpha); return (float)(t * t / (H + p.lambda)); }
-  float g = (float)G, h = (float)H;
-  return -(2.0f * g * w + (h + p.lambda) * w * w);
+  return gain_at_weight_f((float)G, (float)H, p.lambda, w);
 }
 __device__ __forceinline__ float calc_gain(const TrainParamDev& p, double G, double H) {
   return calc_gain_given_weight(p, G, H, calc_weight(p, G, H));
@@ -62,8 +66,7 @@ __device__ __forceinline__ void interaction_children(const ApplyArgs& a, int nid
 __device__ __forceinline__ float clamp_weight(float w, float lo, float hi) { return w < lo ? lo : (w > hi ? hi : w); }
 __device__ __forceinline__ float gain_at_weight(const TrainParamDev& p, double G, double H, float w) {
   if (H <= 0.0) return 0.0f;
-  const float g = (float)G, h = (float)H;
-  return -(2.0f * g * w + (h + p.lambda) * w * w);
+  return gain_at_weight_f((float)G, (float)H, p.lambda, w);
 }
 // gain of a candidate under constraints; returns false when it violates the feature's constraint c
 __device__ __forceinline__ bool constrained_split_gain(const TrainParamDev& p, double GL, double HL, double GR, double HR, float lo, float hi, int c, float* gain) {
@@ -74,10 +77,11 @@ __device__ __forceinline__ bool constrained_split_gain(const TrainParamDev& p, d
 
 // Total order of candidates == upstream SplitEntry::NeedReplace: larger loss_chg, then lower feature,
 // then earlier position in scan order (forward bins ascending, then backward bins descending).
+// Key: 32 bits of loss | 23 bits of inverted feature | 9 bits of inverted ord (ord < 512); features below kMaxSplitFeatures.
 __device__ __forceinline__ unsigned long long cand_key(float loss, int f, int ord) {
   if (!(loss > 0.0f) || isinf(loss)) return 0ull;
-  return ((unsigned long long)__float_as_uint(loss) << 32) | ((unsigned long long)(0xFFFFu - (unsigned)f) << 16) |
-         (unsigned long long)(0xFFFFu - (unsigned)ord);
+  return ((unsigned long long)__float_as_uint(loss) << 32) | ((unsigned long long)(0x7FFFFFu - (unsigned)f) << 9) |
+         (unsigned long long)(0x1FFu - (unsigned)ord);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -634,9 +638,11 @@ __global__ void __launch_bounds__(256, GONLY ? (TL ? 5 : 6) : 4) part_kernel(Par
 
 // Prediction-cache update of a finished tree: one streaming pass in ROW order over the column-major bins
 // (coalesced, no scattered read-modify-write of the cache).  The tree is packed into shared memory first
-// (8 B per node) so that a traversal step costs one LDS + one global byte load.
-struct PackedNode { unsigned short feat_dl; unsigned short bin_plus1; unsigned short left, right; };   // feat | dl << 15; left == 0xffff: leaf
+// (8 B per node) so that a traversal step costs one LDS + one global byte load.  The feature id keeps all its bits; the right
+// child is left + 1 (both growth policies allocate the children as an adjacent pair).
+struct PackedNode { unsigned feat; unsigned short bin_dl; unsigned short left; };   // bin_dl: (split_bin + 1) | dl << 15; left == 0xffff: leaf
 constexpr int kPackedNodesSmem = 2048;
+static_assert(sizeof(PackedNode) == 8, "PackedNode is 8 B");
 
 __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing,
                                                             float* margin, int K, int k) {
@@ -646,8 +652,8 @@ __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const 
   const bool packed = nn <= kPackedNodesSmem && nn < 0xffff;
   if (packed) {
     for (int i = threadIdx.x; i < nn; i += blockDim.x) {
-      PackedNode p; p.feat_dl = (unsigned short)(t.split_index[i] | (t.default_left[i] ? 0x8000 : 0)); p.bin_plus1 = (unsigned short)(t.split_bin[i] + 1);
-      const int l = t.left[i]; p.left = l < 0 ? 0xffff : (unsigned short)l; p.right = l < 0 ? 0xffff : (unsigned short)t.right[i];
+      PackedNode p; p.feat = (unsigned)t.split_index[i]; p.bin_dl = (unsigned short)((t.split_bin[i] + 1) | (t.default_left[i] ? 0x8000 : 0));
+      const int l = t.left[i]; p.left = l < 0 ? 0xffff : (unsigned short)l;
       s_nodes[i] = p; s_leaf[i] = t.split_cond[i];
     }
     __syncthreads();
@@ -663,7 +669,7 @@ __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const 
     int byte[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const int f = packed ? (int)(s_nodes[nid[j]].feat_dl & 0x7fff) : t.split_index[nid[j]];
+      const int f = packed ? (int)s_nodes[nid[j]].feat : t.split_index[nid[j]];
       byte[j] = done[j] ? 0 : bins_col[(int64_t)f * n + base + j * 256];
     }
     any = false;
@@ -673,8 +679,8 @@ __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const 
       const int nd = nid[j];
       if (packed) {
         const PackedNode p = s_nodes[nd];
-        const bool left = (has_missing && byte[j] == kMissingBin) ? ((p.feat_dl & 0x8000) != 0) : (byte[j] < (int)p.bin_plus1);
-        nid[j] = left ? p.left : p.right;
+        const bool left = (has_missing && byte[j] == kMissingBin) ? ((p.bin_dl & 0x8000) != 0) : (byte[j] < (int)(p.bin_dl & 0x7fff));
+        nid[j] = left ? p.left : p.left + 1;
         done[j] = s_nodes[nid[j]].left == 0xffff;
       } else {
         const bool left = (has_missing && byte[j] == kMissingBin) ? (t.default_left[nd] != 0) : (byte[j] <= t.split_bin[nd]);
