@@ -5,13 +5,12 @@
 #include <string>
 #include <vector>
 #include "engine.h"
+#include "grow.h"
 #include "json.h"
 #include "misc.h"
 #include "tree.h"
 
 namespace b200 {
-
-cudaStream_t engine_stream();
 
 // ---------------------------------------------------------------------------------------------
 // DMatrix: features resident on the device (raw float row-major + lazily the binned feature blocks)
@@ -67,10 +66,6 @@ struct HostTree {
   std::vector<uint8_t> default_left;
   std::vector<float> split_cond, base_weight, loss_chg, sum_hess;
   int num_nodes() const { return (int)left.size(); }
-};
-
-struct PendingTree {            // a tree still on its way from the device (async copy into pinned memory)
-  void* staging = nullptr; size_t cap_nodes = 0; cudaEvent_t ready = nullptr;
 };
 
 struct PredCache { DevBuf<float> margin; int trees_applied = 0; int64_t n = 0; uint64_t model_version = 0; };
@@ -131,7 +126,6 @@ class Booster {
                               float lower, float upper, const unsigned char* feat_mask);
 
  private:
-  friend struct GrowerImpl;
   PredictArgs predict_args(DMatrix* dm, int tree_begin, int tree_end);   // the device model on dm (outputs left unset)
   std::map<std::string, std::string> raw_params_;
   std::vector<std::string> eval_metrics_;
@@ -150,21 +144,11 @@ class Booster {
   DevBuf<DevNode> d_nodes; std::vector<int64_t> h_tree_offset; DevBuf<int64_t> d_tree_offset; DevBuf<int> d_tree_info;
   size_t d_nodes_used = 0; int d_trees_uploaded = 0;
   std::map<uint64_t, PredCache> caches_;
-  struct GrowerImpl* grower_ = nullptr;
+  std::unique_ptr<TreeBuilder> builder_ = std::make_unique<TreeBuilder>();   // its device buffers are sized by builder_for
+  DevBuf<double> dsum_;                         // device sums of the metrics and of the base-score stump
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1
-  bool profile_ = false;
-  enum ProfKind { kProfRootHist, kProfDeepHist, kProfPartition, kProfMargin, kProfKinds };
-  struct ProfEvent { cudaEvent_t a, b; int kind; long long launches; };
-  std::vector<ProfEvent> prof_events_;
-  // [0] rows through root launches, [1] rows through deeper launches, [2] rows of split nodes read by the partition,
-  // [3] rows the partition wrote
-  DevBuf<unsigned long long> prof_rows_;
-  long long prof_margin_rows_ = 0;
-  // partition byte model per row of the last profiled tree: [0] read at the root level (no row id), [1] read at deeper levels,
-  // [2] written (row id + gradient payload + tail bytes when they travel with the ids)
-  int prof_part_row_bytes_[3] = {0, 0, 0};
 
   void configure();
   float base_margin() const;
@@ -173,11 +157,10 @@ class Booster {
   PredCache& cache_for(DMatrix* dm);
   void bring_cache_up_to_date(DMatrix* dm, PredCache& c);
   void append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt);
+  void reserve_nodes(size_t count, size_t slack);    // room for `count` more nodes in d_nodes
+  TreeBuilder& builder_for(DMatrix* dm);             // the builder sized for the binned dm and the parameters
+  TreeInputs tree_inputs(const DMatrix& dm, const std::string& mask, int tree_index, float* margin, int k);
   void grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_index);
-  // root_mode: 0 = accumulate G and H, 1 = G and H + snapshot of the root H plane, 2 = G only on top of the cached H plane
-  void enqueue_tree(DMatrix* dtrain, float* margin, int k, const unsigned char* mask, DevNode* packed_out, int root_mode);
-  void prof_begin(ProfKind kind);
-  void prof_end();
   JPtr model_to_json();
   void model_from_json(const JValue& doc);
   JPtr config_to_json();

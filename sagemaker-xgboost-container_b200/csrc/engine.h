@@ -22,7 +22,8 @@ struct Error : std::runtime_error { using std::runtime_error::runtime_error; };
 // number of kernels this library has launched (reported by bench.py as gpu_launches)
 extern long long g_kernel_launches;
 
-// streaming multiprocessors of the engine's device (grid sizes of the grid-stride kernels scale with it)
+// the engine's stream, and the streaming multiprocessors of its device (grid sizes of the grid-stride kernels scale with it)
+cudaStream_t engine_stream();
 int engine_num_sms();
 
 template <typename T> struct DevBuf {
@@ -75,6 +76,7 @@ struct BinnedMatrix {
   int64_t n = 0;
   int F = 0, ngroups = 0, tw = 0, ntail = 0;
   int has_missing = 0;
+  int unused = 0;                         // makes the padding explicit: grow.h TreeInputs compares this block as bytes
 };
 
 // F = 32 a + L: a tail exists when there is at least one full group and 1 <= L <= 8; otherwise L features get a padded group.
