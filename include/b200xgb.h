@@ -190,6 +190,8 @@ XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dma
 XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_begin, int iter_end, const char** out_json);
 /* raw margins of the prediction cache the trainer keeps for `dmat` (n x num_class), brought up to date first */
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
+/* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
+XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
 /* CUDA-event stopwatch on the engine's stream: Start records an event, Stop records another, waits, returns ms */
 XGB_DLL int XGB200TimerStart(void);
 XGB_DLL int XGB200TimerStop(float* out_ms);

@@ -429,6 +429,14 @@ class CudaBackend:
         self._check(self.lib.XGB200BoosterGetCachedMargin(bh, dh, out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
 
+    def booster_tree_weights(self, bh):
+        """Each tree's weight in model order (booster=dart: weight_drop; all 1 for gbtree)."""
+        n = c_bst_ulong()
+        self._check(self.lib.XGB200BoosterGetTreeWeights(bh, C.byref(n), None))
+        out = np.zeros(n.value, np.float32)
+        self._check(self.lib.XGB200BoosterGetTreeWeights(bh, C.byref(n), out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out
+
     def timer_start(self):
         self._check(self.lib.XGB200TimerStart())
 

@@ -234,7 +234,7 @@ _IGNORED_PARAMS = {
     "csv_weights", "verbosity", "verbose", "silent", "nthread", "n_jobs", "predictor", "sketch_eps", "dsplit", "prob_buffer_row",
     "deterministic_histogram", "single_precision_histogram", "updater", "refresh_leaf", "process_type", "device", "gpu_id",
     "sampling_method", "validate_parameters", "max_cat_to_onehot", "max_cat_threshold", "num_parallel_tree",
-    "rate_drop", "one_drop", "skip_drop", "sample_type", "normalize_type", "lambda_bias", "feature_selector", "top_k",
+    "lambda_bias", "feature_selector", "top_k",
     "aft_loss_distribution", "aft_loss_distribution_scale", "disable_default_eval_metric",
     "multi_strategy", "max_cached_hist_node", "random_state",
 }

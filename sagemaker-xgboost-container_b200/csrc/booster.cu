@@ -241,7 +241,10 @@ void DMatrix::ensure_binned(int max_bin) {
 // subset keeps max(1, floor(frac * |parent|)) features).  Upstream shuffles with a mt19937; product and oracle share a
 // counter-based rule instead: feature f of the parent set is kept iff fewer than `keep` parent features have a smaller
 // hash u(stream, f) (ties: lower index first).  Streams: tree 0x1000 + t, level 0x300000 + 64 t + depth, node (eval kernel)
-// 0x80000000 + 2^20 t + nid.
+// 0x80000000 + 2^20 t + nid; the gradient subsample (misc.cu) draws from 0x2000 + round.  booster=dart draws its skip from
+// kDartSkipStream (index: round), its per-tree drops from kDartTreeStream + round (index: tree) and its one_drop pick from
+// kDartOneStream (index: round), all above 2^40 where no other stream reaches.
+constexpr uint64_t kDartSkipStream = 0x10000000000ull, kDartOneStream = 0x20000000000ull, kDartTreeStream = 0x30000000000ull;
 std::string subset_mask(const std::string& parent, float frac, unsigned seed, uint64_t stream) {
   if (frac >= 1.0f) return parent;
   const int F = (int)parent.size();
@@ -326,7 +329,24 @@ void Booster::configure() {
     // every method maps onto the device hist builder; exact/approx are accepted for hyperparameter compatibility
   }
   auto bo = raw_params_.find("booster");
-  if (bo != raw_params_.end()) B200_CHECK(bo->second == "gbtree", "Only booster=gbtree is implemented on the CUDA hist path (got " + bo->second + ")");
+  if (bo != raw_params_.end()) B200_CHECK(bo->second == "gbtree" || bo->second == "dart", "Only booster=gbtree and booster=dart are implemented on the CUDA hist path (got " + bo->second + ")");
+  dart_ = DartParam{};
+  if (bo != raw_params_.end() && bo->second == "dart") {      // the DART parameters are read (and checked) only under booster=dart
+    dart_.on = true;
+    dart_.rate_drop = getf("rate_drop", nullptr, 0.0f); dart_.skip_drop = getf("skip_drop", nullptr, 0.0f); dart_.one_drop = geti("one_drop", 0);
+    B200_CHECK(dart_.rate_drop >= 0.0f && dart_.rate_drop <= 1.0f, "Parameter rate_drop should be in [0, 1]");
+    B200_CHECK(dart_.skip_drop >= 0.0f && dart_.skip_drop <= 1.0f, "Parameter skip_drop should be in [0, 1]");
+    B200_CHECK(dart_.one_drop == 0 || dart_.one_drop == 1, "Parameter one_drop should be 0 or 1");
+    auto st = raw_params_.find("sample_type"), nt = raw_params_.find("normalize_type");
+    if (st != raw_params_.end()) {
+      B200_CHECK(st->second == "uniform" || st->second == "weighted", "Invalid sample_type: " + st->second + " (uniform, weighted)");
+      dart_.sample_type = st->second == "weighted" ? 1 : 0;
+    }
+    if (nt != raw_params_.end()) {
+      B200_CHECK(nt->second == "tree" || nt->second == "forest", "Invalid normalize_type: " + nt->second + " (tree, forest)");
+      dart_.normalize_type = nt->second == "forest" ? 1 : 0;
+    }
+  }
   auto gp = raw_params_.find("grow_policy");
   if (gp != raw_params_.end()) {
     B200_CHECK(gp->second == "depthwise" || gp->second == "lossguide", "Invalid grow_policy: " + gp->second + " (depthwise, lossguide)");
@@ -414,8 +434,8 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
   } else base_score_ = w;
 }
 
-void Booster::append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt) {
-  trees_.emplace_back(); tree_info_.push_back(class_id); pending_.push_back(pt); on_device_.push_back(1);
+void Booster::append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt, float weight) {
+  trees_.emplace_back(); tree_info_.push_back(class_id); pending_.push_back(pt); on_device_.push_back(1); weight_drop_.push_back(weight);
   h_tree_offset.resize(trees_.size() + 1);
   h_tree_offset[trees_.size() - 1] = (int64_t)device_offset;
   h_tree_offset[trees_.size()] = (int64_t)device_offset + max_nodes;
@@ -494,15 +514,96 @@ void Booster::bring_cache_up_to_date(DMatrix* dm, PredCache& c) {
       B200_CHECK(dm->base_margin.size() == (size_t)dm->n * K, "base_margin size does not match rows x groups");
       CUDA_OK(cudaMemcpyAsync(c.margin.p, dm->d_base_margin.p, sizeof(float) * dm->n * K, cudaMemcpyDeviceToDevice, s));
     } else launch_fill(c.margin.p, dm->n * K, base_margin(), s);
-    c.trees_applied = 0;
+    c.trees_applied = 0; c.weights.clear();
   }
-  if (c.trees_applied < nt) {
+  if (dart_.on) {
+    // booster=dart: first fl(w_now - w_applied) * leaf for the trees whose weight changed since, then the new trees with their
+    // weights, in one pass of the weighted tree-list kernel
+    std::vector<int> ids; std::vector<float> coef;
+    for (int t = 0; t < c.trees_applied; ++t)
+      if (c.weights[t] != weight_drop_[t]) { ids.push_back(t); coef.push_back(weight_drop_[t] - c.weights[t]); }
+    for (int t = c.trees_applied; t < nt; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
+    if (!ids.empty()) dart_margin(dm, ids, coef, {}, c.margin.p, nullptr);
+  } else if (c.trees_applied < nt) {
     upload_model();
     PredictArgs pa = predict_args(dm, c.trees_applied, nt);
     pa.margin = c.margin.p;
     launch_predict(pa, s);
-    c.trees_applied = nt;
   }
+  c.trees_applied = nt;
+  c.weights.assign(weight_drop_.begin(), weight_drop_.begin() + nt);
+}
+
+// ---------------------------------------------------------------------------------------------
+// booster=dart (upstream src/gbm/gbtree.cc Dart: DropTrees, NormalizeTrees), with this project's counter-based draws
+// ---------------------------------------------------------------------------------------------
+// The drop set D of boosting round `round` over the trees so far (T of them, every class), drawn from the streams listed at
+// subset_mask: skip_drop decides first, then one draw per tree, then the one_drop pick when D came out empty.
+std::vector<int> Booster::dart_drop_set(int round) const {
+  std::vector<int> D;
+  const int T = (int)weight_drop_.size();
+  const unsigned seed = param_.seed;
+  if (T == 0) return D;
+  if (dart_.skip_drop > 0.0f && rng_uniform(seed, kDartSkipStream, (uint64_t)round) < dart_.skip_drop) return D;
+  const uint64_t tree_stream = kDartTreeStream + (uint64_t)round;
+  float sum_w = 0.0f;
+  for (float w : weight_drop_) sum_w += w;
+  for (int i = 0; i < T; ++i) {
+    const float u = rng_uniform(seed, tree_stream, (uint64_t)i);
+    const float thr = dart_.sample_type == 1 ? dart_.rate_drop * (float)T * weight_drop_[i] / sum_w : dart_.rate_drop;
+    if (u < thr) D.push_back(i);
+  }
+  if (dart_.one_drop && D.empty()) {
+    const double u = (double)rng_uniform(seed, kDartOneStream, (uint64_t)round);
+    int pick = std::min(T - 1, (int)(u * (double)T));          // uniform
+    if (dart_.sample_type == 1) {                                 // in proportion to the weights: first tree whose prefix sum exceeds u * sum
+      double tot = 0.0; for (float w : weight_drop_) tot += (double)w;
+      const double target = u * tot; double acc = 0.0; pick = T - 1;
+      for (int i = 0; i < T; ++i) { acc += (double)weight_drop_[i]; if (acc > target) { pick = i; break; } }
+    }
+    D.push_back(pick);
+  }
+  return D;
+}
+
+// Draws D, updates the weights of the dropped trees and, in one pass over the rows, the training cache with them; returns
+// the margin the round's gradients read (the cache itself when nothing is dropped).  The new trees' weight goes to the builder.
+float* Booster::dart_begin_round(DMatrix* dtrain, PredCache& c, int round) {
+  const std::vector<int> D = dart_drop_set(round);
+  const int K = param_.num_class;
+  const float lr = (float)((double)param_.eta / (double)K);
+  float factor = 1.0f; dart_new_weight_ = 1.0f;
+  if (!D.empty()) {
+    if (dart_.normalize_type == 1) { factor = (float)(1.0 / (1.0 + (double)lr)); dart_new_weight_ = factor; }
+    else { const float denom = (float)D.size() + lr; factor = (float)((double)D.size() / (double)denom); dart_new_weight_ = (float)(1.0 / (double)denom); }
+  }
+  builder_->set_leaf_scale(dart_new_weight_);
+  if (D.empty()) return c.margin.p;
+  std::vector<float> coef_full, coef_drop;
+  for (int j : D) {
+    const float w = weight_drop_[j], w2 = w * factor;
+    coef_drop.push_back(w); coef_full.push_back(w2 - w);
+    weight_drop_[j] = w2; c.weights[j] = w2;
+  }
+  dart_drop_margin_.ensure((size_t)dtrain->n * K);
+  dart_margin(dtrain, D, coef_full, coef_drop, c.margin.p, dart_drop_margin_.p);
+  return dart_drop_margin_.p;
+}
+
+void Booster::dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop,
+                          float* m_full, float* m_drop) {
+  cudaStream_t s = engine_stream();
+  upload_model();
+  const size_t m = ids.size();
+  dart_ids_.ensure(m); dart_coef_.ensure(2 * m);
+  CUDA_OK(cudaMemcpyAsync(dart_ids_.p, ids.data(), sizeof(int) * m, cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(dart_coef_.p, coef_full.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
+  if (m_drop) CUDA_OK(cudaMemcpyAsync(dart_coef_.p + m, coef_drop.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
+  DartArgs a{}; a.X = dm->X.p; a.n = dm->n; a.F = dm->F; a.nodes = d_nodes.p; a.tree_offset = d_tree_offset.p; a.tree_info = d_tree_info.p;
+  a.trees = dart_ids_.p; a.ntrees = (int)m; a.K = param_.num_class; a.coef_full = dart_coef_.p; a.coef_drop = dart_coef_.p + m;
+  a.m_full = m_full; a.m_drop = m_drop;
+  launch_dart_margin(a, s);
+  Comm::get().sync_stream(s);            // the host vectors and the list buffers are reused by the next call
 }
 
 static void check_labels(const DMatrix* dm) {
@@ -545,9 +646,11 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   bring_cache_up_to_date(dtrain, cache);
 
   const int round = (int)trees_.size() / K;
+  // booster=dart: the gradients see the margin without the dropped trees; the cache already holds their new weights
+  const float* grad_margin = dart_.on ? dart_begin_round(dtrain, cache, round) : cache.margin.p;
   // ---- gradients + fixed-point scales
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
-  GradArgs ga{}; ga.margin = cache.margin.p; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
+  GradArgs ga{}; ga.margin = grad_margin; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
   ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = b.gs.absmax; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = K; ga.objective = param_.objective;
   ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = param_.subsample; ga.seed = param_.seed; ga.iter = (unsigned long long)round;
   ga.row_offset = (int64_t)Comm::get().rank() << 40; ga.aux = objective_aux(param_);
@@ -613,10 +716,12 @@ void Booster::grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_i
   reserve_nodes((size_t)b.cap_nodes, 64 * (size_t)b.cap_nodes);
   CUDA_OK(cudaMemcpyAsync(d_nodes.p + d_nodes_used, b.packed.p, sizeof(DevNode) * (size_t)b.cap_nodes, cudaMemcpyDeviceToDevice, s));
   if (pending_.size() - (size_t)std::count_if(pending_.begin(), pending_.end(), [](const PendingTree& p) { return p.staging == nullptr; }) >= 512) sync_model();
-  append_device_tree(k, d_nodes_used, b.cap_nodes, b.stage_tree());
+  const float weight = dart_.on ? dart_new_weight_ : 1.0f;
+  append_device_tree(k, d_nodes_used, b.cap_nodes, b.stage_tree(), weight);
   d_nodes_used += (size_t)b.cap_nodes;
   d_trees_uploaded = 0;                      // offsets/info arrays need a refresh before the next predict
-  cache.trees_applied = (int)trees_.size();  // update_margin_kernel already added this tree's leaves to the cache
+  cache.trees_applied = (int)trees_.size();  // update_margin_kernel already added this tree's leaves (times its weight) to the cache
+  cache.weights.push_back(weight);
 }
 
 void Booster::boost_one_iter(DMatrix*, const float*, const float*, size_t) {
@@ -748,8 +853,14 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     B200_CHECK(dm->base_margin.size() == (size_t)n * K, "base_margin size does not match rows x groups");
     CUDA_OK(cudaMemcpyAsync(margin.p, dm->d_base_margin.p, sizeof(float) * n * K, cudaMemcpyDeviceToDevice, s));
   } else launch_fill(margin.p, n * K, base_margin(), s);
-  pa.margin = margin.p; pa.leaf = nullptr;
-  launch_predict(pa, s);
+  if (dart_.on) {            // booster=dart: base + sum_t fl(w_t * leaf_t) in tree order (training=True predicts the same)
+    std::vector<int> ids; std::vector<float> coef;
+    for (int t = tb; t < te; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
+    if (!ids.empty()) dart_margin(dm, ids, coef, {}, margin.p, nullptr);
+  } else {
+    pa.margin = margin.p; pa.leaf = nullptr;
+    launch_predict(pa, s);
+  }
   int out_cols = K;
   DevBuf<float>& cls = pred_cls_;
   if (type == 0) {
@@ -810,7 +921,11 @@ void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* 
       else { float r = nodes[base + d.left].mean * nodes[base + d.left].sum_hess; r += nodes[base + d.right].mean * nodes[base + d.right].sum_hess; d.mean = r / d.sum_hess; }
     }
   }
-  DevBuf<ShapNode> d_sn; DevBuf<int64_t> d_off; DevBuf<int> d_info; DevBuf<float> d_out;
+  DevBuf<ShapNode> d_sn; DevBuf<int64_t> d_off; DevBuf<int> d_info; DevBuf<float> d_out, d_w;
+  if (dart_.on && te > tb) {
+    d_w.alloc((size_t)(te - tb));
+    CUDA_OK(cudaMemcpyAsync(d_w.p, weight_drop_.data() + tb, sizeof(float) * (te - tb), cudaMemcpyHostToDevice, s));
+  }
   d_sn.alloc(std::max<size_t>(nodes.size(), 1)); d_off.alloc(std::max<size_t>(offs.size(), 1)); d_info.alloc(std::max<size_t>(info.size(), 1));
   const size_t total = (size_t)n * K * (F + 1);
   d_out.alloc(std::max<size_t>(total, 1));
@@ -821,7 +936,7 @@ void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* 
   }
   CUDA_OK(cudaMemsetAsync(d_out.p, 0, sizeof(float) * std::max<size_t>(total, 1), s));
   ShapArgs sa{}; sa.X = dm->X.p; sa.n = n; sa.F = F; sa.nodes = d_sn.p; sa.tree_offset = d_off.p; sa.tree_info = d_info.p; sa.tree_begin = tb; sa.tree_end = te; sa.K = K;
-  sa.out = d_out.p; sa.base_margin = base_margin();
+  sa.out = d_out.p; sa.base_margin = base_margin(); sa.tree_weight = d_w.p;
   if (!dm->base_margin.empty()) { B200_CHECK(dm->base_margin.size() == (size_t)n * K, "base_margin size does not match rows x groups"); sa.base_margin_rows = dm->d_base_margin.p; }
   launch_shap(sa, max_depth, s);
   out->resize(total);

@@ -68,7 +68,13 @@ struct HostTree {
   int num_nodes() const { return (int)left.size(); }
 };
 
-struct PredCache { DevBuf<float> margin; int trees_applied = 0; int64_t n = 0; uint64_t model_version = 0; };
+struct PredCache {
+  DevBuf<float> margin; int trees_applied = 0; int64_t n = 0; uint64_t model_version = 0;
+  std::vector<float> weights;     // the weight each applied tree was added with (booster=dart changes them after the fact)
+};
+
+// booster=dart (upstream DartTrainParam); sample_type 0 uniform / 1 weighted, normalize_type 0 tree / 1 forest
+struct DartParam { bool on = false; float rate_drop = 0.0f, skip_drop = 0.0f; int one_drop = 0, sample_type = 0, normalize_type = 0; };
 
 // legacy_io.cc: the pre-JSON binary model format -> the 3.x model document
 bool looks_like_legacy_binary(const char* buf, size_t len);
@@ -109,6 +115,7 @@ class Booster {
   std::string debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end);   // JSON of the plan predict() would run
   const std::vector<HostTree>& trees() { sync_model(); return trees_; }
   const std::vector<int>& tree_info() const { return tree_info_; }
+  const std::vector<float>& tree_weights() const { return weight_drop_; }   // all 1 unless booster=dart
   float base_score() const { return base_score_; }
   int num_class() const { return param_.num_class; }
   const TrainParam& param() { configure(); return param_; }
@@ -137,6 +144,11 @@ class Booster {
   bool base_score_set_ = false; float base_score_ = 0.5f; bool base_score_estimated_ = false;
   int num_feature_ = 0;
   std::vector<HostTree> trees_; std::vector<int> tree_info_;
+  std::vector<float> weight_drop_;              // parallel to trees_: the tree's weight in every margin (booster=dart; else 1)
+  DartParam dart_;
+  float dart_new_weight_ = 1.0f;                // weight of the trees the current dart round grows
+  DevBuf<float> dart_drop_margin_;              // the training margin without the round's dropped trees (gradients read it)
+  DevBuf<int> dart_ids_; DevBuf<float> dart_coef_;    // tree list and coefficients of the last dart_margin launch
   std::vector<PendingTree> pending_;            // parallel to trees_ (nullptr staging once materialised)
   std::vector<char> on_device_;                 // parallel to trees_: nodes already in d_nodes
   uint64_t model_version_ = 0;
@@ -156,7 +168,11 @@ class Booster {
   void upload_model();
   PredCache& cache_for(DMatrix* dm);
   void bring_cache_up_to_date(DMatrix* dm, PredCache& c);
-  void append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt);
+  void append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt, float weight);
+  std::vector<int> dart_drop_set(int round) const;
+  float* dart_begin_round(DMatrix* dtrain, PredCache& c, int round);
+  void dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop,
+                   float* m_full, float* m_drop);
   void reserve_nodes(size_t count, size_t slack);    // room for `count` more nodes in d_nodes
   TreeBuilder& builder_for(DMatrix* dm);             // the builder sized for the binned dm and the parameters
   TreeInputs tree_inputs(const DMatrix& dm, const std::string& mask, int tree_index, float* margin, int k);

@@ -529,6 +529,13 @@ int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_
   API_BEGIN(); BoosterBox* box = static_cast<BoosterBox*>(handle); box->ret_str = BST(handle)->debug_predict_plan(DM(dmat), iter_begin, iter_end);
   *out_json = box->ret_str.c_str(); API_END();
 }
+int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out) {
+  API_BEGIN();
+  const std::vector<float>& w = BST(handle)->tree_weights();
+  if (len) *len = w.size();
+  if (out) memcpy(out, w.data(), sizeof(float) * w.size());
+  API_END();
+}
 int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out) {
   API_BEGIN();
   std::vector<float> v;

@@ -87,6 +87,7 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
   B200_CHECK(pool_bytes < free_b / 2 + hist_pool.n * sizeof(GH64), "histogram pool for this max_depth / max_leaves / feature count does not fit in device memory");
   hist_pool.alloc(pool_slots * slot_stride);
   gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(s); err.alloc(1); tree_index_dev.alloc(1);
+  if (!leaf_scale.p) { leaf_scale.alloc(1); set_leaf_scale(1.0f); }
   root_h_cache.alloc(slot_stride);
   for (int i = 0; i < 2; ++i) { ridx[i].alloc(n); gp[i].alloc(n); tl[i].alloc(tail_pos ? n : 0); }
   max_tiles = (unsigned)((n + kPartTile - 1) / kPartTile) + max_level_nodes + 1;
@@ -110,6 +111,12 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
     Comm::get().sync_stream(s);
     global_n = (int64_t)v;
   }
+}
+
+void TreeBuilder::set_leaf_scale(float v) {
+  cudaStream_t s = engine_stream();
+  CUDA_OK(cudaMemcpyAsync(leaf_scale.p, &v, sizeof v, cudaMemcpyHostToDevice, s));
+  Comm::get().sync_stream(s);
 }
 
 const unsigned char* TreeBuilder::upload_mask(const std::string& mask, int tree_index) {
@@ -281,7 +288,7 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     launch_eval(eval_args(in, L + 1, in.mask ? in.mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
   }
   // prediction cache += leaf values of this tree: one row-order pass over the column-major bins
-  timed(kProfMargin, [&] { launch_update_margin(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, in.margin, in.K, k, s); });
+  timed(kProfMargin, [&] { launch_update_margin(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, in.margin, in.K, k, leaf_scale.p, s); });
   if (profile) prof_margin_rows += bm.n;
   pack_tree_kernel<<<(cap_nodes + 255) / 256, 256, 0, s>>>(ta, gs.n_nodes, packed.p, cap_nodes); ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());

@@ -82,6 +82,9 @@ struct TreeBuilder {
   DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx[2], scratch;
   DevBuf<float2> gpair, gp[2]; DevBuf<unsigned> tl[2]; DevBuf<int> err, tree_index_dev; DevBuf<unsigned char> ic_path, ic_allowed, ic_sets;
   DevBuf<DevNode> packed;                  // the finished tree in the predictor's node format
+  // the factor of the tree's leaves in the prediction cache (booster=dart: the new trees' weight, else 1).  A buffer of the
+  // builder, not a TreeInputs field: a different weight every round must not force a fresh graph capture.
+  DevBuf<float> leaf_scale;
   // uploaded per tree; their addresses are part of TreeInputs
   DevBuf<unsigned char> feat_mask; DevBuf<int> monotone_dev;
   std::vector<unsigned char> ic_sets_host; // what ic_sets holds
@@ -107,6 +110,7 @@ struct TreeBuilder {
   const unsigned char* upload_mask(const std::string& mask, int tree_index);
   const int* upload_monotone(const std::vector<int>& mono, int F);    // nullptr when there are none
   void upload_interaction(const std::vector<std::vector<int>>& sets, int F);
+  void set_leaf_scale(float v);            // for the trees grown next
   void grow(const TreeInputs& in);         // one tree into packed / tree_block: issued directly or replayed from a graph
   PendingTree stage_tree();                // async copy of the finished tree block into pinned memory
   void set_profile(bool on); std::string profile_json();

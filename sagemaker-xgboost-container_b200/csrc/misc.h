@@ -54,8 +54,21 @@ struct ShapArgs {
   float* out;                      // [n][K][F + 1], zero-initialised by the caller
   const float* base_margin_rows;   // [n][K] user base margins, or nullptr -> base_margin
   float base_margin;
+  const float* tree_weight;        // per tree from tree_begin: its contributions are multiplied by it (booster=dart); nullptr = 1
 };
 void launch_shap(const ShapArgs& a, int max_depth, cudaStream_t s);
+
+// booster=dart (dart.cu): the leaf values of the listed trees on each row, weighted, into the margins [n][K]
+struct DartArgs {
+  const float* X; int64_t n; int F;
+  const DevNode* nodes; const int64_t* tree_offset; const int* tree_info;   // the device model, indexed by tree id
+  const int* trees; int ntrees; int K;          // the listed tree ids, in the order they are added
+  const float* coef_full;                       // per listed tree: m_full += fl(coef_full * leaf)
+  const float* coef_drop;                       // per listed tree: m_drop -= fl(coef_drop * leaf); unused without m_drop
+  float* m_full;
+  float* m_drop;                                // nullptr = no dropped margin; else written as m_full minus the dropped trees
+};
+void launch_dart_margin(const DartArgs& a, cudaStream_t s);
 
 void launch_gradient(const GradArgs& a, cudaStream_t s);
 void launch_sum_gpair(const float2* gp, int64_t n, double* out, cudaStream_t s);

@@ -73,6 +73,11 @@ JPtr Booster::model_to_json() {
   }
   model->set("trees", trees);
   gb->set("model", model); gb->set("name", S("gbtree"));
+  if (dart_.on) {            // upstream Dart::SaveModel: the gbtree object under "gbtree", the tree weights beside it
+    JPtr dart = JValue::Object(); dart->set("name", S("dart")); dart->set("gbtree", gb);
+    dart->set("weight_drop", JValue::F32(std::vector<float>(weight_drop_.begin(), weight_drop_.begin() + trees_.size())));
+    gb = dart;
+  }
   learner->set("gradient_booster", gb);
   JPtr lmp = JValue::Object();
   // scalar form = the 3.0.x schema this document is stamped with (3.1+ writes the bracketed vector "[1.0E1]", which the
@@ -92,7 +97,7 @@ JPtr Booster::model_to_json() {
 
 void Booster::reset_model() {
   sync_model();
-  trees_.clear(); tree_info_.clear(); pending_.clear(); on_device_.clear(); h_tree_offset.clear();
+  trees_.clear(); tree_info_.clear(); weight_drop_.clear(); pending_.clear(); on_device_.clear(); h_tree_offset.clear();
   d_nodes_used = 0; d_trees_uploaded = 0; caches_.clear(); ++model_version_; children_adjacent_ = true;
 }
 
@@ -123,8 +128,13 @@ void Booster::model_from_json(const JValue& doc) {
   base_score_ = (float)lmp.at("base_score").as_double(); base_score_set_ = true; base_score_estimated_ = true;
   raw_params_.erase("base_score");
   configured_ = false;
-  const JValue& gb = learner.at("gradient_booster");
-  B200_CHECK(gb.at("name").s == "gbtree", "Only gbtree models can be loaded (got " + gb.at("name").s + ")");
+  const JValue* gbp = &learner.at("gradient_booster");
+  const std::string gb_name = gbp->at("name").s;
+  B200_CHECK(gb_name == "gbtree" || gb_name == "dart", "Only gbtree and dart models can be loaded (got " + gb_name + ")");
+  const JValue* weights = nullptr;
+  if (gb_name == "dart") { weights = &gbp->at("weight_drop"); gbp = &gbp->at("gbtree"); raw_params_["booster"] = "dart"; }
+  else if (raw_params_.count("booster") && raw_params_["booster"] == "dart") raw_params_.erase("booster");
+  const JValue& gb = *gbp;
   const JValue& model = gb.at("model");
   const JValue& trees = model.at("trees");
   const JValue& tinfo = model.at("tree_info");
@@ -154,6 +164,16 @@ void Booster::model_from_json(const JValue& doc) {
       B200_CHECK(h.split_index[i] >= 0 && h.split_index[i] < std::max(num_feature_, 1), "model: tree " + std::to_string(t) + " node " + std::to_string(i) + " splits on feature " + std::to_string(h.split_index[i]) + " but the model has " + std::to_string(num_feature_) + " features");
     }
     trees_.push_back(std::move(h)); tree_info_.push_back((int)tinfo.num_at(t)); pending_.emplace_back(); on_device_.push_back(0);
+  }
+  weight_drop_.assign(trees_.size(), 1.0f);
+  if (weights) {             // a typed f32 array or a plain numeric array, one finite weight per tree
+    B200_CHECK(weights->type == JValue::kF32Array || weights->type == JValue::kArray, "model: weight_drop must be an array of numbers");
+    B200_CHECK(weights->length() == trees_.size(), "model: weight_drop has " + std::to_string(weights->length()) + " entries for " + std::to_string(trees_.size()) + " trees");
+    for (size_t t = 0; t < trees_.size(); ++t) {
+      const double w = weights->num_at(t);
+      B200_CHECK(std::isfinite(w) && std::isfinite((float)w), "model: weight_drop entry " + std::to_string(t) + " is not finite");
+      weight_drop_[t] = (float)w;
+    }
   }
   ++model_version_;
 }
@@ -206,11 +226,20 @@ JPtr Booster::config_to_json() {
     v += "]"; ttp->set("interaction_constraints", S(v));
   }
   gb->set("tree_train_param", ttp);
+  if (dart_.on) {            // upstream Dart::SaveConfig: {"name": "dart", "dart_train_param": {...}, "gbtree": {<gbtree config>}}
+    JPtr dart = JValue::Object(); dart->set("name", S("dart"));
+    JPtr dtp = JValue::Object();
+    dtp->set("normalize_type", S(dart_.normalize_type == 1 ? "forest" : "tree")); dtp->set("one_drop", S(dart_.one_drop ? "1" : "0"));
+    dtp->set("rate_drop", S(float_repr(dart_.rate_drop))); dtp->set("sample_type", S(dart_.sample_type == 1 ? "weighted" : "uniform"));
+    dtp->set("skip_drop", S(float_repr(dart_.skip_drop)));
+    dart->set("dart_train_param", dtp); dart->set("gbtree", gb);
+    gb = dart;
+  }
   learner->set("gradient_booster", gb);
   JPtr lmp = JValue::Object(); lmp->set("base_score", S(float_repr(base_score_))); lmp->set("boost_from_average", S("1"));
   lmp->set("num_class", S(std::to_string(param_.num_class > 1 ? param_.num_class : 0))); lmp->set("num_feature", S(std::to_string(num_feature_))); lmp->set("num_target", S("1"));
   learner->set("learner_model_param", lmp);
-  JPtr ltp = JValue::Object(); ltp->set("booster", S("gbtree")); ltp->set("disable_default_eval_metric", S("0")); ltp->set("multi_strategy", S("one_output_per_tree")); ltp->set("objective", S(objective_name_));
+  JPtr ltp = JValue::Object(); ltp->set("booster", S(dart_.on ? "dart" : "gbtree")); ltp->set("disable_default_eval_metric", S("0")); ltp->set("multi_strategy", S("one_output_per_tree")); ltp->set("objective", S(objective_name_));
   learner->set("learner_train_param", ltp);
   JPtr metrics = JValue::Array(); for (auto& m : eval_metrics_) { JPtr mo = JValue::Object(); mo->set("name", S(m)); metrics->arr.push_back(mo); } learner->set("metrics", metrics);
   JPtr obj = JValue::Object(); obj->set("name", S(objective_name_));
@@ -224,7 +253,14 @@ JPtr Booster::config_to_json() {
 
 void Booster::config_from_json(const JValue& doc) {
   const JValue& learner = doc.at("learner");
-  if (auto gb = learner.get("gradient_booster")) if (auto ttp = gb->get("tree_train_param")) for (auto& kv : ttp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+  if (auto gb = learner.get("gradient_booster")) {
+    if (gb->get("name") && gb->at("name").s == "dart") {
+      raw_params_["booster"] = "dart";
+      if (auto dtp = gb->get("dart_train_param")) for (auto& kv : dtp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+      if (auto inner = gb->get("gbtree")) gb = inner;
+    }
+    if (auto ttp = gb->get("tree_train_param")) for (auto& kv : ttp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+  }
   if (auto gp = learner.get("generic_param")) if (auto sd = gp->get("seed")) raw_params_["seed"] = sd->s;
   if (auto o = learner.get("objective")) {
     raw_params_["objective"] = o->at("name").s;
@@ -259,7 +295,8 @@ std::unique_ptr<Booster> Booster::slice(int begin, int end, int step) {
   b->objective_name_ = objective_name_; b->base_score_ = base_score_; b->base_score_set_ = base_score_set_; b->base_score_estimated_ = true; b->num_feature_ = num_feature_;
   b->raw_params_.erase("base_score"); b->base_score_set_ = true;
   for (int r = begin; r < end; r += step)
-    for (int k = 0; k < K; ++k) { b->trees_.push_back(trees_[(size_t)r * K + k]); b->tree_info_.push_back(tree_info_[(size_t)r * K + k]); b->pending_.emplace_back(); b->on_device_.push_back(0); }
+    for (int k = 0; k < K; ++k) { b->trees_.push_back(trees_[(size_t)r * K + k]); b->tree_info_.push_back(tree_info_[(size_t)r * K + k]); b->weight_drop_.push_back(weight_drop_[(size_t)r * K + k]);
+                                  b->pending_.emplace_back(); b->on_device_.push_back(0); }
   return b;
 }
 

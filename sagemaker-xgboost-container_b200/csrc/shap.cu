@@ -66,6 +66,7 @@ __global__ void __launch_bounds__(128) shap_kernel(ShapArgs a) {
   for (int t = a.tree_begin; t < a.tree_end; ++t) {
     const ShapNode* nodes = a.nodes + a.tree_offset[t - a.tree_begin];
     float* phi = a.out + (r * a.K + a.tree_info[t - a.tree_begin]) * cols;
+    const float tw = a.tree_weight ? a.tree_weight[t - a.tree_begin] : 1.0f;     // booster=dart: the tree's weight
     int sp = 0;
     stack[sp++] = ShapFrame{0, 0, 0, 1.0f, 1.0f, -1};
     while (sp > 0) {
@@ -80,7 +81,8 @@ __global__ void __launch_bounds__(128) shap_kernel(ShapArgs a) {
       if (nd.left < 0) {
         for (int i = 1; i <= depth; ++i) {
           const float w = unwound_path_sum(up, depth, i);
-          phi[up[i].feature] += w * (up[i].one_fraction - up[i].zero_fraction) * nd.cond;
+          if (a.tree_weight) phi[up[i].feature] += (w * (up[i].one_fraction - up[i].zero_fraction) * nd.cond) * tw;
+          else phi[up[i].feature] += w * (up[i].one_fraction - up[i].zero_fraction) * nd.cond;
         }
       } else {
         const int split = (int)(nd.fidx_dl & 0x7fffffffu);
@@ -102,7 +104,8 @@ __global__ void __launch_bounds__(128) shap_kernel(ShapArgs a) {
         stack[sp++] = ShapFrame{hot, depth + 1, my_off, hot_zero * incoming_zero, incoming_one, split};
       }
     }
-    phi[a.F] += nodes[0].mean;          // expected value of the tree (cover-weighted mean of its leaves)
+    if (a.tree_weight) phi[a.F] += nodes[0].mean * tw;
+    else phi[a.F] += nodes[0].mean;     // expected value of the tree (cover-weighted mean of its leaves)
   }
 }
 

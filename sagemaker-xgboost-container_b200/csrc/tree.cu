@@ -645,7 +645,7 @@ constexpr int kPackedNodesSmem = 2048;
 static_assert(sizeof(PackedNode) == 8, "PackedNode is 8 B");
 
 __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing,
-                                                            float* margin, int K, int k) {
+                                                            float* margin, int K, int k, const float* leaf_scale) {
   __shared__ PackedNode s_nodes[kPackedNodesSmem];
   __shared__ float s_leaf[kPackedNodesSmem];
   const int nn = *n_nodes;
@@ -690,8 +690,10 @@ __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const 
       any |= !done[j];
     }
   }
+  // margin += fl(scale * leaf), rounded separately (booster=dart restates it); scale == 1 (gbtree) adds the leaf itself
+  const float sc = *leaf_scale;
 #pragma unroll
-  for (int j = 0; j < 4; ++j) { const int64_t r = base + j * 256; if (r < n) margin[r * K + k] += packed ? s_leaf[nid[j]] : t.split_cond[nid[j]]; }
+  for (int j = 0; j < 4; ++j) { const int64_t r = base + j * 256; if (r < n) margin[r * K + k] = __fadd_rn(margin[r * K + k], __fmul_rn(sc, packed ? s_leaf[nid[j]] : t.split_cond[nid[j]])); }
 }
 
 // sibling = parent - built child (exact int64)
@@ -738,9 +740,10 @@ void launch_partition(const PartArgs& a, unsigned max_tiles, cudaStream_t s) {
   else { if (tl) part_kernel<false, true><<<max_tiles, 256, 0, s>>>(a); else part_kernel<false, false><<<max_tiles, 256, 0, s>>>(a); }
   ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
-void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k, cudaStream_t s) {
+void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k,
+                          const float* leaf_scale, cudaStream_t s) {
   if (n == 0) return;
-  update_margin_kernel<<<(unsigned)((n + 1023) / 1024), 256, 0, s>>>(t, n_nodes, bins_col, n, has_missing, margin, K, k); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  update_margin_kernel<<<(unsigned)((n + 1023) / 1024), 256, 0, s>>>(t, n_nodes, bins_col, n, has_missing, margin, K, k, leaf_scale); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_subtract(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s) {
   dim3 grid(max_build, (unsigned)((slot_entries + 1023) / 1024)); subtract_kernel<<<grid, 256, 0, s>>>(gs, pool, slot_entries); ++g_kernel_launches; CUDA_OK(cudaGetLastError());

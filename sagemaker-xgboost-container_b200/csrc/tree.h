@@ -84,7 +84,9 @@ void launch_scales(const GrowState& gs, int grad_bits, cudaStream_t s);
 void launch_eval(const EvalArgs& a, int max_nodes_level, cudaStream_t s);
 void launch_apply(const ApplyArgs& a, cudaStream_t s);
 void launch_partition(const PartArgs& a, unsigned max_tiles, cudaStream_t s);
-void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k, cudaStream_t s);
+// margin[:, k] += fl(*leaf_scale * leaf) of the finished tree (leaf_scale: one float on the device, 1 except under booster=dart)
+void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k,
+                          const float* leaf_scale, cudaStream_t s);
 void launch_subtract(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s);
 
 }  // namespace b200
