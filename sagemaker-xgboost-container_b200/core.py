@@ -233,7 +233,7 @@ def _param_items(params):
 _IGNORED_PARAMS = {
     "csv_weights", "verbosity", "verbose", "silent", "nthread", "n_jobs", "predictor", "sketch_eps", "dsplit", "prob_buffer_row",
     "deterministic_histogram", "single_precision_histogram", "updater", "refresh_leaf", "process_type", "device", "gpu_id",
-    "sampling_method", "validate_parameters", "max_cat_to_onehot", "max_cat_threshold", "num_parallel_tree",
+    "sampling_method", "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
     "lambda_bias", "feature_selector", "top_k",
     "aft_loss_distribution", "aft_loss_distribution_scale", "disable_default_eval_metric",
     "multi_strategy", "max_cached_hist_node", "random_state",
@@ -271,8 +271,6 @@ def _check_unapplied(k, v):
     if k == "tree_method" and str(v) in ("exact", "approx"):
         warnings.warn("tree_method=%s runs the CUDA hist builder (quantile-binned histograms), not xgboost's %s updater" % (v, v))
         return v
-    if k == "num_parallel_tree" and _as_float(v, 1) > 1:
-        raise XGBoostError("num_parallel_tree=%s (boosted random forests) is not implemented by the CUDA hist builder" % v)
     if k == "process_type" and str(v) == "update":
         raise XGBoostError("process_type=update is not implemented by the CUDA hist builder")
     if k == "sampling_method" and str(v) == "gradient_based":

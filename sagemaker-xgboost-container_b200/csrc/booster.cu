@@ -5,6 +5,7 @@
 #include "booster.h"
 #include <algorithm>
 #include <atomic>
+#include <cctype>
 #include <cmath>
 #include <cstring>
 #include "comm.h"
@@ -243,8 +244,10 @@ void DMatrix::ensure_binned(int max_bin) {
 // hash u(stream, f) (ties: lower index first).  Streams: tree 0x1000 + t, level 0x300000 + 64 t + depth, node (eval kernel)
 // 0x80000000 + 2^20 t + nid; the gradient subsample (misc.cu) draws from 0x2000 + round.  booster=dart draws its skip from
 // kDartSkipStream (index: round), its per-tree drops from kDartTreeStream + round (index: tree) and its one_drop pick from
-// kDartOneStream (index: round), all above 2^40 where no other stream reaches.
+// kDartOneStream (index: round), all above 2^40 where no other stream reaches.  A forest (num_parallel_tree > 1) draws the
+// rows of tree j >= 1 of a round from kForestRowStream + 2^20 round + j (index: row); tree 0 keeps 0x2000 + round.
 constexpr uint64_t kDartSkipStream = 0x10000000000ull, kDartOneStream = 0x20000000000ull, kDartTreeStream = 0x30000000000ull;
+constexpr uint64_t kForestRowStream = 0x40000000000ull;
 std::string subset_mask(const std::string& parent, float frac, unsigned seed, uint64_t stream) {
   if (frac >= 1.0f) return parent;
   const int F = (int)parent.size();
@@ -309,6 +312,13 @@ void Booster::configure() {
   p.subsample = getf("subsample", nullptr, 1.0f); p.colsample_bytree = getf("colsample_bytree", nullptr, 1.0f);
   p.colsample_bylevel = getf("colsample_bylevel", nullptr, 1.0f); p.colsample_bynode = getf("colsample_bynode", nullptr, 1.0f);
   p.seed = (unsigned)geti("seed", 0);
+  if (auto it = raw_params_.find("num_parallel_tree"); it != raw_params_.end()) {
+    double v = 0.0; size_t used = 0;
+    try { v = std::stod(it->second, &used); } catch (...) { used = 0; }
+    while (used > 0 && used < it->second.size() && std::isspace((unsigned char)it->second[used])) ++used;
+    B200_CHECK(used > 0 && used == it->second.size() && v == std::floor(v) && v >= 1.0 && v <= (double)(1 << 20), "num_parallel_tree must be an integer in [1, 1048576] (got " + it->second + ")");
+    p.num_parallel_tree = (int)v;
+  }
   p.huber_slope = getf("huber_slope", nullptr, 1.0f); p.tweedie_variance_power = getf("tweedie_variance_power", nullptr, 1.5f);
   B200_CHECK(p.huber_slope != 0.0f, "Check failed: slope != 0.0 (huber_slope)");
   B200_CHECK(p.tweedie_variance_power >= 1.0f && p.tweedie_variance_power < 2.0f, "tweedie_variance_power must be in interval [1, 2)");
@@ -645,7 +655,14 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   PredCache& cache = cache_for(dtrain);
   bring_cache_up_to_date(dtrain, cache);
 
-  const int round = (int)trees_.size() / K;
+  const int round = layers();
+  const int P = param_.num_parallel_tree;
+  // a forest with row sampling draws one row sample per tree: the gradients of every row go to a round buffer first, and each
+  // tree's masked copy (and its scales) is made before the tree is grown.  Otherwise every tree of the round shares them.
+  const bool per_tree_sample = P > 1 && param_.subsample < 1.0f;
+  // dart forests (a dart model written elsewhere with num_parallel_tree > 1) load and predict, but do not train on
+  B200_CHECK(!dart_.on || P == 1, "booster=dart with num_parallel_tree > 1 is not implemented on the CUDA hist path");
+  if (!per_tree_sample) forest_gpair_.release();
   // booster=dart: the gradients see the margin without the dropped trees; the cache already holds their new weights
   const float* grad_margin = dart_.on ? dart_begin_round(dtrain, cache, round) : cache.margin.p;
   // ---- gradients + fixed-point scales
@@ -654,11 +671,28 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = b.gs.absmax; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = K; ga.objective = param_.objective;
   ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = param_.subsample; ga.seed = param_.seed; ga.iter = (unsigned long long)round;
   ga.row_offset = (int64_t)Comm::get().rank() << 40; ga.aux = objective_aux(param_);
+  if (per_tree_sample) { forest_gpair_.ensure((size_t)b.gp_stride * K); ga.gpair = forest_gpair_.p; ga.absmax = nullptr; ga.subsample = 1.0f; }
   launch_gradient(ga, s);
-  Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
-  launch_scales(b.gs, grad_bits_for(b.global_n), s);
+  if (!per_tree_sample) {
+    Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
+    launch_scales(b.gs, grad_bits_for(b.global_n), s);
+  }
 
-  for (int k = 0; k < K; ++k) grow_one_tree(dtrain, cache, k, round * K + k);
+  // K * P trees, class-major: tree j of class k is tree k * P + j of the layer
+  for (int k = 0; k < K; ++k)
+    for (int j = 0; j < P; ++j) {
+      if (per_tree_sample) {     // tree j's rows (shared by the K classes): j = 0 draws the stream a single tree draws
+        CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
+        SampleArgs sa{}; sa.src = forest_gpair_.p; sa.dst = b.gpair.p; sa.absmax = b.gs.absmax; sa.gp_stride = b.gp_stride; sa.n = dtrain->n;
+        sa.row_offset = ga.row_offset; sa.K = K; sa.subsample = param_.subsample; sa.seed = param_.seed;
+        sa.stream = j == 0 ? 0x2000ull + (uint64_t)round : kForestRowStream + ((uint64_t)round << 20) + (uint64_t)j;
+        launch_sample_gpair(sa, s);
+        Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
+        launch_scales(b.gs, grad_bits_for(b.global_n), s);
+      }
+      grow_one_tree(dtrain, cache, k, iteration_indptr_[round] + k * P + j);
+    }
+  iteration_indptr_.push_back((int)trees_.size());
 }
 
 // grow_policy=lossguide: expansions per tree = leaves - 1, bounded by max_leaves or by a full tree of max_depth
@@ -668,8 +702,9 @@ static int lossguide_iters(const TrainParam& p) {
   return (1 << p.max_depth) - 1;
 }
 
+// a round's P trees of a class share its learning rate: leaves are fl(eta / P) * w (upstream BoostNewTrees); exact eta at P = 1
 static TrainParamDev to_dev(const TrainParam& p) {
-  TrainParamDev d; d.eta = p.eta; d.lambda = p.lambda; d.alpha = p.alpha; d.gamma = p.gamma; d.min_child_weight = p.min_child_weight;
+  TrainParamDev d; d.eta = p.eta / (float)p.num_parallel_tree; d.lambda = p.lambda; d.alpha = p.alpha; d.gamma = p.gamma; d.min_child_weight = p.min_child_weight;
   d.max_delta_step = p.max_delta_step; d.max_depth = p.max_depth; d.max_leaves = p.max_leaves; return d;
 }
 
@@ -728,7 +763,7 @@ void Booster::boost_one_iter(DMatrix*, const float*, const float*, size_t) {
   throw Error("custom objective (BoostOneIter) is not implemented on the CUDA hist path");
 }
 
-int Booster::boosted_rounds() { configure(); return (int)trees_.size() / std::max(1, param_.num_class); }
+int Booster::boosted_rounds() { configure(); return layers(); }
 
 // ---------------------------------------------------------------------------------------------
 // evaluation  (upstream src/learner.cc EvalOneIter: "[iter]\t<name>-<metric>:<value>")
@@ -824,15 +859,15 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
   (void)training;
   cudaStream_t s = engine_stream();
   const int K = param_.num_class;
-  const int rounds = (int)trees_.size() / K;
+  const int rounds = layers();
   if (iter_end == 0) iter_end = rounds;
   B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end <= rounds, "Invalid iteration range: [" + std::to_string(iter_begin) + ", " + std::to_string(iter_end) + ") for a model with " + std::to_string(rounds) + " rounds");
   if (num_feature_ > 0 && !trees_.empty())
     B200_CHECK(dm->F <= num_feature_ || true, "feature count mismatch");
   B200_CHECK(type == 0 || type == 1 || type == 2 || type == 6, "predict type " + std::to_string(type) + " (approximate contributions / interactions) is not implemented on the CUDA path");
-  if (type == 2) { predict_contribs(dm, iter_begin * K, iter_end * K, out, shape); return; }
+  const int tb = iteration_indptr_[iter_begin], te = iteration_indptr_[iter_end];
+  if (type == 2) { predict_contribs(dm, tb, te, out, shape); return; }
   upload_model();
-  const int tb = iter_begin * K, te = iter_end * K;
   const int64_t n = dm->n;
   PredictArgs pa = predict_args(dm, tb, te);
   if (type == 6) {
@@ -957,10 +992,9 @@ PredictArgs Booster::predict_args(DMatrix* dm, int tree_begin, int tree_end) {
 std::string Booster::debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end) {
   configure();
   upload_model();
-  const int K = param_.num_class;
-  if (iter_end == 0) iter_end = (int)trees_.size() / K;
-  B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end * K <= (int)trees_.size(), "debug_predict_plan: invalid iteration range");
-  const PredictArgs pa = predict_args(dm, iter_begin * K, iter_end * K);
+  if (iter_end == 0) iter_end = layers();
+  B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end <= layers(), "debug_predict_plan: invalid iteration range");
+  const PredictArgs pa = predict_args(dm, iteration_indptr_[iter_begin], iteration_indptr_[iter_end]);
   return predict_plan_json(plan_for(pa), pa.tree_begin, pa.tree_end, pa.has_nan != 0);
 }
 

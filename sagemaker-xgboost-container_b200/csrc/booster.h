@@ -144,7 +144,11 @@ class Booster {
   bool base_score_set_ = false; float base_score_ = 0.5f; bool base_score_estimated_ = false;
   int num_feature_ = 0;
   std::vector<HostTree> trees_; std::vector<int> tree_info_;
-  std::vector<float> weight_drop_;              // parallel to trees_: the tree's weight in every margin (booster=dart; else 1)
+  // boosting round (layer) r holds trees [iteration_indptr_[r], iteration_indptr_[r + 1]): K * num_parallel_tree of them,
+  // class-major.  The only round <-> tree map; always starts with 0 and ends with trees_.size()
+  std::vector<int> iteration_indptr_{0};
+  DevBuf<float2> forest_gpair_;                 // num_parallel_tree > 1 with subsample < 1: the round's unsampled gradients
+  std::vector<float> weight_drop_;             // parallel to trees_: the tree's weight in every margin (booster=dart; else 1)
   DartParam dart_;
   float dart_new_weight_ = 1.0f;                // weight of the trees the current dart round grows
   DevBuf<float> dart_drop_margin_;              // the training margin without the round's dropped trees (gradients read it)
@@ -163,6 +167,7 @@ class Booster {
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1
 
   void configure();
+  int layers() const { return (int)iteration_indptr_.size() - 1; }
   float base_margin() const;
   void estimate_base_score(DMatrix* dtrain);
   void upload_model();

@@ -113,6 +113,7 @@ struct TrainParam {
   float eta = 0.3f, lambda = 1.0f, alpha = 0.0f, gamma = 0.0f, min_child_weight = 1.0f, max_delta_step = 0.0f;
   float scale_pos_weight = 1.0f, subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   unsigned seed = 0;
+  int num_parallel_tree = 1;    // trees per class per boosting round (boosted random forests)
   float huber_slope = 1.0f, tweedie_variance_power = 1.5f, poisson_max_delta_step = 0.7f;   // objective parameters (upstream defaults)
 };
 

@@ -102,6 +102,29 @@ __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
   }
 }
 
+// one tree's row sample of a forest round: the kept rows' pairs of every class copied, the others zeroed, and max|g|, max h of
+// the copy folded into absmax (the tree's fixed-point scales).  Reads and writes 8 K bytes per row.
+__global__ void __launch_bounds__(256) sample_gpair_kernel(SampleArgs a) {
+  float mg = 0.f, mh = 0.f;
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < a.n; r += (int64_t)gridDim.x * blockDim.x) {
+    const bool keep = rng_uniform(a.seed, a.stream, (unsigned long long)(r + a.row_offset)) < a.subsample;
+    for (int k = 0; k < a.K; ++k) {
+      const float2 v = keep ? a.src[(int64_t)k * a.gp_stride + r] : make_float2(0.f, 0.f);
+      a.dst[(int64_t)k * a.gp_stride + r] = v;
+      mg = fmaxf(mg, fabsf(v.x)); mh = fmaxf(mh, v.y);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { mg = fmaxf(mg, __shfl_xor_sync(0xffffffffu, mg, o)); mh = fmaxf(mh, __shfl_xor_sync(0xffffffffu, mh, o)); }
+  __shared__ float sg[8], sh[8];
+  if ((threadIdx.x & 31) == 0) { sg[threadIdx.x >> 5] = mg; sh[threadIdx.x >> 5] = mh; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; ++w) { mg = fmaxf(mg, sg[w]); mh = fmaxf(mh, sh[w]); }
+    atomicMax(a.absmax, __float_as_uint(mg)); atomicMax(a.absmax + 1, __float_as_uint(mh));
+  }
+}
+
 // sum of (g,h) over rows in double (base-score stump)
 __global__ void __launch_bounds__(256) sum_gpair_kernel(const float2* gp, int64_t n, double* out) {
   double g = 0, h = 0;
@@ -388,6 +411,10 @@ static inline int grid_for(int64_t n, int block = 256, int cap = engine_num_sms(
 void launch_gradient(const GradArgs& a, cudaStream_t s) {
   if (a.n == 0) return;
   gradient_kernel<<<grid_for(a.n, 256, engine_num_sms() * 8), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+void launch_sample_gpair(const SampleArgs& a, cudaStream_t s) {
+  if (a.n == 0) return;
+  sample_gpair_kernel<<<grid_for(a.n, 256, engine_num_sms() * 8), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_sum_gpair(const float2* gp, int64_t n, double* out, cudaStream_t s) {
   sum_gpair_kernel<<<grid_for(n), 256, 0, s>>>(gp, n, out); ++g_kernel_launches; CUDA_OK(cudaGetLastError());

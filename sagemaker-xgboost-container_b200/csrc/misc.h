@@ -70,7 +70,17 @@ struct DartArgs {
 };
 void launch_dart_margin(const DartArgs& a, cudaStream_t s);
 
+// num_parallel_tree > 1 with subsample < 1: one tree's row sample of the round's unsampled gradients (misc.cu)
+struct SampleArgs {
+  const float2* src;        // [K][gp_stride] the round's gradients, every row
+  float2* dst;              // [K][gp_stride] the tree's copy: unsampled rows get (0, 0)
+  unsigned* absmax;         // max|g|, max h of dst as float bits (atomicMax)
+  int64_t gp_stride, n, row_offset;
+  int K; float subsample; unsigned seed; unsigned long long stream;
+};
+
 void launch_gradient(const GradArgs& a, cudaStream_t s);
+void launch_sample_gpair(const SampleArgs& a, cudaStream_t s);
 void launch_sum_gpair(const float2* gp, int64_t n, double* out, cudaStream_t s);
 void launch_bin(const float* X, int64_t n, int F, int ngroups, int tw, const int* cut_ptrs, const float* cut_vals, uint8_t* bins, uint8_t* bins_tail, cudaStream_t s);
 void launch_transpose_bins(const uint8_t* bins, const uint8_t* bins_tail, int64_t n, int F, int ngroups, int tw, uint8_t* bins_col, cudaStream_t s);

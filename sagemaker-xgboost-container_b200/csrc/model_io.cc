@@ -44,11 +44,9 @@ JPtr Booster::model_to_json() {
   JPtr fn = JValue::Array(); for (auto& x : feature_names) fn->arr.push_back(S(x)); learner->set("feature_names", fn);
   JPtr ft = JValue::Array(); for (auto& x : feature_types) ft->arr.push_back(S(x)); learner->set("feature_types", ft);
   JPtr gb = JValue::Object(); JPtr model = JValue::Object();
-  JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S("1")); gmp->set("num_trees", S(std::to_string(trees_.size())));
+  JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S(std::to_string(param_.num_parallel_tree))); gmp->set("num_trees", S(std::to_string(trees_.size())));
   model->set("gbtree_model_param", gmp);
-  std::vector<int32_t> indptr; const int rounds = (int)trees_.size() / std::max(1, K);
-  for (int r = 0; r <= rounds; ++r) indptr.push_back(r * K);
-  model->set("iteration_indptr", JValue::I32(indptr));
+  model->set("iteration_indptr", JValue::I32(std::vector<int32_t>(iteration_indptr_.begin(), iteration_indptr_.end())));
   model->set("tree_info", JValue::I32(std::vector<int32_t>(tree_info_.begin(), tree_info_.end())));
   JPtr trees = JValue::Array();
   for (size_t t = 0; t < trees_.size(); ++t) {
@@ -97,7 +95,7 @@ JPtr Booster::model_to_json() {
 
 void Booster::reset_model() {
   sync_model();
-  trees_.clear(); tree_info_.clear(); weight_drop_.clear(); pending_.clear(); on_device_.clear(); h_tree_offset.clear();
+  trees_.clear(); tree_info_.clear(); iteration_indptr_.assign(1, 0); weight_drop_.clear(); pending_.clear(); on_device_.clear(); h_tree_offset.clear();
   d_nodes_used = 0; d_trees_uploaded = 0; caches_.clear(); ++model_version_; children_adjacent_ = true;
 }
 
@@ -139,8 +137,34 @@ void Booster::model_from_json(const JValue& doc) {
   const JValue& trees = model.at("trees");
   const JValue& tinfo = model.at("tree_info");
   B200_CHECK(trees.type == JValue::kArray && tinfo.length() == trees.arr.size(), "model: tree_info does not have one entry per tree");
-  { int K = std::max(1, nc); if (nc <= 1) if (auto sp = obj.get("softmax_multiclass_param")) K = std::max(1, (int)sp->at("num_class").as_int());
-    for (size_t t = 0; t < trees.arr.size(); ++t) { const double g = tinfo.num_at(t); B200_CHECK(g >= 0 && g < K, "model: tree_info entry out of range"); } }
+  int K = std::max(1, nc); if (nc <= 1) if (auto sp = obj.get("softmax_multiclass_param")) K = std::max(1, (int)sp->at("num_class").as_int());
+  for (size_t t = 0; t < trees.arr.size(); ++t) { const double g = tinfo.num_at(t); B200_CHECK(g >= 0 && g < K, "model: tree_info entry out of range"); }
+  // the layer layout: iteration_indptr when the document has it (2.x / 3.x), else K * num_parallel_tree trees per round (1.x)
+  int P = 1;
+  if (auto gmp = model.get("gbtree_model_param")) if (auto v = gmp->get("num_parallel_tree")) {
+    const double d = v->as_double();
+    B200_CHECK(d >= 1.0 && d <= (double)(1 << 20) && d == std::floor(d), "model: num_parallel_tree must be a positive integer");
+    P = (int)d;
+  }
+  const int64_t ntrees = (int64_t)trees.arr.size();
+  std::vector<int> indptr;
+  if (auto ip = model.get("iteration_indptr")) {
+    B200_CHECK(ip->length() >= 1, "model: iteration_indptr is empty");
+    for (size_t r = 0; r < ip->length(); ++r) {
+      const double v = ip->num_at(r);
+      B200_CHECK(v == std::floor(v) && v >= 0 && v <= (double)ntrees, "model: iteration_indptr entry " + std::to_string(r) + " is not a tree count in [0, " + std::to_string(ntrees) + "]");
+      B200_CHECK(r > 0 || v == 0, "model: iteration_indptr must start with 0");
+      B200_CHECK(r == 0 || (int)v >= indptr.back(), "model: iteration_indptr must not decrease");
+      indptr.push_back((int)v);
+    }
+    B200_CHECK(indptr.back() == ntrees, "model: iteration_indptr ends at " + std::to_string(indptr.back()) + " but the model has " + std::to_string(ntrees) + " trees");
+  } else {
+    const int64_t per = (int64_t)K * P;
+    B200_CHECK(ntrees % per == 0, "model: " + std::to_string(ntrees) + " trees are not whole rounds of num_class x num_parallel_tree = " + std::to_string(per));
+    for (int64_t t = 0; t <= ntrees; t += per) indptr.push_back((int)t);
+  }
+  iteration_indptr_ = indptr;
+  raw_params_["num_parallel_tree"] = std::to_string(P);
   for (size_t t = 0; t < trees.arr.size(); ++t) {
     const JValue& tj = *trees.arr[t];
     HostTree h;
@@ -211,7 +235,7 @@ JPtr Booster::config_to_json() {
   JPtr gp = JValue::Object(); gp->set("device", S("cuda:0")); gp->set("seed", S(std::to_string(param_.seed))); gp->set("nthread", S("0"));
   learner->set("generic_param", gp);
   JPtr gb = JValue::Object(); gb->set("name", S("gbtree"));
-  JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S("1")); gmp->set("num_trees", S(std::to_string(trees_.size()))); gb->set("gbtree_model_param", gmp);
+  JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S(std::to_string(param_.num_parallel_tree))); gmp->set("num_trees", S(std::to_string(trees_.size()))); gb->set("gbtree_model_param", gmp);
   JPtr gtp = JValue::Object(); gtp->set("process_type", S("default")); gtp->set("tree_method", S("hist")); gtp->set("updater", S("grow_b200_hist")); gb->set("gbtree_train_param", gtp);
   JPtr ttp = JValue::Object();
   auto f = [&](const char* k, float v) { ttp->set(k, S(float_repr(v))); }; auto i = [&](const char* k, int v) { ttp->set(k, S(std::to_string(v))); };
@@ -260,6 +284,7 @@ void Booster::config_from_json(const JValue& doc) {
       if (auto inner = gb->get("gbtree")) gb = inner;
     }
     if (auto ttp = gb->get("tree_train_param")) for (auto& kv : ttp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+    if (auto gmp = gb->get("gbtree_model_param")) if (auto v = gmp->get("num_parallel_tree")) if (v->type == JValue::kString) raw_params_["num_parallel_tree"] = v->s;
   }
   if (auto gp = learner.get("generic_param")) if (auto sd = gp->get("seed")) raw_params_["seed"] = sd->s;
   if (auto o = learner.get("objective")) {
@@ -285,8 +310,7 @@ void Booster::unserialize(const char* buf, size_t len) { load_model_buffer(buf, 
 
 std::unique_ptr<Booster> Booster::slice(int begin, int end, int step) {
   configure(); sync_model();
-  const int K = std::max(1, param_.num_class);
-  const int rounds = (int)trees_.size() / K;
+  const int rounds = layers();
   if (end == 0) end = rounds;
   B200_CHECK(step >= 1, "Invalid slice step");
   B200_CHECK(begin >= 0 && begin < end && end <= rounds, "Layer index out of range");     // upstream message for an empty / OOB slice
@@ -294,9 +318,13 @@ std::unique_ptr<Booster> Booster::slice(int begin, int end, int step) {
   b->raw_params_ = raw_params_; b->eval_metrics_ = eval_metrics_; b->attrs = attrs; b->feature_names = feature_names; b->feature_types = feature_types;
   b->objective_name_ = objective_name_; b->base_score_ = base_score_; b->base_score_set_ = base_score_set_; b->base_score_estimated_ = true; b->num_feature_ = num_feature_;
   b->raw_params_.erase("base_score"); b->base_score_set_ = true;
-  for (int r = begin; r < end; r += step)
-    for (int k = 0; k < K; ++k) { b->trees_.push_back(trees_[(size_t)r * K + k]); b->tree_info_.push_back(tree_info_[(size_t)r * K + k]); b->weight_drop_.push_back(weight_drop_[(size_t)r * K + k]);
-                                  b->pending_.emplace_back(); b->on_device_.push_back(0); }
+  for (int r = begin; r < end; r += step) {
+    for (int t = iteration_indptr_[r]; t < iteration_indptr_[r + 1]; ++t) {
+      b->trees_.push_back(trees_[t]); b->tree_info_.push_back(tree_info_[t]); b->weight_drop_.push_back(weight_drop_[t]);
+      b->pending_.emplace_back(); b->on_device_.push_back(0);
+    }
+    b->iteration_indptr_.push_back((int)b->trees_.size());
+  }
   return b;
 }
 

@@ -29,7 +29,8 @@ class XGBModel:
 
     # ---- sklearn plumbing
     def get_params(self, deep=True):
-        p = {k: getattr(self, k) for k in self.__init__.__code__.co_varnames[1:self.__init__.__code__.co_argcount]}
+        code = XGBModel.__init__.__code__
+        p = {k: getattr(self, k) for k in code.co_varnames[1:code.co_argcount]}
         p.update(self.kwargs)
         return p
 
@@ -156,3 +157,32 @@ class XGBClassifier(XGBModel):
             return XGBModel.predict(self, X, True, validate_features, base_margin, iteration_range)
         p = self.predict_proba(X, validate_features, base_margin, iteration_range)
         return np.argmax(p, axis=1)
+
+
+class _RandomForest:
+    """Random forests the way `xgboost.sklearn` builds them: one boosting round of `n_estimators` parallel trees
+    (num_parallel_tree), each on its own row and column sample, with learning rate 1 and almost no L2 penalty."""
+
+    def __init__(self, *, learning_rate=1.0, subsample=0.8, colsample_bynode=0.8, reg_lambda=1e-5, **kwargs):
+        super().__init__(learning_rate=learning_rate, subsample=subsample, colsample_bynode=colsample_bynode, reg_lambda=reg_lambda, **kwargs)
+
+    def get_xgb_params(self):
+        p = super().get_xgb_params()
+        p["num_parallel_tree"] = super().get_num_boosting_rounds()
+        return p
+
+    def get_num_boosting_rounds(self):
+        return 1
+
+    def _fit(self, *args, **kwargs):
+        if self.early_stopping_rounds is not None or self.callbacks:
+            raise NotImplementedError("`early_stopping_rounds` and `callbacks` are not implemented for random forest.")
+        return super()._fit(*args, **kwargs)
+
+
+class XGBRFRegressor(_RandomForest, XGBRegressor):
+    pass
+
+
+class XGBRFClassifier(_RandomForest, XGBClassifier):
+    pass
