@@ -192,6 +192,9 @@ XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, i
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
 XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
+/* the configured objective's gradient pairs on `dmat` at the given margins (n x num_class, host), with the row sample of boosting
+ * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x num_class x 2 floats (g, h) */
+XGB_DLL int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair);
 /* CUDA-event stopwatch on the engine's stream: Start records an event, Stop records another, waits, returns ms */
 XGB_DLL int XGB200TimerStart(void);
 XGB_DLL int XGB200TimerStop(float* out_ms);

@@ -429,6 +429,16 @@ class CudaBackend:
         self._check(self.lib.XGB200BoosterGetCachedMargin(bh, dh, out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
 
+    def booster_compute_gradient(self, bh, dh, margin, round=0):
+        """The configured objective's (g, h) at the given margins with round `round`'s row sample: float32 (n, K, 2)
+        (include/b200xgb.h XGB200BoosterComputeGradient)."""
+        n = self.dmatrix_num_row(dh)
+        margin = np.ascontiguousarray(margin, np.float32).reshape(n, -1)
+        out = np.zeros((n, margin.shape[1], 2), np.float32)
+        self._check(self.lib.XGB200BoosterComputeGradient(bh, dh, margin.ctypes.data_as(C.POINTER(C.c_float)), C.c_int(int(round)),
+                                                          out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out
+
     def booster_tree_weights(self, bh):
         """Each tree's weight in model order (booster=dart: weight_drop; all 1 for gbtree)."""
         n = c_bst_ulong()

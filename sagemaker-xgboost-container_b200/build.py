@@ -14,10 +14,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "lib", "libb200xgb.so")
-SOURCES = ["hist.cu", "tree.cu", "misc.cu", "quantile.cu", "auc.cu", "shap.cu", "dart.cu", "csv.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
+SOURCES = ["hist.cu", "tree.cu", "misc.cu", "quantile.cu", "auc.cu", "shap.cu", "dart.cu", "survival.cu", "csv.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
          "-diag-suppress", "177", "-I", os.path.join(HERE, "..", "include")]
+# survival.cu computes its objectives in double: no fused multiply-adds, so they round like a host restatement of the formulas
+EXTRA_FLAGS = {"survival.cu": ["--fmad=false"]}
 
 
 def _newest_header():
@@ -34,7 +36,7 @@ def _compile(src, force):
     sp = os.path.join(CSRC, src)
     if not force and os.path.exists(obj) and os.path.getmtime(obj) > max(os.path.getmtime(sp), _newest_header()):
         return obj, False
-    cmd = [NVCC] + FLAGS + (["-x", "cu"] if src.endswith(".cc") else []) + ["-c", sp, "-o", obj]
+    cmd = [NVCC] + FLAGS + EXTRA_FLAGS.get(src, []) + (["-x", "cu"] if src.endswith(".cc") else []) + ["-c", sp, "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (src, r.stdout, r.stderr))

@@ -83,6 +83,10 @@ class DMatrix:
             self.set_weight(weight)
         if base_margin is not None:
             self.set_base_margin(base_margin)
+        if label_lower_bound is not None:
+            self.set_float_info("label_lower_bound", label_lower_bound)
+        if label_upper_bound is not None:
+            self.set_float_info("label_upper_bound", label_upper_bound)
         if feature_names is not None:
             self.feature_names = feature_names
         if feature_types is not None:
@@ -160,13 +164,18 @@ class DMatrix:
     def get_base_margin(self):
         return self.get_float_info("base_margin")
 
-    def set_info(self, *, label=None, weight=None, base_margin=None, feature_names=None, feature_types=None, **kwargs):
+    def set_info(self, *, label=None, weight=None, base_margin=None, label_lower_bound=None, label_upper_bound=None, feature_names=None,
+                 feature_types=None, **kwargs):
         if label is not None:
             self.set_label(label)
         if weight is not None:
             self.set_weight(weight)
         if base_margin is not None:
             self.set_base_margin(base_margin)
+        if label_lower_bound is not None:
+            self.set_float_info("label_lower_bound", label_lower_bound)
+        if label_upper_bound is not None:
+            self.set_float_info("label_upper_bound", label_upper_bound)
         if feature_names is not None:
             self.feature_names = feature_names
         if feature_types is not None:
@@ -235,7 +244,7 @@ _IGNORED_PARAMS = {
     "deterministic_histogram", "single_precision_histogram", "updater", "refresh_leaf", "process_type", "device", "gpu_id",
     "sampling_method", "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
     "lambda_bias", "feature_selector", "top_k",
-    "aft_loss_distribution", "aft_loss_distribution_scale", "disable_default_eval_metric",
+    "disable_default_eval_metric",
     "multi_strategy", "max_cached_hist_node", "random_state",
 }
 

@@ -114,6 +114,8 @@ std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len) const {
     for (int64_t i = 0; i < len; ++i) for (size_t k = 0; k < per_row; ++k) o[i * per_row + k] = src[(size_t)idx[i] * per_row + k]; return o; };
   if (!labels.empty()) { auto v = take(labels, 1); dm->set_float_info("label", v.data(), v.size()); }
   if (!weights.empty()) { auto v = take(weights, 1); dm->set_float_info("weight", v.data(), v.size()); }
+  if (!label_lower.empty()) { auto v = take(label_lower, 1); dm->set_float_info("label_lower_bound", v.data(), v.size()); }
+  if (!label_upper.empty()) { auto v = take(label_upper, 1); dm->set_float_info("label_upper_bound", v.data(), v.size()); }
   if (!base_margin.empty() && n > 0) { size_t per = base_margin.size() / n; auto v = take(base_margin, per); dm->set_float_info("base_margin", v.data(), v.size()); }
   return dm;
 }
@@ -124,7 +126,9 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
     h.assign(v, v + len); d.alloc(len);
     if (len) { CUDA_OK(cudaMemcpyAsync(d.p, h.data(), sizeof(float) * len, cudaMemcpyHostToDevice, s)); Comm::get().sync_stream(s); }
   };
-  if (field == "label") put(labels, d_labels);
+  if (field == "label") { put(labels, d_labels); cox_order.valid = false; }
+  else if (field == "label_lower_bound") put(label_lower, d_label_lower);      // survival:aft; the bins do not depend on them
+  else if (field == "label_upper_bound") put(label_upper, d_label_upper);
   else if (field == "weight") {
     for (size_t i = 0; i < len; ++i) B200_CHECK(v[i] >= 0 && !std::isnan(v[i]), "Weights must be positive values.");
     put(weights, d_weights);
@@ -138,6 +142,8 @@ const std::vector<float>& DMatrix::get_float_info(const std::string& field) cons
   if (field == "label") return labels;
   if (field == "weight") return weights;
   if (field == "base_margin") return base_margin;
+  if (field == "label_lower_bound") return label_lower;
+  if (field == "label_upper_bound") return label_upper;
   throw Error("Unknown float field name: " + field);
 }
 
@@ -280,7 +286,7 @@ static const std::map<std::string, int>& objective_table() {
   static const std::map<std::string, int> t = {{"reg:squarederror", kSquaredError}, {"reg:linear", kSquaredError}, {"binary:logistic", kBinaryLogistic},
     {"reg:logistic", kRegLogistic}, {"binary:logitraw", kLogitRaw}, {"multi:softprob", kSoftprob}, {"multi:softmax", kSoftmax},
     {"reg:squaredlogerror", kSquaredLogError}, {"reg:pseudohubererror", kPseudoHuber}, {"count:poisson", kPoisson}, {"reg:gamma", kGamma},
-    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}};
+    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}};
   return t;
 }
 
@@ -300,7 +306,7 @@ void Booster::configure() {
   auto ito = raw_params_.find("objective");
   if (ito != raw_params_.end()) objective_name_ = ito->second;
   auto ot = objective_table().find(objective_name_);
-  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax)");
+  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
   p.objective = ot->second;
   if (objective_name_ == "reg:linear") objective_name_ = "reg:squarederror";
   p.num_class = (p.objective == kSoftprob || p.objective == kSoftmax) ? geti("num_class", 0) : 1;
@@ -322,6 +328,16 @@ void Booster::configure() {
   p.huber_slope = getf("huber_slope", nullptr, 1.0f); p.tweedie_variance_power = getf("tweedie_variance_power", nullptr, 1.5f);
   B200_CHECK(p.huber_slope != 0.0f, "Check failed: slope != 0.0 (huber_slope)");
   B200_CHECK(p.tweedie_variance_power >= 1.0f && p.tweedie_variance_power < 2.0f, "tweedie_variance_power must be in interval [1, 2)");
+  if (p.objective == kAft) {      // the AFT parameters are read (and checked) only under survival:aft
+    if (auto d = raw_params_.find("aft_loss_distribution"); d != raw_params_.end()) {
+      if (d->second == "normal") p.aft_dist = kAftNormal;
+      else if (d->second == "logistic") p.aft_dist = kAftLogistic;
+      else if (d->second == "extreme") p.aft_dist = kAftExtreme;
+      else throw Error("Invalid aft_loss_distribution: " + d->second + " (normal, logistic, extreme)");
+    }
+    p.aft_sigma = getf("aft_loss_distribution_scale", nullptr, 1.0f);
+    B200_CHECK(p.aft_sigma > 0.0f && std::isfinite(p.aft_sigma), "aft_loss_distribution_scale must be a finite number > 0 (got " + std::to_string(p.aft_sigma) + ")");
+  }
   // count:poisson: max_delta_step defaults to 0.7 for the objective's hessian AND the tree's leaf clipping (upstream learner.cc sets
   // the shared parameter when the user did not)
   if (p.objective == kPoisson) {
@@ -407,7 +423,7 @@ void Booster::configure() {
 
 float Booster::base_margin() const {
   if (objective_is_logistic(param_.objective)) return -std::log(1.0f / base_score_ - 1.0f);
-  if (objective_is_log_link(param_.objective)) return std::log(base_score_);          // ProbToMargin of the log-link objectives
+  if (objective_is_log_link(param_.objective) || objective_is_survival(param_.objective)) return std::log(base_score_);   // ProbToMargin of the log-link objectives
   return base_score_;
 }
 
@@ -422,7 +438,7 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
   if (param_.objective == kSoftprob || param_.objective == kSoftmax) { base_score_ = 0.5f; return; }
   // 3.0.x fits the intercept for the RegLossObj family only; the log-link objectives and binary:hinge keep the 0.5 default
   // [UPSTREAM-RECALL: src/objective/init_estimation.cc; later releases changed the GLM objectives]
-  if (objective_is_log_link(param_.objective) || param_.objective == kHinge) { base_score_ = 0.5f; return; }
+  if (objective_is_log_link(param_.objective) || param_.objective == kHinge || objective_is_survival(param_.objective)) { base_score_ = 0.5f; return; }
   cudaStream_t s = engine_stream();
   TreeBuilder& b = *builder_;
   GradArgs ga{}; ga.margin = nullptr; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
@@ -620,6 +636,12 @@ static void check_labels(const DMatrix* dm) {
   B200_CHECK(dm->labels.size() == (size_t)dm->n, "Check failed: preds.size() == info.labels_.size() (" + std::to_string(dm->n) + " vs. " +
              std::to_string(dm->labels.size()) + ") : labels are not correctly provided");
 }
+// survival:aft reads the interval bounds instead of the label
+static void check_aft_bounds(const DMatrix* dm) {
+  B200_CHECK(dm->label_lower.size() == (size_t)dm->n && dm->label_upper.size() == (size_t)dm->n,
+             "survival:aft needs label_lower_bound and label_upper_bound with one entry per row (" + std::to_string(dm->n) + " rows, " +
+             std::to_string(dm->label_lower.size()) + " lower and " + std::to_string(dm->label_upper.size()) + " upper bounds)");
+}
 static void check_train_width(const DMatrix* dm) {
   B200_CHECK(dm->F <= kMaxTrainFeatures, "the CUDA hist builder trains on at most " + std::to_string(kMaxTrainFeatures) + " features (the data has " +
              std::to_string(dm->F) + ")");
@@ -629,7 +651,8 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   configure();
   (void)iter;
   cudaStream_t s = engine_stream();
-  check_labels(dtrain);
+  if (param_.objective == kAft) check_aft_bounds(dtrain); else check_labels(dtrain);
+  B200_CHECK(param_.objective != kCox || !Comm::get().distributed(), "survival:cox is not supported with more than one GPU (world_size > 1): its risk sets span the rows of every rank");
   if (num_feature_ == 0) num_feature_ = dtrain->F;
   B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
              " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
@@ -649,6 +672,12 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
     if (param_.objective == kPoisson) for (float v : y) B200_CHECK(v >= 0.0f, "PoissonRegression: label must be nonnegative");
     if (param_.objective == kGamma) for (float v : y) B200_CHECK(v > 0.0f, "GammaRegression: label must be positive.");
     if (param_.objective == kTweedie) for (float v : y) B200_CHECK(v >= 0.0f, "TweedieRegression: label must be nonnegative");
+    if (param_.objective == kAft)
+      for (int64_t i = 0; i < dtrain->n; ++i) {
+        const float lo = dtrain->label_lower[i], hi = dtrain->label_upper[i];
+        B200_CHECK(lo >= 0.0f, "survival:aft: label_lower_bound must be >= 0 (row " + std::to_string(i) + ": " + std::to_string(lo) + ")");
+        B200_CHECK(hi >= lo, "survival:aft: label_upper_bound must be >= label_lower_bound (row " + std::to_string(i) + ": " + std::to_string(lo) + " > " + std::to_string(hi) + ")");
+      }
     labels_checked_ = true;
   }
   estimate_base_score(dtrain);
@@ -667,12 +696,10 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   const float* grad_margin = dart_.on ? dart_begin_round(dtrain, cache, round) : cache.margin.p;
   // ---- gradients + fixed-point scales
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
-  GradArgs ga{}; ga.margin = grad_margin; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
-  ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = b.gs.absmax; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = K; ga.objective = param_.objective;
-  ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = param_.subsample; ga.seed = param_.seed; ga.iter = (unsigned long long)round;
-  ga.row_offset = (int64_t)Comm::get().rank() << 40; ga.aux = objective_aux(param_);
-  if (per_tree_sample) { forest_gpair_.ensure((size_t)b.gp_stride * K); ga.gpair = forest_gpair_.p; ga.absmax = nullptr; ga.subsample = 1.0f; }
-  launch_gradient(ga, s);
+  if (per_tree_sample) {
+    forest_gpair_.ensure((size_t)b.gp_stride * K);
+    launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f);
+  } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample);
   if (!per_tree_sample) {
     Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
     launch_scales(b.gs, grad_bits_for(b.global_n), s);
@@ -684,7 +711,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
       if (per_tree_sample) {     // tree j's rows (shared by the K classes): j = 0 draws the stream a single tree draws
         CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
         SampleArgs sa{}; sa.src = forest_gpair_.p; sa.dst = b.gpair.p; sa.absmax = b.gs.absmax; sa.gp_stride = b.gp_stride; sa.n = dtrain->n;
-        sa.row_offset = ga.row_offset; sa.K = K; sa.subsample = param_.subsample; sa.seed = param_.seed;
+        sa.row_offset = (int64_t)Comm::get().rank() << 40; sa.K = K; sa.subsample = param_.subsample; sa.seed = param_.seed;
         sa.stream = j == 0 ? 0x2000ull + (uint64_t)round : kForestRowStream + ((uint64_t)round << 20) + (uint64_t)j;
         launch_sample_gpair(sa, s);
         Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
@@ -693,6 +720,45 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
       grow_one_tree(dtrain, cache, k, iteration_indptr_[round] + k * P + j);
     }
   iteration_indptr_.push_back((int)trees_.size());
+}
+
+// The objective's gradient pairs at `margin` into gpair ([K][gp_stride]), rows outside round `round`'s sample zeroed, max|g| and
+// max h folded into absmax (nullptr: not taken).  The survival objectives have their own kernels (survival.cu); every other
+// objective runs gradient_kernel.
+void Booster::launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample) {
+  cudaStream_t s = engine_stream();
+  const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
+  if (objective_is_survival(param_.objective)) {
+    SurvivalGradArgs sa{}; sa.margin = margin; sa.label = dm->d_labels.p; sa.lower = dm->d_label_lower.p; sa.upper = dm->d_label_upper.p;
+    sa.weight = dm->weights.empty() ? nullptr : dm->d_weights.p; sa.gpair = gpair; sa.absmax = absmax; sa.n = dm->n; sa.row_offset = row_offset;
+    sa.subsample = subsample; sa.seed = param_.seed; sa.iter = (unsigned long long)round; sa.dist = param_.aft_dist; sa.sigma = param_.aft_sigma;
+    if (param_.objective == kAft) { launch_aft_gradient(sa, s); return; }
+    if (!dm->cox_order.valid) cox_sort(dm->d_labels.p, dm->n, &dm->cox_order, &cox_scratch_, s);
+    launch_cox_gradient(sa, dm->cox_order, &cox_scratch_, s);
+    return;
+  }
+  GradArgs ga{}; ga.margin = margin; ga.label = dm->d_labels.p; ga.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
+  ga.gpair = gpair; ga.gp_stride = gp_stride; ga.absmax = absmax; ga.err = builder_->err.p; ga.n = dm->n; ga.row_offset = row_offset; ga.K = param_.num_class;
+  ga.objective = param_.objective; ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = subsample; ga.seed = param_.seed;
+  ga.iter = (unsigned long long)round; ga.aux = objective_aux(param_);
+  launch_gradient(ga, s);
+}
+
+void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float* out) {
+  configure();
+  cudaStream_t s = engine_stream();
+  if (param_.objective == kAft) check_aft_bounds(dm); else check_labels(dm);
+  dm->ensure_binned(param_.max_bin); builder_for(dm);        // the builder owns the label-error flag gradient_kernel writes
+  const int K = param_.num_class;
+  const int64_t n = dm->n;
+  DevBuf<float> d_margin; DevBuf<float2> d_gp; d_margin.alloc((size_t)n * K); d_gp.alloc((size_t)n * K);
+  if (n) CUDA_OK(cudaMemcpyAsync(d_margin.p, margin, sizeof(float) * n * K, cudaMemcpyHostToDevice, s));
+  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample);
+  std::vector<float2> h((size_t)n * K);
+  if (n) CUDA_OK(cudaMemcpyAsync(h.data(), d_gp.p, sizeof(float2) * h.size(), cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
+  for (int64_t r = 0; r < n; ++r)
+    for (int k = 0; k < K; ++k) { out[(r * K + k) * 2] = h[(size_t)k * n + r].x; out[(r * K + k) * 2 + 1] = h[(size_t)k * n + r].y; }
 }
 
 // grow_policy=lossguide: expansions per tree = leaves - 1, bounded by max_leaves or by a full tree of max_depth
@@ -778,6 +844,8 @@ static std::string default_metric(const TrainParam& p) {
     case kGamma: return "gamma-nloglik";
     case kTweedie: { char buf[64]; snprintf(buf, sizeof buf, "tweedie-nloglik@%g", (double)p.tweedie_variance_power); return buf; }
     case kHinge: return "error";
+    case kAft: return "aft-nloglik";
+    case kCox: return "cox-nloglik";
     default: return "mlogloss";
   }
 }
@@ -791,7 +859,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
   std::string out = "[" + std::to_string(iter) + "]";
   for (size_t i = 0; i < dms.size(); ++i) {
     DMatrix* dm = dms[i];
-    check_labels(dm);
+    if (param_.objective != kAft) check_labels(dm);
     PredCache& c = cache_for(dm);
     bring_cache_up_to_date(dm, c);
     for (const std::string& mname : metrics) {
@@ -822,19 +890,32 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         out += "\t" + names[i] + "-" + mname + ":" + buf;
         continue;
       }
-      if (base == "rmse") ma.metric = kMetricRmse; else if (base == "mse") ma.metric = kMetricRmse; else if (base == "mae") ma.metric = kMetricMae;
-      else if (base == "logloss") ma.metric = kMetricLogloss; else if (base == "error") ma.metric = kMetricError;
-      else if (base == "merror") ma.metric = kMetricMerror; else if (base == "mlogloss") ma.metric = kMetricMlogloss;
-      else if (base == "rmsle") ma.metric = kMetricRmsle; else if (base == "mape") ma.metric = kMetricMape;
-      else if (base == "mphe") { ma.metric = kMetricMphe; ma.aux = param_.huber_slope; }
-      else if (base == "poisson-nloglik") ma.metric = kMetricPoissonNll; else if (base == "gamma-nloglik") ma.metric = kMetricGammaNll;
-      else if (base == "gamma-deviance") ma.metric = kMetricGammaDeviance;
-      else if (base == "tweedie-nloglik") { ma.metric = kMetricTweedieNll; if (ma.aux == 0.0f) throw Error("tweedie-nloglik needs its variance power: tweedie-nloglik@rho"); }
-      else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho)");
-      if (param_.objective == kLogitRaw && (ma.metric == kMetricLogloss || ma.metric == kMetricError)) ma.is_logistic = 1;
-      if ((ma.metric == kMetricMerror || ma.metric == kMetricMlogloss)) B200_CHECK(param_.num_class > 1, "Check failed: preds.size() == info.labels_.size() : label and prediction size not match, hint: use merror or mlogloss for multi-class classification");
-      CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
-      launch_metric(ma, s);
+      if (mname == "aft-nloglik" || mname == "interval-regression-accuracy") {     // at the margin, in double (survival.cu)
+        check_aft_bounds(dm);
+        CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
+        launch_aft_metric(c.margin.p, dm->d_label_lower.p, dm->d_label_upper.p, ma.weight, dm->n, param_.aft_dist, param_.aft_sigma,
+                          mname == "aft-nloglik" ? 0 : 1, dsum_.p, s);
+      } else if (mname == "cox-nloglik") {        // unweighted, per event, with the deterministic risk-set sums of survival:cox
+        B200_CHECK(!Comm::get().distributed(), "cox-nloglik is not supported with more than one GPU (world_size > 1)");
+        check_labels(dm);
+        if (!dm->cox_order.valid) cox_sort(dm->d_labels.p, dm->n, &dm->cox_order, &cox_scratch_, s);
+        cox_nloglik(c.margin.p, dm->n, dm->cox_order, &cox_scratch_, dsum_.p, s);
+      } else {
+        if (param_.objective == kAft) check_labels(dm);
+        if (base == "rmse") ma.metric = kMetricRmse; else if (base == "mse") ma.metric = kMetricRmse; else if (base == "mae") ma.metric = kMetricMae;
+        else if (base == "logloss") ma.metric = kMetricLogloss; else if (base == "error") ma.metric = kMetricError;
+        else if (base == "merror") ma.metric = kMetricMerror; else if (base == "mlogloss") ma.metric = kMetricMlogloss;
+        else if (base == "rmsle") ma.metric = kMetricRmsle; else if (base == "mape") ma.metric = kMetricMape;
+        else if (base == "mphe") { ma.metric = kMetricMphe; ma.aux = param_.huber_slope; }
+        else if (base == "poisson-nloglik") ma.metric = kMetricPoissonNll; else if (base == "gamma-nloglik") ma.metric = kMetricGammaNll;
+        else if (base == "gamma-deviance") ma.metric = kMetricGammaDeviance;
+        else if (base == "tweedie-nloglik") { ma.metric = kMetricTweedieNll; if (ma.aux == 0.0f) throw Error("tweedie-nloglik needs its variance power: tweedie-nloglik@rho"); }
+        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik)");
+        if (param_.objective == kLogitRaw && (ma.metric == kMetricLogloss || ma.metric == kMetricError)) ma.is_logistic = 1;
+        if ((ma.metric == kMetricMerror || ma.metric == kMetricMlogloss)) B200_CHECK(param_.num_class > 1, "Check failed: preds.size() == info.labels_.size() : label and prediction size not match, hint: use merror or mlogloss for multi-class classification");
+        CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
+        launch_metric(ma, s);
+      }
       Comm::get().allreduce_sum_f64(dsum_.p, 2, s);
       double h[2];
       CUDA_OK(cudaMemcpyAsync(h, dsum_.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, s));

@@ -8,6 +8,7 @@
 #include "grow.h"
 #include "json.h"
 #include "misc.h"
+#include "survival.h"
 #include "tree.h"
 
 namespace b200 {
@@ -22,6 +23,9 @@ class DMatrix {
   DevBuf<float> X;                                    // n x F, NaN = missing
   std::vector<float> labels, weights, base_margin;    // host copies (returned by GetFloatInfo)
   DevBuf<float> d_labels, d_weights, d_base_margin;
+  std::vector<float> label_lower, label_upper;         // survival:aft interval bounds (label_lower_bound / label_upper_bound)
+  DevBuf<float> d_label_lower, d_label_upper;
+  CoxOrder cox_order;                                 // survival:cox: the rows sorted by |label|, built on first use, reset with the labels
   std::vector<std::string> feature_names, feature_types;
   // binned representation (built on first use as a training matrix)
   bool binned = false; int binned_max_bin = 0;
@@ -120,6 +124,8 @@ class Booster {
   int num_class() const { return param_.num_class; }
   const TrainParam& param() { configure(); return param_; }
   void set_profile(bool on);
+  // the configured objective's gradient pairs at the given host margins [n][K], with round `round`'s row sample; out [n][K][2]
+  void debug_gradient(DMatrix* dm, const float* margin, int round, float* out);
   std::string get_profile();                      // JSON, see include/b200xgb.h
   // histogram of one node for kernel-level parity tests / the roofline bench
   // mode: 0 = production choice (TMA root kernel), 1 = gather kernel, 2 = G-only TMA root kernel (H plane stays zero);
@@ -162,6 +168,7 @@ class Booster {
   std::map<uint64_t, PredCache> caches_;
   std::unique_ptr<TreeBuilder> builder_ = std::make_unique<TreeBuilder>();   // its device buffers are sized by builder_for
   DevBuf<double> dsum_;                         // device sums of the metrics and of the base-score stump
+  CoxScratch cox_scratch_;                      // survival:cox: per-round scratch of the gradient and of cox-nloglik
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1
@@ -182,6 +189,7 @@ class Booster {
   TreeBuilder& builder_for(DMatrix* dm);             // the builder sized for the binned dm and the parameters
   TreeInputs tree_inputs(const DMatrix& dm, const std::string& mask, int tree_index, float* margin, int k);
   void grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_index);
+  void launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample);
   JPtr model_to_json();
   void model_from_json(const JValue& doc);
   JPtr config_to_json();

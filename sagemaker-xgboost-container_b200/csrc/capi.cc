@@ -536,6 +536,12 @@ int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out
   if (out) memcpy(out, w.data(), sizeof(float) * w.size());
   API_END();
 }
+int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair) {
+  API_BEGIN();
+  B200_CHECK(round >= 0, "XGB200BoosterComputeGradient: round must be >= 0");
+  BST(handle)->debug_gradient(DM(dmat), margin, round, out_gpair);
+  API_END();
+}
 int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out) {
   API_BEGIN();
   std::vector<float> v;

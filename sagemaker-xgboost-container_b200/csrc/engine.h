@@ -93,15 +93,17 @@ inline size_t hist_slot_entries(int ngroups, int tw) { return (size_t)ngroups * 
 // reference: src/sagemaker_xgboost_container/algorithm_mode/hyperparameter_validation.py:141-346)
 // ---------------------------------------------------------------------------------------------
 enum Objective : int { kSquaredError = 0, kBinaryLogistic = 1, kRegLogistic = 2, kLogitRaw = 3, kSoftprob = 4, kSoftmax = 5,
-                       kSquaredLogError = 6, kPseudoHuber = 7, kPoisson = 8, kGamma = 9, kTweedie = 10, kHinge = 11 };
+                       kSquaredLogError = 6, kPseudoHuber = 7, kPoisson = 8, kGamma = 9, kTweedie = 10, kHinge = 11,
+                       kAft = 12, kCox = 13 };       // survival objectives: own gradient kernels (survival.cu), not gradient_kernel
 // prediction transform of an objective (upstream ObjFunction::PredTransform / ProbToMargin): 0 identity, 1 sigmoid / logit,
-// 2 exp / log (count:poisson, reg:gamma, reg:tweedie), 3 step at 0 (binary:hinge; its margin is the raw score)
+// 2 exp / log (count:poisson, reg:gamma, reg:tweedie, survival:aft, survival:cox), 3 step at 0 (binary:hinge; its margin is the raw score)
 enum Transform : int { kTransformNone = 0, kTransformSigmoid = 1, kTransformExp = 2, kTransformHinge = 3 };
 inline bool objective_is_logistic(int o) { return o == kBinaryLogistic || o == kRegLogistic || o == kLogitRaw; }
 inline bool objective_is_log_link(int o) { return o == kPoisson || o == kGamma || o == kTweedie; }
+inline bool objective_is_survival(int o) { return o == kAft || o == kCox; }
 inline int objective_transform(int o) {
   if (o == kBinaryLogistic || o == kRegLogistic) return kTransformSigmoid;
-  if (objective_is_log_link(o)) return kTransformExp;
+  if (objective_is_log_link(o) || objective_is_survival(o)) return kTransformExp;
   return o == kHinge ? kTransformHinge : kTransformNone;
 }
 
@@ -115,6 +117,7 @@ struct TrainParam {
   unsigned seed = 0;
   int num_parallel_tree = 1;    // trees per class per boosting round (boosted random forests)
   float huber_slope = 1.0f, tweedie_variance_power = 1.5f, poisson_max_delta_step = 0.7f;   // objective parameters (upstream defaults)
+  int aft_dist = 0; float aft_sigma = 1.0f;     // survival:aft: aft_loss_distribution (survival.h AftDist), aft_loss_distribution_scale
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(256) transform_kernel(float* m, int64_t n, int
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
   if (objective == kBinaryLogistic || objective == kRegLogistic) m[r] = sigmoidf_xgb(m[r]);
-  else if (objective == kPoisson || objective == kGamma || objective == kTweedie) m[r] = expf(m[r]);
+  else if (objective == kPoisson || objective == kGamma || objective == kTweedie || objective == kAft || objective == kCox) m[r] = expf(m[r]);
   else if (objective == kHinge) m[r] = m[r] > 0.0f ? 1.0f : 0.0f;
   else if (objective == kSoftprob || objective == kSoftmax) {
     float* p = m + r * K;

@@ -20,6 +20,13 @@ static std::string float_repr(float v) {       // shortest round-trip, xgboost s
   return mant + "E" + std::to_string(ex);
 }
 static JPtr S(const std::string& s) { return JValue::Str(s); }
+// the AFT parameter block into raw parameters (read back, and range-checked, only under survival:aft by configure)
+static void aft_params_from_json(const JValue& obj, std::map<std::string, std::string>* raw) {
+  auto ap = obj.get("aft_loss_param");
+  if (!ap) return;
+  if (auto v = ap->get("aft_loss_distribution")) (*raw)["aft_loss_distribution"] = v->s;
+  if (auto v = ap->get("aft_loss_distribution_scale")) (*raw)["aft_loss_distribution_scale"] = v->type == JValue::kString ? v->s : float_repr((float)v->as_double());
+}
 
 // per-objective parameter block of the model / config documents (upstream ObjFunction::SaveConfig)
 static void objective_params_to_json(JValue& obj, const TrainParam& p) {
@@ -28,7 +35,11 @@ static void objective_params_to_json(JValue& obj, const TrainParam& p) {
     case kPoisson: rp->set("max_delta_step", S(float_repr(p.poisson_max_delta_step))); obj.set("poisson_regression_param", rp); break;
     case kTweedie: rp->set("tweedie_variance_power", S(float_repr(p.tweedie_variance_power))); obj.set("tweedie_regression_param", rp); break;
     case kPseudoHuber: rp->set("huber_slope", S(float_repr(p.huber_slope))); obj.set("pseudo_huber_param", rp); break;
-    case kGamma: case kHinge: break;
+    case kGamma: case kHinge: case kCox: break;
+    case kAft: {
+      static const char* dist[] = {"normal", "logistic", "extreme"};
+      rp->set("aft_loss_distribution", S(dist[p.aft_dist])); rp->set("aft_loss_distribution_scale", S(float_repr(p.aft_sigma)));
+      obj.set("aft_loss_param", rp); break; }
     default: rp->set("scale_pos_weight", S(float_repr(p.scale_pos_weight))); obj.set("reg_loss_param", rp); break;
   }
 }
@@ -118,6 +129,7 @@ void Booster::model_from_json(const JValue& doc) {
   if (auto pp = obj.get("poisson_regression_param")) if (auto v = pp->get("max_delta_step")) raw_params_["max_delta_step"] = std::to_string(v->as_double());
   if (auto tp = obj.get("tweedie_regression_param")) if (auto v = tp->get("tweedie_variance_power")) raw_params_["tweedie_variance_power"] = std::to_string(v->as_double());
   if (auto hp = obj.get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = std::to_string(v->as_double());
+  aft_params_from_json(obj, &raw_params_);
   const JValue& lmp = learner.at("learner_model_param");
   num_feature_ = (int)lmp.at("num_feature").as_int();
   int nc = lmp.has("num_class") ? (int)lmp.at("num_class").as_int() : 0;
@@ -294,6 +306,7 @@ void Booster::config_from_json(const JValue& doc) {
     if (auto pp = o->get("poisson_regression_param")) if (auto v = pp->get("max_delta_step")) raw_params_["max_delta_step"] = v->s;
     if (auto tp = o->get("tweedie_regression_param")) if (auto v = tp->get("tweedie_variance_power")) raw_params_["tweedie_variance_power"] = v->s;
     if (auto hp = o->get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = v->s;
+    aft_params_from_json(*o, &raw_params_);
   }
   if (auto m = learner.get("metrics")) { eval_metrics_.clear(); for (auto& x : m->arr) eval_metrics_.push_back(x->at("name").s); }
   configured_ = false;
