@@ -154,6 +154,15 @@ XGB_DLL int XGB200DMatrixCreateFromColumns(const void* const* cols, const int* c
 XGB_DLL int XGB200DMatrixGetRaw(DMatrixHandle handle, float* out_row_major);
 /* binned feature blocks back on the host in plain row-major n x F order (for bit-exact checks of the binning kernel) */
 XGB_DLL int XGB200DMatrixGetBins(DMatrixHandle handle, int max_bin, uint8_t* out_row_major);
+/* the two other binned copies the kernels read: the 128 B line-aligned row copy (built when the main block is 96 B wide;
+ * *out_aligned_stride = 128 and out_aligned gets n x 128 bytes, else *out_aligned_stride = 0 and out_aligned is not written)
+ * and the column-major copy (out_col: F x n).  Any pointer may be NULL. */
+XGB_DLL int XGB200DMatrixGetBinCopies(DMatrixHandle handle, int max_bin, int* out_aligned_stride, uint8_t* out_aligned, uint8_t* out_col);
+/* the multi-GPU cut recipe run on one GPU: rows [row_bounds[r], row_bounds[r + 1]) of `handle` (r < n_ranges, covering all rows)
+ * stand for rank r's shard; each gets the capped per-rank summary, the summaries are merged in rank order and the cuts derived
+ * as every rank would.  Does not touch the matrix's own cuts.  out_ptrs: F+1, out_vals: capacity F x 256, out_mins: F. */
+XGB_DLL int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_bounds, int n_ranges, int* out_ptrs,
+                          float* out_vals, float* out_mins);
 /* flat tree arrays of the model; any pointer may be NULL. tree_offset has num_trees+1 entries. */
 XGB_DLL int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class);
 XGB_DLL int XGB200BoosterExportModel(BoosterHandle handle, int64_t* tree_offset, int32_t* tree_info, int32_t* left, int32_t* right,

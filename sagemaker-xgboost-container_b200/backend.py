@@ -353,6 +353,32 @@ class CudaBackend:
         self._check(self.lib.XGB200DMatrixGetBins(h, C.c_int(max_bin), out.ctypes.data_as(C.POINTER(C.c_uint8))))
         return out
 
+    def dmatrix_get_bin_copies(self, h, max_bin):
+        """(aligned, col): the 128 B line-aligned row copy as [n][128] uint8 (None when the matrix has none) and the
+        column-major copy as [F][n] uint8 (include/b200xgb.h XGB200DMatrixGetBinCopies)."""
+        n, F = self.dmatrix_num_row(h), self.dmatrix_num_col(h)
+        stride = C.c_int()
+        self._check(self.lib.XGB200DMatrixGetBinCopies(h, C.c_int(max_bin), C.byref(stride), None, None))
+        aligned = np.zeros((n, stride.value), np.uint8) if stride.value else None
+        col = np.zeros((F, n), np.uint8)
+        u8 = C.POINTER(C.c_uint8)
+        self._check(self.lib.XGB200DMatrixGetBinCopies(h, C.c_int(max_bin), C.byref(stride),
+                                                       aligned.ctypes.data_as(u8) if aligned is not None else None, col.ctypes.data_as(u8)))
+        return aligned, col
+
+    def dmatrix_rank_cuts(self, h, max_bin, row_bounds):
+        """Cuts of the multi-GPU recipe with rows [row_bounds[r], row_bounds[r+1]) as rank r's shard: (ptrs, vals, mins)
+        (include/b200xgb.h XGB200DMatrixRankCuts)."""
+        F = self.dmatrix_num_col(h)
+        bounds = np.ascontiguousarray(row_bounds, np.int64)
+        ptrs = np.zeros(F + 1, np.int32)
+        vals = np.zeros(max(F, 1) * 256, np.float32)
+        mins = np.zeros(max(F, 1), np.float32)
+        self._check(self.lib.XGB200DMatrixRankCuts(h, C.c_int(max_bin), bounds.ctypes.data_as(C.POINTER(C.c_int64)), C.c_int(len(bounds) - 1),
+                                                   ptrs.ctypes.data_as(C.POINTER(C.c_int)), vals.ctypes.data_as(C.POINTER(C.c_float)),
+                                                   mins.ctypes.data_as(C.POINTER(C.c_float))))
+        return ptrs, vals[:ptrs[-1]].copy(), mins[:F].copy()
+
     def booster_export_model(self, h):
         nt, nn = c_bst_ulong(), c_bst_ulong()
         bs = C.c_float()

@@ -195,7 +195,7 @@ void DMatrix::ensure_binned(int max_bin) {
   } else {
     // every rank summarises its shard (exact when a feature has <= cap distinct values), the summaries are
     // all-gathered and merged, and every rank derives the same cuts.
-    const int cap = 2048;
+    const int cap = kRankSummaryCap;
     int hm = has_missing ? 1 : 0;
     {   // has_missing must agree across ranks (bin code 255 reservation)
       DevBuf<unsigned> flag; flag.alloc(1); unsigned v = (unsigned)hm;
@@ -222,22 +222,19 @@ void DMatrix::ensure_binned(int max_bin) {
     std::vector<unsigned char> all(sendbuf.size() * W);
     CUDA_OK(cudaMemcpyAsync(all.data(), drecv.p, all.size(), cudaMemcpyDeviceToHost, s));
     Comm::get().sync_stream(s);
-    std::vector<FeatureSummary> merged(F);
-    for (int f = 0; f < F; ++f) {
-      std::vector<std::pair<float, double>> pts;
-      for (int r = 0; r < W; ++r) {
+    std::vector<std::vector<FeatureSummary>> per_rank(W, std::vector<FeatureSummary>(F));
+    for (int r = 0; r < W; ++r) {
+      for (int f = 0; f < F; ++f) {
         const unsigned char* p = all.data() + (size_t)r * sendbuf.size() + (size_t)f * rec;
         double cntd; memcpy(&cntd, p, 8); size_t c = (size_t)cntd;
-        const float* v = reinterpret_cast<const float*>(p + 8);
-        std::vector<double> w(c); memcpy(w.data(), p + 8 + per_feat * sizeof(float), sizeof(double) * c);
-        for (size_t i = 0; i < c; ++i) pts.emplace_back(v[i], w[i]);
-      }
-      std::stable_sort(pts.begin(), pts.end(), [](const std::pair<float, double>& a, const std::pair<float, double>& b) { return a.first < b.first; });
-      for (auto& pw : pts) {
-        if (!merged[f].vals.empty() && merged[f].vals.back() == pw.first) merged[f].weights.back() += pw.second;
-        else { merged[f].vals.push_back(pw.first); merged[f].weights.push_back(pw.second); }
+        FeatureSummary& fs = per_rank[r][f];
+        fs.vals.resize(c); fs.weights.resize(c);
+        memcpy(fs.vals.data(), p + 8, sizeof(float) * c);
+        memcpy(fs.weights.data(), p + 8 + per_feat * sizeof(float), sizeof(double) * c);
       }
     }
+    std::vector<FeatureSummary> merged;
+    merge_summaries(per_rank, F, &merged);
     cuts_from_summaries(merged, max_bin, has_missing, &cuts);
   }
   binned_max_bin = max_bin;

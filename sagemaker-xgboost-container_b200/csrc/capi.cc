@@ -423,6 +423,29 @@ int XGB200DMatrixGetBins(DMatrixHandle handle, int max_bin, uint8_t* out_row_maj
     out_row_major[r * dm->F + f] = (size_t)f < W ? h[(size_t)r * W + f] : t[(size_t)r * dm->tw + (f - W)];
   API_END();
 }
+int XGB200DMatrixGetBinCopies(DMatrixHandle handle, int max_bin, int* out_aligned_stride, uint8_t* out_aligned, uint8_t* out_col) {
+  API_BEGIN();
+  DMatrix* dm = DM(handle); dm->ensure_binned(max_bin);
+  const int stride = dm->bins_gather.p ? dm->gather_stride : 0;
+  if (out_aligned_stride) *out_aligned_stride = stride;
+  if (out_aligned && stride && dm->n) CUDA_OK(cudaMemcpy(out_aligned, dm->bins_gather.p, (size_t)dm->n * stride, cudaMemcpyDeviceToHost));
+  if (out_col && dm->n * dm->F) CUDA_OK(cudaMemcpy(out_col, dm->bins_col.p, (size_t)dm->n * dm->F, cudaMemcpyDeviceToHost));
+  API_END();
+}
+int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_bounds, int n_ranges, int* out_ptrs, float* out_vals, float* out_mins) {
+  API_BEGIN();
+  DMatrix* dm = DM(handle);
+  B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
+  B200_CHECK(n_ranges >= 1 && row_bounds[0] == 0 && row_bounds[n_ranges] == dm->n, "XGB200DMatrixRankCuts: the ranges must cover the rows");
+  for (int r = 0; r < n_ranges; ++r) B200_CHECK(row_bounds[r] <= row_bounds[r + 1], "XGB200DMatrixRankCuts: row_bounds must not decrease");
+  HostCuts c;
+  compute_rank_cuts_device(dm->X.p, dm->F, dm->weights.empty() ? nullptr : dm->d_weights.p, row_bounds, n_ranges, max_bin, dm->has_missing, &c,
+                           engine_stream());
+  memcpy(out_ptrs, c.ptrs.data(), sizeof(int) * c.ptrs.size());
+  memcpy(out_vals, c.vals.data(), sizeof(float) * c.vals.size());
+  memcpy(out_mins, c.mins.data(), sizeof(float) * c.mins.size());
+  API_END();
+}
 int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class) {
   API_BEGIN();
   Booster* b = BST(handle); const auto& trees = b->trees();

@@ -98,14 +98,22 @@ void compute_auc_device(const float* margin, const float* label, const float* we
 // quantile.cu: exact weighted-quantile cuts per feature (same definition as oracle/gbt_oracle.c cuts_from_distinct).
 // X: device, row-major n x F. Returns host vectors.
 struct HostCuts { std::vector<int> ptrs; std::vector<float> vals; std::vector<float> mins; };
-// Per-feature summary for distributed merging: distinct values + weights (host), capped.
 void compute_cuts_device(const float* dX, int64_t n, int F, const float* dweights, int max_bin, bool has_missing,
                          HostCuts* out, cudaStream_t s);
 // Distinct-value summary of one rank (for merging cuts across ranks): per feature the sorted distinct values and
-// their weights, exact when a feature has <= cap distinct values, else a cap-point weighted-quantile summary.
+// their weights (summed in double, in an order fixed by the input), exact when a feature has <= cap distinct values, else
+// a cap-point weighted-quantile summary.  A column that holds +inf and missing values keeps +inf as a value.
 struct FeatureSummary { std::vector<float> vals; std::vector<double> weights; };
 void compute_summaries_device(const float* dX, int64_t n, int F, const float* dweights, int cap,
                               std::vector<FeatureSummary>* out, cudaStream_t s);
 void cuts_from_summaries(const std::vector<FeatureSummary>& sums, int max_bin, bool has_missing, HostCuts* out);
+// Multi-rank cuts: every rank summarises its shard with at most kRankSummaryCap points per feature (exact while the shard
+// has no more distinct values), and merge_summaries joins the summaries of all ranks, taken in rank order: a stable sort by
+// value, equal values adding their weights.  compute_rank_cuts_device runs that recipe on one GPU over the row ranges
+// [row_bounds[r], row_bounds[r + 1]) of one matrix, as if each range were a rank's shard.
+constexpr int kRankSummaryCap = 2048;
+void merge_summaries(const std::vector<std::vector<FeatureSummary>>& per_rank, int F, std::vector<FeatureSummary>* merged);
+void compute_rank_cuts_device(const float* dX, int F, const float* dweights, const int64_t* row_bounds, int nranges, int max_bin,
+                              bool has_missing, HostCuts* out, cudaStream_t s);
 
 }  // namespace b200
