@@ -4,7 +4,14 @@ update, timed with CUDA events around each launch group (Booster profile mode) o
     python microbench/partition_profile.py --rows 50000000 --cols 100 [--out partition_profile.json]
 The round time is taken over graph-replayed rounds (as bench.py times them); the profiled rounds that follow are issued
 directly so that every launch group can be bracketed.
-Partition byte model per row, as the library reports it for the profiled trees (profile keys part_row_bytes_*):
+Partition byte model, as the library reports it for the profiled trees (profile keys part_*).  Depth-wise trees up to
+max_depth 7 are routed (route_kernel + route_scan_kernel + scatter_kernel); part_rows counts the rows routed (every row at
+every split level), part_rows_written the built children's rows scattered:
+  per row at the root level:    1 [split-feature byte] + 1 [node id written] + 1 [node id read by the scatter]
+  per row at deeper levels:     1 [node id read] + 3
+  per built row (_out):         8 [the float2 gpair by row] + tail [by row] + 4 [row id] + payload + tail  [written]
+Lossguide and deeper trees move every row of a split node through part_kernel; then part_rows counts the rows of split
+nodes read and part_rows_written the rows written:
   read at the root level:   8 [the float2 gpair, also when only g is kept] + tail + 1 [split-feature byte]
   read at deeper levels:    4 [row id] + payload + tail + 1
   written:                  4 + payload + tail

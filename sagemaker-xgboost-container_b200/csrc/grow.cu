@@ -89,7 +89,11 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
   gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(s); err.alloc(1); tree_index_dev.alloc(1);
   if (!leaf_scale.p) { leaf_scale.alloc(1); set_leaf_scale(1.0f); }
   root_h_cache.alloc(slot_stride);
-  for (int i = 0; i < 2; ++i) { ridx[i].alloc(n); gp[i].alloc(n); tl[i].alloc(tail_pos ? n : 0); }
+  const bool routed = routes(lg_iters, max_depth);
+  for (int i = 0; i < 2; ++i) { const size_t m = i == 0 || !routed ? (size_t)n : 0; ridx[i].alloc(m); gp[i].alloc(m); tl[i].alloc(tail_pos ? m : 0); }
+  route_tiles = routed ? (unsigned)((n + kRouteTile - 1) / kRouteTile) : 0u;
+  node_of_row.alloc(routed ? (size_t)n : 0);
+  route_counts.alloc(routed && max_depth >= 2 ? ((size_t)1 << (max_depth - 2)) * route_tiles : 0);     // built children of the deepest routed level
   max_tiles = (unsigned)((n + kPartTile - 1) / kPartTile) + max_level_nodes + 1;
   scratch.alloc(3 * (size_t)max_level_nodes + 8);
   state_block.alloc(carve(gs, 0)); state_block.zero(s);
@@ -208,7 +212,12 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
   // histograms add the constant h_q), else (g,h); plus the 4 tail bytes when the aligned row copy does not hold them.
   const bool g_only = in.root_mode != 0;
   const bool carry_tail = tail_by_position(bm);
-  if (profile) {                                   // partition byte model per row (microbench/partition_profile.py)
+  const bool routed = routes(in.lg_iters, D);
+  if (profile && routed) {                         // route + scatter byte model per row (microbench/partition_profile.py)
+    prof_part_row_bytes[0] = 3;                    // root level: split byte, node id out, node id into the scatter
+    prof_part_row_bytes[1] = 4;                    // deeper levels: node id in as well
+    prof_part_row_bytes[2] = 8 + 4 + (g_only ? 4 : 8) + (carry_tail ? 8 : 0);    // a built row: float2 gpair (+ tail) by row in, id + payload (+ tail) out
+  } else if (profile) {                            // partition byte model per row
     prof_part_row_bytes[0] = 8 + (carry_tail ? 4 : 0) + 1;                        // root level: the float2 gpair, tail, split byte
     prof_part_row_bytes[2] = 4 + (g_only ? 4 : 8) + (carry_tail ? 4 : 0);         // written: id + payload
     prof_part_row_bytes[1] = prof_part_row_bytes[2] + 1;                          // deeper levels: id + payload + split byte
@@ -277,18 +286,29 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     const int next_base = ((L + 1) & 1) * region, next_half = 1 << L;
     launch_apply(apply_args(in, L, next_base, next_half), s);
     if (final_level) break;                  // children of the last level are leaves: no partition, no histograms
-    PartArgs pa = part_args(L, L == 0 ? kRootRows : (L & 1) ^ 1, L & 1);     // the buffer sets alternate
-    pa.build_only = L == D - 2 ? 1 : 0;                    // the next level is the last one: only the built children are read again
-    timed(kProfPartition, [&] { launch_partition(pa, max_tiles, s); });
+    if (routed) {                            // the built children's rows into buffer set 0, by row from the class's gpair
+      RouteArgs ra{}; ra.gs = gs; ra.tree = ta; ra.bins_col = bm.bins_col; ra.n = bm.n; ra.node_of_row = node_of_row.p;
+      ra.tile_counts = route_counts.p; ra.ntiles = route_tiles; ra.has_missing = bm.has_missing; ra.level = L;
+      ra.gpair = gpair.p + (size_t)k * gp_stride; ra.g_only = g_only ? 1 : 0;
+      ra.tail_row = carry_tail ? reinterpret_cast<const unsigned*>(bm.bins_tail) : nullptr;
+      ra.ridx = ridx[0].p; ra.gp = gp[0].p; ra.tl = carry_tail ? tl[0].p : nullptr; ra.rows_counter = profile ? prof_rows.p + 2 : nullptr;
+      timed(kProfPartition, [&] { launch_route(ra, s); });
+    } else {
+      PartArgs pa = part_args(L, L == 0 ? kRootRows : (L & 1) ^ 1, L & 1);     // the buffer sets alternate
+      pa.build_only = L == D - 2 ? 1 : 0;                    // the next level is the last one: only the built children are read again
+      timed(kProfPartition, [&] { launch_partition(pa, max_tiles, s); });
+    }
     // histograms of the next level: build the smaller children, all-reduce, subtract for the siblings
     CUDA_OK(cudaMemsetAsync(hist_pool.p + (size_t)next_base * slot_stride, 0, (size_t)next_half * slot_stride * sizeof(GH64), s));
-    timed(kProfDeepHist, [&] { launch_hist_build(level_hist_args(L & 1), num_sms, s); });
+    timed(kProfDeepHist, [&] { launch_hist_build(level_hist_args(routed ? 0 : L & 1), num_sms, s); });
     allreduce_hist(hist_pool.p + (size_t)next_base * slot_stride, (size_t)next_half * slot_stride * 2);
     launch_subtract(gs, hist_pool.p, slot_stride, next_half, s);
     launch_eval(eval_args(in, L + 1, in.mask ? in.mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
   }
-  // prediction cache += leaf values of this tree: one row-order pass over the column-major bins
-  timed(kProfMargin, [&] { launch_update_margin(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, in.margin, in.K, k, leaf_scale.p, s); });
+  // prediction cache += leaf values of this tree: one row-order pass over the column-major bins, from the node each row was
+  // routed to (at most one split above its leaf) when the levels were routed
+  const uint8_t* start = routed && D >= 2 ? node_of_row.p : nullptr;
+  timed(kProfMargin, [&] { launch_update_margin(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, start, in.margin, in.K, k, leaf_scale.p, s); });
   if (profile) prof_margin_rows += bm.n;
   pack_tree_kernel<<<(cap_nodes + 255) / 256, 256, 0, s>>>(ta, gs.n_nodes, packed.p, cap_nodes); ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());

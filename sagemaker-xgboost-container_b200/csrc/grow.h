@@ -78,9 +78,11 @@ struct TreeBuilder {
   DevBuf<unsigned char> state_block;       // all GrowState arrays
   DevBuf<unsigned char> tree_block;        // tree_block_layout()
   // the partition's two buffer sets: row ids, the gradients (float g alone in the first n floats for constant-hessian objectives)
-  // and the 4 tail bytes of each row, by position
+  // and the 4 tail bytes of each row, by position.  Routed growth (routes()) writes only set 0; set 1 exists only without it.
   DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx[2], scratch;
   DevBuf<float2> gpair, gp[2]; DevBuf<unsigned> tl[2]; DevBuf<int> err, tree_index_dev; DevBuf<unsigned char> ic_path, ic_allowed, ic_sets;
+  // routed growth: the node each row is in (row order) and the route tiles' row counts per built child (tree.h RouteArgs)
+  DevBuf<uint8_t> node_of_row; DevBuf<unsigned> route_counts; unsigned route_tiles = 0;
   DevBuf<DevNode> packed;                  // the finished tree in the predictor's node format
   // the factor of the tree's leaves in the prediction cache (booster=dart: the new trees' weight, else 1).  A buffer of the
   // builder, not a TreeInputs field: a different weight every round must not force a fresh graph capture.
@@ -96,16 +98,20 @@ struct TreeBuilder {
   enum ProfKind { kProfRootHist, kProfDeepHist, kProfPartition, kProfMargin, kProfKinds };
   struct ProfEvent { cudaEvent_t a, b; int kind; long long launches; };
   bool profile = false; std::vector<ProfEvent> prof_events;
-  // [0] rows through root launches, [1] rows through deeper launches, [2] rows of split nodes read by the partition,
-  // [3] rows the partition wrote
+  // [0] rows through root launches, [1] rows through deeper launches, [2] rows of split nodes read by the partition (routed:
+  // rows routed), [3] rows the partition wrote (routed: built rows scattered)
   DevBuf<unsigned long long> prof_rows;
   long long prof_margin_rows = 0;
   // partition byte model per row of the last profiled tree: [0] read at the root level (no row id), [1] read at deeper levels,
-  // [2] written (row id + gradient payload + tail bytes when they travel with the ids)
+  // [2] written (row id + gradient payload + tail bytes when they travel with the ids; routed: plus what a built row reads by row)
   int prof_part_row_bytes[3] = {0, 0, 0};
 
   ~TreeBuilder() { for (auto e : free_events) cudaEventDestroy(e); for (auto& e : prof_events) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); } }
   void ensure(const BinnedMatrix& bm, int max_depth, int K, int lg_iters, int n_ic);
+  // Depth-wise trees up to kRouteMaxDepth keep a node id per row and write only the built children's rows per level (node ids
+  // fit a byte); loss-guided growth expands one node at a time and deeper trees have too many built children per level, so
+  // both move the rows of every split node through part_kernel.
+  static bool routes(int lg_iters, int max_depth) { return lg_iters == 0 && max_depth <= kRouteMaxDepth; }
   // uploads outside the launch sequence: the tree's column sets and its index (colsample_bynode draws from it), the constraints
   const unsigned char* upload_mask(const std::string& mask, int tree_index);
   const int* upload_monotone(const std::vector<int>& mono, int F);    // nullptr when there are none

@@ -2,6 +2,7 @@
 // depth-wise hist tree builder (SURVEY.md section 8a rows A9, A10, A11).  Mirrors the behaviour of upstream
 // xgboost's src/tree/hist/evaluate_splits.h, src/tree/driver.h, src/tree/updater_quantile_hist.cc and
 // src/common/partition_builder.h as restated in oracle/gbt_oracle.c; all control flow stays on the device.
+#include <algorithm>
 #include <type_traits>
 #include "engine.h"
 #include "rng.h"
@@ -289,7 +290,7 @@ __device__ __forceinline__ void finish_root(const ApplyArgs& a, double ish) {
 }
 
 // Split nid by `best` into the new leaves Lc, Rc: tree arrays, the children's weight bounds and allowed features, their sums.
-// Their row segments are set by part_kernel.
+// Their row segments are set by part_kernel (built children: route_scan_kernel and scatter_kernel).
 __device__ __forceinline__ void expand_node(const ApplyArgs& a, int nid, const SplitCand& best, const GH64& tot, int Lc, int Rc, double isg, double ish) {
   const GrowState& gs = a.gs; const TreeArrays& t = a.tree;
   const long long GLq = best.GL, HLq = best.HL, GRq = tot.g - best.GL, HRq = tot.h - best.HL;
@@ -643,27 +644,234 @@ __global__ void __launch_bounds__(256, GONLY ? (TL ? 5 : 6) : 4) part_kernel(Par
 struct PackedNode { unsigned feat; unsigned short bin_dl; unsigned short left; };   // bin_dl: (split_bin + 1) | dl << 15; left == 0xffff: leaf
 constexpr int kPackedNodesSmem = 2048;
 static_assert(sizeof(PackedNode) == 8, "PackedNode is 8 B");
+__device__ __forceinline__ PackedNode pack_node(const TreeArrays& t, int i) {
+  PackedNode p; p.feat = (unsigned)t.split_index[i]; p.bin_dl = (unsigned short)((t.split_bin[i] + 1) | (t.default_left[i] ? 0x8000 : 0));
+  const int l = t.left[i]; p.left = l < 0 ? 0xffff : (unsigned short)l;
+  return p;
+}
+// part_kernel's rule on a packed node: missing goes to the default side, else byte <= split_bin goes left
+__device__ __forceinline__ bool goes_left(const PackedNode& p, int byte, int has_missing) {
+  return (has_missing && byte == kMissingBin) ? ((p.bin_dl & 0x8000) != 0) : (byte < (int)(p.bin_dl & 0x7fff));
+}
+
+// ---------------------------------------------------------------------------------------------
+// row routing (depth-wise growth up to kRouteMaxDepth; tree.h RouteArgs).  The rows stay in row order with one node-id byte
+// each; per level route_kernel moves every row of a split node to its child and counts each tile's rows per built child,
+// route_scan_kernel turns the counts into offsets (one CTA per built child, tiles in order: the same segments on every run),
+// and scatter_kernel writes only the built children's rows, ascending, with their gradients and tail bytes read by row.
+// A row of a node that stopped splitting keeps that node's id; update_margin_kernel starts its walk there.
+// ---------------------------------------------------------------------------------------------
+// the tree's nodes (n_nodes < kRouteMaxNodes) packed, when s_node is given, and the build list as node id -> index (0xff: not built)
+__device__ __forceinline__ void stage_route_tables(const RouteArgs& a, PackedNode* s_node, unsigned char* s_bidx, int nb) {
+  const int nn = *a.gs.n_nodes;
+  for (int i = threadIdx.x; i < kRouteMaxNodes; i += blockDim.x) {
+    if (s_node) { PackedNode p{0u, 0, 0xffff}; if (i < nn) p = pack_node(a.tree, i); s_node[i] = p; }
+    s_bidx[i] = 0xff;
+  }
+  __syncthreads();
+  for (int r = threadIdx.x; r < nb; r += blockDim.x) s_bidx[a.gs.build_nid[r]] = (unsigned char)r;
+  __syncthreads();
+}
+
+// One CTA per kRouteTile rows; a thread holds kRuns runs of 4 consecutive rows (1024 apart), each loaded and stored as one word.
+constexpr int kRuns = kRouteTile / 1024;
+__global__ void __launch_bounds__(256) route_kernel(RouteArgs a) {
+  __shared__ PackedNode s_node[kRouteMaxNodes];
+  __shared__ unsigned char s_bidx[kRouteMaxNodes];
+  __shared__ unsigned s_cnt[kRouteMaxBuild];
+  const int nb = *a.gs.build_count;
+  if (a.level > 0 && nb == 0) return;                   // no node of this level split: every row keeps its node
+  const int64_t r0 = (int64_t)blockIdx.x * kRouteTile + threadIdx.x * 4;
+  const int lane = threadIdx.x & 31;
+  unsigned ids[kRuns], out[kRuns];
+#pragma unroll
+  for (int j = 0; j < kRuns; ++j) {                     // level 0: every row is at the root
+    const int64_t r = r0 + j * 1024;
+    ids[j] = 0u; out[j] = 0u;
+    if (a.level > 0) {
+      if (r + 4 <= a.n) ids[j] = *reinterpret_cast<const unsigned*>(a.node_of_row + r);
+      else for (int e = 0; e < 4; ++e) if (r + e < a.n) ids[j] |= (unsigned)a.node_of_row[r + e] << (8 * e);
+    }
+  }
+  if (threadIdx.x < kRouteMaxBuild) s_cnt[threadIdx.x] = 0;
+  stage_route_tables(a, s_node, s_bidx, nb);
+  int byte[4 * kRuns];
+#pragma unroll
+  for (int q = 0; q < 4 * kRuns; ++q) {                // every split byte in flight before the first is used
+    const int64_t r = r0 + (q >> 2) * 1024 + (q & 3);
+    const PackedNode p = s_node[(ids[q >> 2] >> (8 * (q & 3))) & 0xffu];
+    byte[q] = (r < a.n && p.left != 0xffff) ? a.bins_col[(int64_t)p.feat * a.n + r] : 0;
+  }
+#pragma unroll
+  for (int q = 0; q < 4 * kRuns; ++q) {
+    const int64_t r = r0 + (q >> 2) * 1024 + (q & 3);
+    const unsigned id = (ids[q >> 2] >> (8 * (q & 3))) & 0xffu;
+    const PackedNode p = s_node[id];
+    const unsigned child = p.left == 0xffff ? id : (goes_left(p, byte[q], a.has_missing) ? p.left : p.left + 1u);
+    out[q >> 2] |= child << (8 * (q & 3));
+    const unsigned c = r < a.n ? s_bidx[child] : 0xffu;
+    const unsigned m = __match_any_sync(0xffffffffu, c);
+    if (c != 0xffu && lane == __ffs(m) - 1) atomicAdd(&s_cnt[c], (unsigned)__popc(m));
+  }
+#pragma unroll
+  for (int j = 0; j < kRuns; ++j) {
+    const int64_t r = r0 + j * 1024;
+    if (a.level > 0 && out[j] == ids[j]) continue;
+    if (r + 4 <= a.n) *reinterpret_cast<unsigned*>(a.node_of_row + r) = out[j];
+    else for (int e = 0; e < 4; ++e) if (r + e < a.n) a.node_of_row[r + e] = (uint8_t)(out[j] >> (8 * e));
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < nb; c += blockDim.x) a.tile_counts[(size_t)c * a.ntiles + blockIdx.x] = s_cnt[c];
+  if (a.rows_counter && threadIdx.x == 0) {
+    const int64_t t0 = (int64_t)blockIdx.x * kRouteTile;
+    atomicAdd(a.rows_counter, (unsigned long long)(a.n - t0 < (int64_t)kRouteTile ? a.n - t0 : (int64_t)kRouteTile));
+  }
+}
+
+// one CTA per built child: exclusive prefix of its tile counts (in place) and the child's row count.  A thread sums a run of
+// consecutive tiles, one block-wide scan orders the runs.
+__global__ void __launch_bounds__(1024) route_scan_kernel(RouteArgs a) {
+  __shared__ unsigned s_run[1024], s_tmp[33];
+  const int c = blockIdx.x;
+  if (c >= *a.gs.build_count) return;
+  unsigned* cnt = a.tile_counts + (size_t)c * a.ntiles;
+  const unsigned per = (a.ntiles + blockDim.x - 1) / blockDim.x, t0 = threadIdx.x * per, t1 = min(t0 + per, a.ntiles);
+  unsigned sum = 0;
+#pragma unroll 8
+  for (unsigned t = t0; t < t1; ++t) sum += cnt[t];
+  s_run[threadIdx.x] = sum;
+  __syncthreads();
+  const unsigned tot = block_exclusive_scan(s_run, s_run, (int)blockDim.x, s_tmp);
+  unsigned run = s_run[threadIdx.x];
+#pragma unroll 8
+  for (unsigned t = t0; t < t1; ++t) { const unsigned v = cnt[t]; cnt[t] = run; run += v; }
+  if (threadIdx.x == 0) a.gs.seg_count[a.gs.build_nid[c]] = tot;
+}
+
+// Persistent CTAs, tiles of kRouteTile rows; warp w owns rows [kWarpRows w, kWarpRows (w + 1)) of a tile in steps of 32.  The
+// built children are laid out back to back in build-list order; a row's position is its child's start + the tile's offset in
+// the child + its rank among the tile's rows of the child (earlier warps first, then row order inside the warp).  The tile's
+// built rows are staged in shared memory grouped by child, so that every child's run leaves in coalesced stores.  CTA 0
+// publishes the segments.
+constexpr int kWarpRows = kRouteTile / 8, kWarpSteps = kWarpRows / 32;
+template <bool GONLY, bool TL>
+__global__ void __launch_bounds__(256, 4) scatter_kernel(RouteArgs a) {
+  typedef typename std::conditional<GONLY, float, float2>::type Pay;
+  __shared__ unsigned char s_bidx[kRouteMaxNodes];
+  __shared__ unsigned s_start[kRouteMaxBuild];          // each built child's first position
+  __shared__ unsigned s_local[kRouteMaxBuild + 1];      // the tile's rows of the earlier children (+ the tile's built rows)
+  __shared__ unsigned s_dst[kRouteMaxBuild];            // position of the child's tile-local index 0
+  __shared__ unsigned s_wofs[8][kRouteMaxBuild];
+  __shared__ unsigned s_rid[kRouteTile];
+  __shared__ Pay s_gp[kRouteTile];
+  __shared__ unsigned s_tl[TL ? kRouteTile : 1];
+  __shared__ unsigned char s_ch[kRouteTile];
+  const GrowState& gs = a.gs;
+  const int nb = *gs.build_count;
+  if (nb == 0) { if (blockIdx.x == 0 && threadIdx.x == 0) gs.build_prefix[0] = 0; return; }
+  stage_route_tables(a, nullptr, s_bidx, nb);
+  if (threadIdx.x < nb) s_start[threadIdx.x] = gs.seg_count[gs.build_nid[threadIdx.x]];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    unsigned run = 0;
+    for (int c = 0; c < nb; ++c) {
+      const unsigned t = s_start[c]; s_start[c] = run;
+      if (blockIdx.x == 0) { gs.build_prefix[c] = run; gs.seg_begin[gs.build_nid[c]] = run; }
+      run += t;
+    }
+    if (blockIdx.x == 0) gs.build_prefix[nb] = run;
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned lanes_below = (1u << lane) - 1u;
+  for (unsigned tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+    const int64_t rw = (int64_t)tile * kRouteTile + warp * kWarpRows + lane;
+    unsigned ck[kWarpSteps];                            // the row's node id, then child << 16 | rank among the warp's rows of that child
+#pragma unroll
+    for (int it = 0; it < kWarpSteps; ++it) { const int64_t r = rw + it * 32; ck[it] = r < a.n ? a.node_of_row[r] : kRouteMaxNodes - 1; }
+    const unsigned toff = threadIdx.x < nb ? a.tile_counts[(size_t)threadIdx.x * a.ntiles + tile] : 0u;
+    __syncthreads();                                    // the previous tile is done with the shared arrays (and s_start is set)
+    for (int i = threadIdx.x; i < 8 * kRouteMaxBuild; i += blockDim.x) s_wofs[i / kRouteMaxBuild][i % kRouteMaxBuild] = 0;
+    __syncthreads();
+#pragma unroll
+    for (int it = 0; it < kWarpSteps; ++it) {
+      const unsigned c = s_bidx[ck[it]];
+      const unsigned m = __match_any_sync(0xffffffffu, c);
+      const unsigned before = c != 0xffu ? s_wofs[warp][c] : 0u;
+      __syncwarp();
+      if (c != 0xffu && lane == __ffs(m) - 1) s_wofs[warp][c] = before + __popc(m);
+      __syncwarp();
+      ck[it] = c << 16 | (before + __popc(m & lanes_below));
+    }
+    __syncthreads();
+    if (threadIdx.x < nb) {                             // the tile's rows of each child
+      unsigned t = 0;
+      for (int w = 0; w < 8; ++w) t += s_wofs[w][threadIdx.x];
+      s_local[threadIdx.x + 1] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) { s_local[0] = 0; for (int c = 0; c < nb; ++c) s_local[c + 1] += s_local[c]; }
+    __syncthreads();
+    if (threadIdx.x < nb) {                             // tile-local start of each (warp, child)
+      const unsigned c = threadIdx.x;
+      unsigned run = s_local[c];
+      s_dst[c] = s_start[c] + toff - run;
+      for (int w = 0; w < 8; ++w) { const unsigned t = s_wofs[w][c]; s_wofs[w][c] = run; run += t; }
+    }
+    __syncthreads();
+    // built rows only: gradient (+ tail) by row into the staging arrays.  Eight rows' loads are issued before their stores: the
+    // compiler may not move a load across a store it cannot prove disjoint, and one round trip per row serialises the tile.
+#pragma unroll
+    for (int h = 0; h < kWarpSteps; h += 8) {
+      Pay pv[8]; unsigned tv[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const unsigned r = (unsigned)(rw + (h + j) * 32);
+        pv[j] = Pay{}; tv[j] = 0u;
+        if ((ck[h + j] >> 16) != 0xffu) {
+          if constexpr (GONLY) pv[j] = __ldg(reinterpret_cast<const float*>(a.gpair) + (size_t)r * 2); else pv[j] = __ldg(a.gpair + r);
+          if constexpr (TL) tv[j] = __ldg(a.tail_row + r);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const unsigned c = ck[h + j] >> 16;
+        if (c == 0xffu) continue;
+        const unsigned k = s_wofs[warp][c] + (ck[h + j] & 0xffffu);
+        s_rid[k] = (unsigned)(rw + (h + j) * 32); s_gp[k] = pv[j]; s_ch[k] = (unsigned char)c;
+        if constexpr (TL) s_tl[k] = tv[j];
+      }
+    }
+    __syncthreads();
+    const unsigned built = s_local[nb];
+    for (unsigned k = threadIdx.x; k < built; k += blockDim.x) {
+      const unsigned pos = s_dst[s_ch[k]] + k;
+      a.ridx[pos] = s_rid[k]; static_cast<Pay*>(a.gp)[pos] = s_gp[k];
+      if constexpr (TL) a.tl[pos] = s_tl[k];
+    }
+    if (a.rows_counter && threadIdx.x == 0) atomicAdd(a.rows_counter + 1, (unsigned long long)built);
+  }
+}
 
 __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing,
-                                                            float* margin, int K, int k, const float* leaf_scale) {
+                                                            const uint8_t* node_of_row, float* margin, int K, int k, const float* leaf_scale) {
   __shared__ PackedNode s_nodes[kPackedNodesSmem];
   __shared__ float s_leaf[kPackedNodesSmem];
   const int nn = *n_nodes;
   const bool packed = nn <= kPackedNodesSmem && nn < 0xffff;
   if (packed) {
-    for (int i = threadIdx.x; i < nn; i += blockDim.x) {
-      PackedNode p; p.feat = (unsigned)t.split_index[i]; p.bin_dl = (unsigned short)((t.split_bin[i] + 1) | (t.default_left[i] ? 0x8000 : 0));
-      const int l = t.left[i]; p.left = l < 0 ? 0xffff : (unsigned short)l;
-      s_nodes[i] = p; s_leaf[i] = t.split_cond[i];
-    }
+    for (int i = threadIdx.x; i < nn; i += blockDim.x) { s_nodes[i] = pack_node(t, i); s_leaf[i] = t.split_cond[i]; }
     __syncthreads();
   }
-  // four independent traversals per thread (rows r, r+256, r+512, r+768 of the block's 1024-row tile): 4 loads in flight
+  // four independent traversals per thread (rows r, r+256, r+512, r+768 of the block's 1024-row tile): 4 loads in flight.
+  // Each starts at the root, or at the node the row was routed to.
   const int64_t base = (int64_t)blockIdx.x * 1024 + threadIdx.x;
   int nid[4]; bool done[4];
-  const bool root_leaf = packed ? (s_nodes[0].left == 0xffff) : (t.left[0] == -1);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) { nid[j] = 0; done[j] = (base + j * 256 >= n) || root_leaf; }
+  for (int j = 0; j < 4; ++j) {
+    const int64_t r = base + j * 256;
+    nid[j] = (node_of_row != nullptr && r < n) ? (int)node_of_row[r] : 0;
+    done[j] = r >= n || (packed ? (s_nodes[nid[j]].left == 0xffff) : (t.left[nid[j]] == -1));
+  }
   bool any = !(done[0] && done[1] && done[2] && done[3]);
   while (any) {
     int byte[4];
@@ -679,8 +887,7 @@ __global__ void __launch_bounds__(256) update_margin_kernel(TreeArrays t, const 
       const int nd = nid[j];
       if (packed) {
         const PackedNode p = s_nodes[nd];
-        const bool left = (has_missing && byte[j] == kMissingBin) ? ((p.bin_dl & 0x8000) != 0) : (byte[j] < (int)(p.bin_dl & 0x7fff));
-        nid[j] = left ? p.left : p.left + 1;
+        nid[j] = goes_left(p, byte[j], has_missing) ? p.left : p.left + 1;
         done[j] = s_nodes[nid[j]].left == 0xffff;
       } else {
         const bool left = (has_missing && byte[j] == kMissingBin) ? (t.default_left[nd] != 0) : (byte[j] <= t.split_bin[nd]);
@@ -740,10 +947,21 @@ void launch_partition(const PartArgs& a, unsigned max_tiles, cudaStream_t s) {
   else { if (tl) part_kernel<false, true><<<max_tiles, 256, 0, s>>>(a); else part_kernel<false, false><<<max_tiles, 256, 0, s>>>(a); }
   ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
-void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k,
-                          const float* leaf_scale, cudaStream_t s) {
+void launch_route(const RouteArgs& a, cudaStream_t s) {
+  if (a.ntiles == 0) return;
+  route_kernel<<<a.ntiles, 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  route_scan_kernel<<<1u << a.level, 1024, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());    // built children of the level, worst case
+  const bool tl = a.tail_row != nullptr;
+  const unsigned grid = std::min(a.ntiles, 4u * (unsigned)engine_num_sms());       // persistent: 4 CTAs per SM
+  if (a.g_only) { if (tl) scatter_kernel<true, true><<<grid, 256, 0, s>>>(a); else scatter_kernel<true, false><<<grid, 256, 0, s>>>(a); }
+  else { if (tl) scatter_kernel<false, true><<<grid, 256, 0, s>>>(a); else scatter_kernel<false, false><<<grid, 256, 0, s>>>(a); }
+  ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, const uint8_t* node_of_row,
+                          float* margin, int K, int k, const float* leaf_scale, cudaStream_t s) {
   if (n == 0) return;
-  update_margin_kernel<<<(unsigned)((n + 1023) / 1024), 256, 0, s>>>(t, n_nodes, bins_col, n, has_missing, margin, K, k, leaf_scale); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  update_margin_kernel<<<(unsigned)((n + 1023) / 1024), 256, 0, s>>>(t, n_nodes, bins_col, n, has_missing, node_of_row, margin, K, k, leaf_scale);
+  ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_subtract(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s) {
   dim3 grid(max_build, (unsigned)((slot_entries + 1023) / 1024)); subtract_kernel<<<grid, 256, 0, s>>>(gs, pool, slot_entries); ++g_kernel_launches; CUDA_OK(cudaGetLastError());

@@ -40,6 +40,25 @@ struct PartArgs {
   unsigned long long* rows_counter;           // optional (profiling): [0] += rows of split nodes read, [1] += rows written
 };
 
+// Depth-wise growth up to kRouteMaxDepth keeps one byte per row, in row order: the id of the row's current node (< 255).  Each
+// level routes every row from its split byte (route_kernel), scans the tiles' row counts per built child in a fixed order
+// (route_scan_kernel) and writes only the built children's rows into their segments (scatter_kernel).
+constexpr int kRouteMaxDepth = 7;
+constexpr unsigned kRouteTile = 2048;      // rows per route / scatter tile (256 threads x 8 rows)
+constexpr int kRouteMaxNodes = 256;        // node ids of a tree of depth kRouteMaxDepth: 0 .. 254
+constexpr int kRouteMaxBuild = 1 << (kRouteMaxDepth - 2);      // built children of the deepest routed level
+struct RouteArgs {
+  GrowState gs; TreeArrays tree; const uint8_t* bins_col; int64_t n;
+  uint8_t* node_of_row;                       // [n] the tree node each row is in
+  unsigned* tile_counts;                      // [kRouteMaxBuild][ntiles]: a tile's rows per built child, then their offset in it
+  unsigned ntiles; int has_missing, level;
+  // what scatter_kernel writes for a built row, read by ROW: g of the class's float2 gpair (g_only) or the pair, and the 4 tail
+  // bytes of a 4-wide tail (tail_row: bins_tail as words; nullptr when the tail does not travel with the ids)
+  const float2* gpair; int g_only; const unsigned* tail_row;
+  unsigned* ridx; void* gp; unsigned* tl;     // the built children's rows by position
+  unsigned long long* rows_counter;           // optional (profiling): [0] += rows routed, [1] += rows scattered
+};
+
 struct HistArgs {
   const uint8_t* bins;          // main: row-major [n][ngroups*32 B]
   const uint8_t* bins_tail;     // tail: row-major [n][tw B], nullptr when tw == 0
@@ -84,9 +103,11 @@ void launch_scales(const GrowState& gs, int grad_bits, cudaStream_t s);
 void launch_eval(const EvalArgs& a, int max_nodes_level, cudaStream_t s);
 void launch_apply(const ApplyArgs& a, cudaStream_t s);
 void launch_partition(const PartArgs& a, unsigned max_tiles, cudaStream_t s);
-// margin[:, k] += fl(*leaf_scale * leaf) of the finished tree (leaf_scale: one float on the device, 1 except under booster=dart)
-void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, float* margin, int K, int k,
-                          const float* leaf_scale, cudaStream_t s);
+void launch_route(const RouteArgs& a, cudaStream_t s);     // route + scan + scatter of one level
+// margin[:, k] += fl(*leaf_scale * leaf) of the finished tree (leaf_scale: one float on the device, 1 except under booster=dart).
+// node_of_row: the node each row was routed to (the walk starts there), nullptr = walk from the root
+void launch_update_margin(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing, const uint8_t* node_of_row,
+                          float* margin, int K, int k, const float* leaf_scale, cudaStream_t s);
 void launch_subtract(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s);
 
 }  // namespace b200
