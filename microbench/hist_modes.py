@@ -2,7 +2,8 @@
 """Kernel-level timing of the histogram kernels through the C-ABI debug entry point (XGB200BuildHistogramEx):
 root pass with the TMA kernel (G+H and G-only) and with the gather kernel, and gathered row subsets (deeper levels).
     python microbench/hist_modes.py --rows 50000000 --cols 100 [--out hist_modes.json]
-Algorithmic bytes: rows * (F + 8) for contiguous passes, rows * (F + 8 + 4) with row ids."""
+Algorithmic bytes: rows * (F + 8) for contiguous (g,h) passes, rows * (F + 4) for the G-only root pass (mode 2: it reads the
+dense g of constant-hessian training, 4 B per row), rows * (F + 8 + 4) with row ids."""
 import argparse
 import json
 import os
@@ -45,7 +46,7 @@ def main():
         gp = gpair if rows is None else gpair[:m]
         be.build_histogram_ex(b.handle, d.handle, gp, mode=mode, row_ids=rows, repeats=2)          # warm-up
         hist, scales, ms, kernel = be.build_histogram_ex(b.handle, d.handle, gp, mode=mode, row_ids=rows, repeats=a.repeats)
-        bytes_ = m * (F + 8 + (0 if rows is None else 4))
+        bytes_ = m * (F + (4 if mode == 2 else 8) + (0 if rows is None else 4))
         r = {"case": label, "kernel": kernel, "rows": m, "ms": ms, "gbs": bytes_ / ms / 1e6, "frac_of_peak": bytes_ / ms / 1e6 / peak,
              "checksum": int(hist[:, :, 0].sum()), "checksum_h": int(hist[:, :, 1].sum())}
         res.append(r)

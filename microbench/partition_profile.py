@@ -9,13 +9,13 @@ max_depth 7 are routed (route_kernel + route_scan_kernel + scatter_kernel); part
 every split level), part_rows_written the built children's rows scattered:
   per row at the root level:    1 [split-feature byte] + 1 [node id written] + 1 [node id read by the scatter]
   per row at deeper levels:     1 [node id read] + 3
-  per built row (_out):         8 [the float2 gpair by row] + tail [by row] + 4 [row id] + payload + tail  [written]
+  per built row (_out):         payload [the round's gradient by row] + tail [by row] + 4 [row id] + payload + tail  [written]
 Lossguide and deeper trees move every row of a split node through part_kernel; then part_rows counts the rows of split
 nodes read and part_rows_written the rows written:
-  read at the root level:   8 [the float2 gpair, also when only g is kept] + tail + 1 [split-feature byte]
+  read at the root level:   payload [the round's gradient by row] + tail + 1 [split-feature byte]
   read at deeper levels:    4 [row id] + payload + tail + 1
   written:                  4 + payload + tail
-payload = 4 (g alone, constant-hessian objectives) or 8 ((g,h)); tail = 4 when the rows' 4 tail bin bytes travel with their
+payload = 4 (g alone, constant-hessian objectives, whose round gradients are a dense float g) or 8 ((g,h)); tail = 4 when the rows' 4 tail bin bytes travel with their
 ids (a 4-wide tail that the line-aligned row copy does not hold), else 0."""
 import argparse
 import json

@@ -692,11 +692,14 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   // booster=dart: the gradients see the margin without the dropped trees; the cache already holds their new weights
   const float* grad_margin = dart_.on ? dart_begin_round(dtrain, cache, round) : cache.margin.p;
   // ---- gradients + fixed-point scales
+  const bool dense_g = constant_hessian(*dtrain);
+  // constant-hessian growth needs subsample >= 1, so a per-tree row sample (which copies (g,h) pairs) never sees dense g
+  B200_CHECK(!(dense_g && per_tree_sample), "per-tree row sampling of a constant-hessian round");
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
   if (per_tree_sample) {
     forest_gpair_.ensure((size_t)b.gp_stride * K);
-    launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f);
-  } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample);
+    launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f, false);
+  } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g);
   if (!per_tree_sample) {
     Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
     launch_scales(b.gs, grad_bits_for(b.global_n), s);
@@ -720,12 +723,14 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
 }
 
 // The objective's gradient pairs at `margin` into gpair ([K][gp_stride]), rows outside round `round`'s sample zeroed, max|g| and
-// max h folded into absmax (nullptr: not taken).  The survival objectives have their own kernels (survival.cu); every other
-// objective runs gradient_kernel.
-void Booster::launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample) {
+// max h folded into absmax (nullptr: not taken).  dense_g (constant_hessian only): g alone, as float[gp_stride].  The survival
+// objectives have their own kernels (survival.cu); every other objective runs gradient_kernel.
+void Booster::launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample,
+                               bool dense_g) {
   cudaStream_t s = engine_stream();
   const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
   if (objective_is_survival(param_.objective)) {
+    B200_CHECK(!dense_g, "the survival objectives write (g,h) pairs");
     SurvivalGradArgs sa{}; sa.margin = margin; sa.label = dm->d_labels.p; sa.lower = dm->d_label_lower.p; sa.upper = dm->d_label_upper.p;
     sa.weight = dm->weights.empty() ? nullptr : dm->d_weights.p; sa.gpair = gpair; sa.absmax = absmax; sa.n = dm->n; sa.row_offset = row_offset;
     sa.subsample = subsample; sa.seed = param_.seed; sa.iter = (unsigned long long)round; sa.dist = param_.aft_dist; sa.sigma = param_.aft_sigma;
@@ -737,7 +742,7 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
   GradArgs ga{}; ga.margin = margin; ga.label = dm->d_labels.p; ga.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
   ga.gpair = gpair; ga.gp_stride = gp_stride; ga.absmax = absmax; ga.err = builder_->err.p; ga.n = dm->n; ga.row_offset = row_offset; ga.K = param_.num_class;
   ga.objective = param_.objective; ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = subsample; ga.seed = param_.seed;
-  ga.iter = (unsigned long long)round; ga.aux = objective_aux(param_);
+  ga.iter = (unsigned long long)round; ga.aux = objective_aux(param_); ga.dense_g = dense_g ? 1 : 0;
   launch_gradient(ga, s);
 }
 
@@ -750,7 +755,7 @@ void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float*
   const int64_t n = dm->n;
   DevBuf<float> d_margin; DevBuf<float2> d_gp; d_margin.alloc((size_t)n * K); d_gp.alloc((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(d_margin.p, margin, sizeof(float) * n * K, cudaMemcpyHostToDevice, s));
-  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample);
+  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample, false);      // always the (g,h) pairs
   std::vector<float2> h((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(h.data(), d_gp.p, sizeof(float2) * h.size(), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
@@ -776,6 +781,14 @@ TreeBuilder& Booster::builder_for(DMatrix* dm) {
   return *builder_;
 }
 
+// Constant-hessian growth: every row has h == 1 in every round.  The round's gradients are then written as a dense float g
+// (launch_objective) and the tree reads them so (root_mode != 0); this one predicate decides both.  B200XGB_NO_CONSTH turns it off.
+bool Booster::constant_hessian(const DMatrix& dm) const {
+  static const bool no_consth = getenv("B200XGB_NO_CONSTH") != nullptr;
+  return !no_consth && param_.objective == kSquaredError && param_.num_class == 1 && dm.weights.empty() &&
+         param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
+}
+
 // The only place TreeInputs are filled.  mask: the tree's column sets (empty = no column sampling), uploaded with its index;
 // the constraints are uploaded here too.
 TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int tree_index, float* margin, int k) {
@@ -787,11 +800,7 @@ TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int 
   in.mask = mask.empty() ? nullptr : b.upload_mask(mask, tree_index);
   in.monotone = b.upload_monotone(monotone_, dm.F);
   b.upload_interaction(interaction_, dm.F); in.n_ic = (int)interaction_.size();
-  // constant-hessian root pass: eligible when every row has h == 1 in every round
-  static const bool no_consth = getenv("B200XGB_NO_CONSTH") != nullptr;
-  const bool consth = !no_consth && param_.objective == kSquaredError && param_.num_class == 1 && dm.weights.empty() &&
-                      param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
-  in.root_mode = !consth ? 0 : b.root_h_valid && b.root_h_uid == dm.uid && b.root_h_version == dm.binned_version ? 2 : 1;
+  in.root_mode = !constant_hessian(dm) ? 0 : b.root_h_valid && b.root_h_uid == dm.uid && b.root_h_version == dm.binned_version ? 2 : 1;
   in.world = Comm::get().world();
   return in;
 }

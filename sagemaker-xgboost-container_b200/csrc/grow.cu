@@ -197,7 +197,7 @@ template <class Launch> void TreeBuilder::timed(ProfKind kind, Launch launch) {
   prof_events.push_back(e);
 }
 
-constexpr int kRootRows = -1;     // the partition's input at the root: every row in order, the float2 gpair and the tail words by row
+constexpr int kRootRows = -1;     // the partition's input at the root: every row in order, the gradients and the tail words by row
 // The fixed launch sequence of one tree (everything data dependent lives in device memory), capturable in a CUDA graph.
 void TreeBuilder::enqueue(const TreeInputs& in) {
   cudaStream_t s = engine_stream();
@@ -209,20 +209,25 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
   if (in.root_mode == 2) { slot_from_cache_kernel<<<num_sms, 256, 0, s>>>(hist_pool.p, root_h_cache.p, slot_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
   else CUDA_OK(cudaMemsetAsync(hist_pool.p, 0, slot_stride * sizeof(GH64), s));
   // What travels with the row ids through the partition: g alone when the hessian is constant (h == 1 for every row, the
-  // histograms add the constant h_q), else (g,h); plus the 4 tail bytes when the aligned row copy does not hold them.
+  // histograms add the constant h_q), else (g,h); plus the 4 tail bytes when the aligned row copy does not hold them.  The
+  // round's gradients are then the dense g of gpair (g_dense) too, so every pass of the tree reads 4 B of gradient per row.
   const bool g_only = in.root_mode != 0;
+  const int pay = g_only ? 4 : 8;
   const bool carry_tail = tail_by_position(bm);
   const bool routed = routes(in.lg_iters, D);
   if (profile && routed) {                         // route + scatter byte model per row (microbench/partition_profile.py)
     prof_part_row_bytes[0] = 3;                    // root level: split byte, node id out, node id into the scatter
     prof_part_row_bytes[1] = 4;                    // deeper levels: node id in as well
-    prof_part_row_bytes[2] = 8 + 4 + (g_only ? 4 : 8) + (carry_tail ? 8 : 0);    // a built row: float2 gpair (+ tail) by row in, id + payload (+ tail) out
+    prof_part_row_bytes[2] = pay + 4 + pay + (carry_tail ? 8 : 0);                // a built row: gradient (+ tail) by row in, id + payload (+ tail) out
   } else if (profile) {                            // partition byte model per row
-    prof_part_row_bytes[0] = 8 + (carry_tail ? 4 : 0) + 1;                        // root level: the float2 gpair, tail, split byte
-    prof_part_row_bytes[2] = 4 + (g_only ? 4 : 8) + (carry_tail ? 4 : 0);         // written: id + payload
+    prof_part_row_bytes[0] = pay + (carry_tail ? 4 : 0) + 1;                      // root level: the gradient, tail, split byte
+    prof_part_row_bytes[2] = 4 + pay + (carry_tail ? 4 : 0);                      // written: id + payload
     prof_part_row_bytes[1] = prof_part_row_bytes[2] + 1;                          // deeper levels: id + payload + split byte
   }
+  // the root pass: (g,h) pairs by row; with constant hessian the dense g, through hist_gather_kernel's contiguous G-only-payload
+  // mode on the snapshot tree (root_mode 1: it needs the H plane) and through hist_root_kernel<GONLY> after it (root_mode 2)
   HistArgs root = hist_args(bm, k);
+  if (g_only) { root.gpair = nullptr; root.gpos = g_dense(); }
   root.g_only = in.root_mode == 2 ? 1 : 0; root.rows_counter = profile ? prof_rows.p : nullptr;
   timed(kProfRootHist, [&] { launch_hist_build(root, num_sms, s); });
   if (in.root_mode == 1) { snapshot_h_kernel<<<num_sms, 256, 0, s>>>(hist_pool.p, root_h_cache.p, slot_stride); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
@@ -251,8 +256,8 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     const bool root = cur == kRootRows;
     PartArgs pa{}; pa.gs = gs; pa.tree = ta; pa.bins_col = bm.bins_col; pa.n = bm.n;
     pa.ridx_cur = root ? nullptr : ridx[cur].p; pa.ridx_next = ridx[next].p;
-    pa.gp_cur = root ? static_cast<const void*>(gpair.p + (size_t)k * gp_stride) : gp[cur].p; pa.gp_next = gp[next].p;
-    pa.gp_cur_stride = root ? 2 : 1; pa.g_only = g_only ? 1 : 0;
+    const void* root_gp = g_only ? static_cast<const void*>(g_dense()) : static_cast<const void*>(gpair.p + (size_t)k * gp_stride);
+    pa.gp_cur = root ? root_gp : gp[cur].p; pa.gp_next = gp[next].p; pa.g_only = g_only ? 1 : 0;
     pa.tl_cur = !carry_tail ? nullptr : (root ? reinterpret_cast<const unsigned*>(bm.bins_tail) : tl[cur].p); pa.tl_next = carry_tail ? tl[next].p : nullptr;
     pa.has_missing = bm.has_missing; pa.level = level; pa.max_level_nodes = max_level_nodes; pa.rows_counter = profile ? prof_rows.p + 2 : nullptr;
     return pa;
@@ -286,10 +291,11 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     const int next_base = ((L + 1) & 1) * region, next_half = 1 << L;
     launch_apply(apply_args(in, L, next_base, next_half), s);
     if (final_level) break;                  // children of the last level are leaves: no partition, no histograms
-    if (routed) {                            // the built children's rows into buffer set 0, by row from the class's gpair
+    if (routed) {                            // the built children's rows into buffer set 0, by row from the class's gradients
       RouteArgs ra{}; ra.gs = gs; ra.tree = ta; ra.bins_col = bm.bins_col; ra.n = bm.n; ra.node_of_row = node_of_row.p;
       ra.tile_counts = route_counts.p; ra.ntiles = route_tiles; ra.has_missing = bm.has_missing; ra.level = L;
-      ra.gpair = gpair.p + (size_t)k * gp_stride; ra.g_only = g_only ? 1 : 0;
+      if (g_only) ra.g = g_dense(); else ra.gpair = gpair.p + (size_t)k * gp_stride;
+      ra.g_only = g_only ? 1 : 0;
       ra.tail_row = carry_tail ? reinterpret_cast<const unsigned*>(bm.bins_tail) : nullptr;
       ra.ridx = ridx[0].p; ra.gp = gp[0].p; ra.tl = carry_tail ? tl[0].p : nullptr; ra.rows_counter = profile ? prof_rows.p + 2 : nullptr;
       timed(kProfPartition, [&] { launch_route(ra, s); });
@@ -378,10 +384,11 @@ void TreeBuilder::debug_build_root_hist(const BinnedMatrix& bm, const float* gpa
   HistArgs ha = hist_args(bm, 0);                 // the training path's arguments; the row ids and the mode bits override
   ha.ridx = row_ids ? ridx[0].p : nullptr;
   ha.force_gather = (mode & 3) == 1 ? 1 : 0; ha.g_only = (mode & 3) == 2 ? 1 : 0;
-  if (mode & 8) {                               // G-only payload: g alone by position, h == 1.0f for every row (the supplied h is ignored)
+  if ((mode & 8) || ha.g_only) {                // G-only payload: g alone, h == 1.0f for every row (the supplied h is ignored)
     std::vector<float> gh((size_t)rows);
     for (int64_t i = 0; i < rows; ++i) gh[i] = gpair_host[2 * i];
-    float* gpos = reinterpret_cast<float*>(gp[0].p);
+    // by position after a partition; at the root the dense g of constant-hessian training, whose allocation covers whole root tiles
+    float* gpos = row_ids ? reinterpret_cast<float*>(gp[0].p) : g_dense();
     if (rows) CUDA_OK(cudaMemcpyAsync(gpos, gh.data(), sizeof(float) * rows, cudaMemcpyHostToDevice, s));
     Comm::get().sync_stream(s);
     ha.gpos = gpos; ha.gpair = nullptr;

@@ -80,6 +80,8 @@ struct TreeBuilder {
   // the partition's two buffer sets: row ids, the gradients (float g alone in the first n floats for constant-hessian objectives)
   // and the 4 tail bytes of each row, by position.  Routed growth (routes()) writes only set 0; set 1 exists only without it.
   DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx[2], scratch;
+  // gpair: the round's gradients by row, [K][gp_stride] (g,h) pairs, or for constant-hessian growth (TreeInputs root_mode != 0,
+  // K == 1) a dense float g[gp_stride] in the same allocation (g_dense)
   DevBuf<float2> gpair, gp[2]; DevBuf<unsigned> tl[2]; DevBuf<int> err, tree_index_dev; DevBuf<unsigned char> ic_path, ic_allowed, ic_sets;
   // routed growth: the node each row is in (row order) and the route tiles' row counts per built child (tree.h RouteArgs)
   DevBuf<uint8_t> node_of_row; DevBuf<unsigned> route_counts; unsigned route_tiles = 0;
@@ -130,6 +132,7 @@ struct TreeBuilder {
   void enqueue(const TreeInputs& in);
   void end_segment();
   HistArgs hist_args(const BinnedMatrix& bm, int k) const;
+  float* g_dense() const { return reinterpret_cast<float*>(gpair.p); }
   EvalArgs eval_args(const TreeInputs& in, int level, const unsigned char* feat_mask) const;
   ApplyArgs apply_args(const TreeInputs& in, int level, int next_base, int next_half) const;
   template <class Launch> void timed(ProfKind kind, Launch launch);

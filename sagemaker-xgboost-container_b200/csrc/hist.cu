@@ -15,7 +15,7 @@
 //                          UBLKCP) into an mbarrier ring; consumer warps read bins with conflict-free LDS.128 and issue
 //                          the atomics.  GONLY variant for constant-hessian objectives: the H plane of the root never
 //                          changes between rounds, so the slot is pre-loaded with the cached H plane and only G is
-//                          accumulated (1 atomic per update instead of 2).
+//                          accumulated (1 atomic per update instead of 2); its gradients are the dense g (4 B per row).
 //      hist_gather_kernel  the deeper levels: rows gathered by row id (LDG.128 per 16 B chunk straight to registers, a
 //                          rolling one-super-tile-ahead prefetch), (g,h) read by POSITION (they travel with the row
 //                          ids through the partition; g alone for constant-hessian objectives, whose h_q is a constant),
@@ -357,7 +357,8 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
   const unsigned bars = ring + (unsigned)c.S * c.stage_bytes;                 // full[S] then empty[S]
   const unsigned row_bytes = 32u * (unsigned)c.box_groups;
   const unsigned main_tile_bytes = (unsigned)R * row_bytes;
-  const unsigned gp_off = main_tile_bytes, tail_tile_off = main_tile_bytes + (unsigned)R * 8u;
+  constexpr unsigned kGradBytes = GONLY ? 4u : 8u;      // per row: the dense g, or the (g,h) pair
+  const unsigned gp_off = main_tile_bytes, tail_tile_off = main_tile_bytes + (unsigned)R * kGradBytes;
   const unsigned ntiles = (T + R - 1) / R;
   const unsigned my_ntiles = ntiles > blockIdx.x ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0u;   // tiles blockIdx.x + i * gridDim.x
 
@@ -388,7 +389,7 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
     if (lane == 0) {
       const unsigned P = (c.flags & 8) ? 1u : (unsigned)kRootProducerWarps, pw = (unsigned)(warp - NCW);
       if (pw < P) {
-        const unsigned tx = main_tile_bytes + (unsigned)R * 8u + (has_tail ? (unsigned)R * (unsigned)a.tw : 0u);
+        const unsigned tx = main_tile_bytes + (unsigned)R * kGradBytes + (has_tail ? (unsigned)R * (unsigned)a.tw : 0u);
         unsigned s = pw % (unsigned)c.S, round = pw / (unsigned)c.S;
         for (unsigned i = pw; i < my_ntiles; i += P) {
           if (round > 0) mbar_wait(bars + 8u * (c.S + s), (round - 1u) & 1u);
@@ -398,7 +399,8 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
           mbar_expect_tx(full, tx);
           if ((c.flags & 1) && gridDim.y == 1) bulk_load_1d(dst, a.bins + (size_t)row0 * a.row_stride, main_tile_bytes, full);
           else tma_load_2d(dst, &tm, g0 * 32, (int)row0, full);
-          bulk_load_1d(dst + gp_off, a.gpair + row0, (unsigned)R * 8u, full);
+          if (GONLY) bulk_load_1d(dst + gp_off, a.gpos + row0, (unsigned)R * 4u, full);
+          else bulk_load_1d(dst + gp_off, a.gpair + row0, (unsigned)R * 8u, full);
           if (has_tail) bulk_load_1d(dst + tail_tile_off, a.bins_tail + (size_t)row0 * a.tw, (unsigned)R * (unsigned)a.tw, full);
           const unsigned tp = t + 8u * gridDim.x;        // warm L2 eight tiles ahead of this CTA
           if (tp < ntiles && !(c.flags & 4)) tma_prefetch_2d(&tm, g0 * 32, (int)(tp * (unsigned)R));
@@ -422,6 +424,19 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
   tc.rep_off = has_tail ? (unsigned)((lane / a.tw) % c.trep) * (unsigned)a.tw * 4u : 0u;
   const unsigned rowl = (unsigned)(wit << 4) + (unsigned)(lane >> 1);          // this lane's row inside a tile
   const unsigned tiles_per_window = (unsigned)a.window_rows / R;
+  // GONLY: h == 1.0f for every row, so every valid row adds rint(1.0f * sh) to the node's H (hist_gather_kernel's GPAY rule)
+  const unsigned hq_one = (unsigned)__float2int_rn(1.0f * sh);
+  // (g_q, h_q) of tile row `row` from the stage's gradients; rows past T add nothing
+  auto quant = [&](unsigned tile, unsigned row, bool valid, int& gq, unsigned& hq) {
+    gq = 0; hq = 0;
+    if constexpr (GONLY) {
+      const float g = __uint_as_float(lds_u32(tile + gp_off + row * 4u));
+      if (valid) { gq = __float2int_rn(g * sg); hq = hq_one; }
+    } else {
+      const uint2 gh = lds_v2(tile + gp_off + row * 8u);
+      if (valid) { gq = __float2int_rn(__uint_as_float(gh.x) * sg); hq = (unsigned)__float2int_rn(__uint_as_float(gh.y) * sh); }
+    }
+  };
   long long accG = 0, accH = 0;
   unsigned i = (unsigned)team, s = (unsigned)team, ph = 0;                      // c.S >= kTeams (root_plan)
   for (unsigned wstart = 0;; wstart += tiles_per_window) {
@@ -431,9 +446,8 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
       const unsigned tile = ring + s * c.stage_bytes;
       const unsigned row0 = (blockIdx.x + i * gridDim.x) * (unsigned)R;
       if (!(c.flags & 2)) {
-        const uint2 ghb = lds_v2(tile + gp_off + rowl * 8u);
-        int gq = 0; unsigned hq = 0;
-        if (row0 + rowl < T) { gq = __float2int_rn(__uint_as_float(ghb.x) * sg); hq = (unsigned)__float2int_rn(__uint_as_float(ghb.y) * sh); }
+        int gq; unsigned hq;
+        quant(tile, rowl, row0 + rowl < T, gq, hq);
         if ((lane & 1) == 0) { accG += gq; accH += hq; }
         const unsigned rowaddr = tile + rowl * row_bytes;
         root_unit<GONLY, 0>(lc, ldsoff, rowaddr, gq, hq);
@@ -446,10 +460,9 @@ hist_root_kernel(const __grid_constant__ CUtensorMap tm, HistArgs a, RootCfg c) 
             unsigned w0, w1 = 0;
             if (a.tw == 4) w0 = lds_u32(tile + tail_tile_off + trow * 4u);
             else { const uint2 ww = lds_v2(tile + tail_tile_off + trow * 8u); w0 = ww.x; w1 = ww.y; }
-            const uint2 gt = lds_v2(tile + gp_off + trow * 8u);
-            int gqt = 0; unsigned hqt = 0;
-            if (row0 + trow < T) { gqt = __float2int_rn(__uint_as_float(gt.x) * sg); hqt = (unsigned)__float2int_rn(__uint_as_float(gt.y) * sh); }
-            else { w0 = 0; w1 = 0; }
+            int gqt; unsigned hqt;
+            quant(tile, trow, row0 + trow < T, gqt, hqt);
+            if (row0 + trow >= T) { w0 = 0; w1 = 0; }
             tail_accumulate<GONLY>(tc, lane, w0, w1, gqt, hqt);
           }
         }
@@ -661,7 +674,9 @@ static bool root_plan(int ngc, int tw, bool gonly, RootCfg* c) {
   const int PL = gonly ? 1 : 2;
   const unsigned main_b = (unsigned)ngc * PL * kPlaneBytes;
   const unsigned avail = kMaxSmem - 128 /* alignment slack */ - 2 * 8 * 16 /* barriers */;
-  const unsigned stage = (unsigned)kRootRows * (32u * ngc + 8u + tw);
+  // a stage: the tile's bins, its gradients (dense g: 4 B per row, (g,h): 8 B) and its tail bytes.  kRootRows * each of these is
+  // a multiple of 256 B, so every bulk copy's size and shared-memory address stay 16 B (and the TMA boxes 128 B) aligned
+  const unsigned stage = (unsigned)kRootRows * (32u * ngc + (gonly ? 4u : 8u) + tw);
   int trep = tw ? 32 / tw : 0;
   unsigned tail_b = (unsigned)PL * 256u * tw * trep * 4u;
   if (tw && main_b + tail_b + kTeams * stage > avail) { trep = 1; tail_b = (unsigned)PL * 256u * tw * 4u; }
@@ -751,9 +766,12 @@ void launch_hist_build(const HistArgs& a_in, int num_sms, cudaStream_t stream) {
   const int nchunks = chunks_for(a.ngroups);
   a.ng_chunk = groups_per_chunk(a.ngroups);
   static const bool no_tma = getenv("B200XGB_NO_TMA") != nullptr;
-  if (a.ridx == nullptr && !no_tma && !a.force_gather && a.gpos == nullptr) {     // the root kernel streams (g,h) pairs
+  // the root kernel streams (g,h) pairs, or in its G-only mode the dense g; the contiguous pass of a G-only payload that needs
+  // the H plane too (gpos without g_only) runs in hist_gather_kernel
+  const bool gonly = a.g_only != 0;
+  B200_CHECK(!gonly || a.gpos != nullptr, "hist: the G-only root pass reads the dense g (gpos)");
+  if (a.ridx == nullptr && !no_tma && !a.force_gather && (a.gpos == nullptr || gonly)) {
     RootCfg c; CUtensorMap tm;
-    const bool gonly = a.g_only != 0;
     if (root_plan(a.ng_chunk, a.tw, gonly, &c) && get_tensor_map(a.bins, a.n, a.row_stride, c.box_groups, kRootRows, &tm)) {
       const int gx = num_sms / nchunks > 0 ? num_sms / nchunks : 1;
       if (gonly) hist_root_kernel<true><<<dim3(gx, nchunks), kRootThreads, c.total, stream>>>(tm, a, c);

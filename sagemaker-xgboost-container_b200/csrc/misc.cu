@@ -19,7 +19,8 @@ __device__ __forceinline__ float sigmoidf_xgb(float x) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// gradient pairs: one thread per row, all K classes; also the running max|g|, max h of the round
+// gradient pairs: one thread per row, all K classes; also the running max|g|, max h of the round.  With dense_g only g is
+// stored (4 B per row instead of 8); h == 1.0f is still folded into max h, so the fixed-point scales keep their bits.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
   float mg = 0.f, mh = 0.f;
@@ -87,7 +88,7 @@ __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
       }
       g *= w; h *= w;
       if (dropped) { g = 0.f; h = 0.f; }
-      a.gpair[r] = make_float2(g, h);
+      if (a.dense_g) reinterpret_cast<float*>(a.gpair)[r] = g; else a.gpair[r] = make_float2(g, h);
       mg = fmaxf(mg, fabsf(g)); mh = fmaxf(mh, h);
     }
   }
@@ -409,6 +410,8 @@ static inline int grid_for(int64_t n, int block = 256, int cap = engine_num_sms(
   int64_t g = (n + block - 1) / block; if (g < 1) g = 1; if (g > cap) g = cap; return (int)g;
 }
 void launch_gradient(const GradArgs& a, cudaStream_t s) {
+  B200_CHECK(!a.dense_g || (a.K == 1 && a.objective == kSquaredError && a.weight == nullptr && a.subsample >= 1.0f),
+             "gradient: the dense g layout is for constant-hessian objectives only");
   if (a.n == 0) return;
   gradient_kernel<<<grid_for(a.n, 256, engine_num_sms() * 8), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }

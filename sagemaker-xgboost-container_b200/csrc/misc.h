@@ -10,6 +10,8 @@ struct GradArgs {
   const float* label; const float* weight;
   float2* gpair;            // [K][gp_stride]
   int64_t gp_stride;        // rows reserved per class (>= n, multiple of 64: keeps class blocks 16 B aligned for the TMA bulk copies)
+  int dense_g;              // constant-hessian objectives (K == 1, h == 1 for every row): gpair holds float g[gp_stride] instead of the
+                            // pairs; max h (1.0f) is folded into absmax as for the pairs
   unsigned* absmax;         // max|g|, max h as float bits (atomicMax), may be nullptr
   int* err;                 // 1 = logistic label range, 2 = multiclass label range, 3 = squaredlogerror label <= -1, 4 = poisson label < 0,
                             // 5 = gamma label <= 0, 6 = tweedie label < 0

@@ -563,8 +563,7 @@ __global__ void __launch_bounds__(256, GONLY ? (TL ? 5 : 6) : 4) part_kernel(Par
       rows[j] = 0; gp[j] = Pay{}; tl[j] = 0u;
       if (p < p1) {
         rows[j] = a.ridx_cur ? a.ridx_cur[p] : p;
-        if constexpr (GONLY) gp[j] = static_cast<const float*>(a.gp_cur)[(size_t)p * a.gp_cur_stride];
-        else gp[j] = gp_cur[p];
+        gp[j] = gp_cur[p];
         if constexpr (TL) tl[j] = a.tl_cur[p];
       }
     }
@@ -828,7 +827,7 @@ __global__ void __launch_bounds__(256, 4) scatter_kernel(RouteArgs a) {
         const unsigned r = (unsigned)(rw + (h + j) * 32);
         pv[j] = Pay{}; tv[j] = 0u;
         if ((ck[h + j] >> 16) != 0xffu) {
-          if constexpr (GONLY) pv[j] = __ldg(reinterpret_cast<const float*>(a.gpair) + (size_t)r * 2); else pv[j] = __ldg(a.gpair + r);
+          if constexpr (GONLY) pv[j] = __ldg(a.g + r); else pv[j] = __ldg(a.gpair + r);
           if constexpr (TL) tv[j] = __ldg(a.tail_row + r);
         }
       }

@@ -31,9 +31,8 @@ struct ApplyArgs {
 struct PartArgs {
   GrowState gs; TreeArrays tree; const uint8_t* bins_col; int64_t n; const unsigned* ridx_cur; unsigned* ridx_next;
   // the gradients travel with the row ids (position order): float2 (g,h) pairs, or with g_only (constant hessian, h == 1 for
-  // every row) float g alone.  gp_cur_stride: floats between two positions' g in gp_cur (2 while it is the float2 gpair of the
-  // root, 1 after); not used without g_only.
-  const void* gp_cur; void* gp_next; int gp_cur_stride; int g_only;
+  // every row) float g alone.  At the root gp_cur is the round's gradients by row, in the same layout (the dense g with g_only).
+  const void* gp_cur; void* gp_next; int g_only;
   const unsigned* tl_cur; unsigned* tl_next;  // ... and so do the 4 tail bin bytes of a row (nullptr: no 4-wide tail, or it is in bins_gather)
   int has_missing, level, max_level_nodes;
   int build_only;                             // write only the child whose histogram is built (its rows are never read again otherwise)
@@ -52,9 +51,9 @@ struct RouteArgs {
   uint8_t* node_of_row;                       // [n] the tree node each row is in
   unsigned* tile_counts;                      // [kRouteMaxBuild][ntiles]: a tile's rows per built child, then their offset in it
   unsigned ntiles; int has_missing, level;
-  // what scatter_kernel writes for a built row, read by ROW: g of the class's float2 gpair (g_only) or the pair, and the 4 tail
-  // bytes of a 4-wide tail (tail_row: bins_tail as words; nullptr when the tail does not travel with the ids)
-  const float2* gpair; int g_only; const unsigned* tail_row;
+  // what scatter_kernel writes for a built row, read by ROW: g of the dense g array (g_only; constant hessian) or the class's
+  // (g,h) pair, and the 4 tail bytes of a 4-wide tail (tail_row: bins_tail as words; nullptr when the tail does not travel with the ids)
+  const float* g; const float2* gpair; int g_only; const unsigned* tail_row;
   unsigned* ridx; void* gp; unsigned* tl;     // the built children's rows by position
   unsigned long long* rows_counter;           // optional (profiling): [0] += rows routed, [1] += rows scattered
 };
@@ -70,7 +69,8 @@ struct HistArgs {
   int tail_in_gather;           // gathered passes read the tail bytes from the row's own line of bins_gather (tail_pos unused)
   int tw;                       // tail width in bytes (0, 4, 8)
   const float2* gpair;          // (g, h) by POSITION in the row-id buffer (== by row at the root)
-  const float* gpos;            // constant hessian: g alone by POSITION, h == 1.0f for every row (gpair unused); nullptr = gpair
+  const float* gpos;            // constant hessian: g alone by POSITION (the dense g at the root), h == 1.0f for every row (gpair
+                                // unused); nullptr = gpair
   const unsigned* ridx;         // row ids by segment position; nullptr = identity (root)
   const int* build_count;       // number of nodes to build
   const int* build_nid;         // their node ids
@@ -83,7 +83,7 @@ struct HistArgs {
   int ngroups;
   int ng_chunk;                 // groups per blockIdx.y chunk (set by the launcher)
   int accumulate_sum;
-  int g_only;                   // constant-hessian root pass: accumulate G only (the slot already holds the cached H plane)
+  int g_only;                   // constant-hessian root pass: accumulate G only from gpos (the slot already holds the cached H plane)
   int window_rows;              // rows a CTA may accumulate between two int32 overflow checks (engine.h window_rows_for)
   int force_gather;             // tests / profiling: use hist_gather_kernel even for the contiguous root pass
   unsigned long long* rows_counter;   // optional: += rows processed by this launch (profiling)
