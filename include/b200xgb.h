@@ -163,6 +163,13 @@ XGB_DLL int XGB200DMatrixGetBinCopies(DMatrixHandle handle, int max_bin, int* ou
  * as every rank would.  Does not touch the matrix's own cuts.  out_ptrs: F+1, out_vals: capacity F x 256, out_mins: F. */
 XGB_DLL int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_bounds, int n_ranges, int* out_ptrs,
                           float* out_vals, float* out_mins);
+/* the alpha-quantile of each segment with the select kernels of reg:absoluteerror's leaf refresh: values[i] belongs to segment
+ * segments[i] (in [0, n_segments), or -1 = left out; NULL = every value in segment 0).  Without weights, upstream's Quantile
+ * (interpolated between order statistics); with weights (rows of weight 0 left out), the first value in sorted order whose
+ * cumulative weight reaches alpha * total, the weights counted on the training histograms' fixed-point grid for n rows.
+ * -0.0 counts as +0.0; a NaN value is an error.  out: n_segments floats, NaN for a segment without values. */
+XGB_DLL int XGB200SegmentedQuantile(const float* values, const int32_t* segments, const float* weights, bst_ulong n, int n_segments,
+                                    float alpha, float* out);
 /* flat tree arrays of the model; any pointer may be NULL. tree_offset has num_trees+1 entries. */
 XGB_DLL int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class);
 XGB_DLL int XGB200BoosterExportModel(BoosterHandle handle, int64_t* tree_offset, int32_t* tree_info, int32_t* left, int32_t* right,

@@ -379,6 +379,19 @@ class CudaBackend:
                                                    mins.ctypes.data_as(C.POINTER(C.c_float))))
         return ptrs, vals[:ptrs[-1]].copy(), mins[:F].copy()
 
+    def segmented_quantile(self, values, segments=None, weights=None, n_segments=1, alpha=0.5):
+        """The alpha-quantile of each segment with the select kernels of reg:absoluteerror's leaf refresh: float32 (n_segments,),
+        NaN for an empty segment (include/b200xgb.h XGB200SegmentedQuantile)."""
+        v = np.ascontiguousarray(values, np.float32)
+        seg = None if segments is None else np.ascontiguousarray(segments, np.int32)
+        w = None if weights is None else np.ascontiguousarray(weights, np.float32)
+        out = np.zeros(int(n_segments), np.float32)
+        fp = C.POINTER(C.c_float)
+        self._check(self.lib.XGB200SegmentedQuantile(v.ctypes.data_as(fp), None if seg is None else seg.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                     None if w is None else w.ctypes.data_as(fp), c_bst_ulong(len(v)), C.c_int(int(n_segments)),
+                                                     C.c_float(alpha), out.ctypes.data_as(fp)))
+        return out
+
     def booster_export_model(self, h):
         nt, nn = c_bst_ulong(), c_bst_ulong()
         bs = C.c_float()

@@ -283,7 +283,7 @@ static const std::map<std::string, int>& objective_table() {
   static const std::map<std::string, int> t = {{"reg:squarederror", kSquaredError}, {"reg:linear", kSquaredError}, {"binary:logistic", kBinaryLogistic},
     {"reg:logistic", kRegLogistic}, {"binary:logitraw", kLogitRaw}, {"multi:softprob", kSoftprob}, {"multi:softmax", kSoftmax},
     {"reg:squaredlogerror", kSquaredLogError}, {"reg:pseudohubererror", kPseudoHuber}, {"count:poisson", kPoisson}, {"reg:gamma", kGamma},
-    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}};
+    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}, {"reg:absoluteerror", kAbsoluteError}};
   return t;
 }
 
@@ -303,7 +303,7 @@ void Booster::configure() {
   auto ito = raw_params_.find("objective");
   if (ito != raw_params_.end()) objective_name_ = ito->second;
   auto ot = objective_table().find(objective_name_);
-  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
+  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:absoluteerror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
   p.objective = ot->second;
   if (objective_name_ == "reg:linear") objective_name_ = "reg:squarederror";
   p.num_class = (p.objective == kSoftprob || p.objective == kSoftmax) ? geti("num_class", 0) : 1;
@@ -438,6 +438,17 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
   if (objective_is_log_link(param_.objective) || param_.objective == kHinge || objective_is_survival(param_.objective)) { base_score_ = 0.5f; return; }
   cudaStream_t s = engine_stream();
   TreeBuilder& b = *builder_;
+  if (param_.objective == kAbsoluteError) {
+    // the median of the labels over every rank's rows, weighted when there are weights (on the fixed-point grid of the
+    // weights, adaptive.h); upstream averages each worker's median [UPSTREAM-RECALL: MeanAbsoluteError::InitEstimation]
+    // sizing the refresh's buffers first (and dropping any captured tree if they move) leaves none for the select to move
+    b.ensure_adaptive();
+    float med = 0.0f;
+    segmented_quantile(dtrain->d_labels.p, nullptr, dtrain->weights.empty() ? nullptr : dtrain->d_weights.p, dtrain->n, b.global_n, 1, 0.5,
+                       &med, &b.adapt, s);
+    base_score_ = std::isnan(med) ? 0.0f : med;
+    return;
+  }
   GradArgs ga{}; ga.margin = nullptr; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
   ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = nullptr; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = 1; ga.objective = param_.objective;
   ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = 1.0f; ga.seed = 0; ga.iter = 0; ga.aux = objective_aux(param_);
@@ -669,6 +680,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
     if (param_.objective == kPoisson) for (float v : y) B200_CHECK(v >= 0.0f, "PoissonRegression: label must be nonnegative");
     if (param_.objective == kGamma) for (float v : y) B200_CHECK(v > 0.0f, "GammaRegression: label must be positive.");
     if (param_.objective == kTweedie) for (float v : y) B200_CHECK(v >= 0.0f, "TweedieRegression: label must be nonnegative");
+    if (param_.objective == kAbsoluteError) for (float v : y) B200_CHECK(!std::isnan(v), "reg:absoluteerror: label must not be NaN");
     if (param_.objective == kAft)
       for (int64_t i = 0; i < dtrain->n; ++i) {
         const float lo = dtrain->label_lower[i], hi = dtrain->label_upper[i];
@@ -696,10 +708,12 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   // constant-hessian growth needs subsample >= 1, so a per-tree row sample (which copies (g,h) pairs) never sees dense g
   B200_CHECK(!(dense_g && per_tree_sample), "per-tree row sampling of a constant-hessian round");
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
+  // reg:absoluteerror: the round's residuals, read by the leaf refresh of every tree of the round
+  float* resid = objective_is_adaptive(param_.objective) ? b.ensure_adaptive() : nullptr;
   if (per_tree_sample) {
     forest_gpair_.ensure((size_t)b.gp_stride * K);
-    launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f, false);
-  } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g);
+    launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f, false, resid);
+  } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g, resid);
   if (!per_tree_sample) {
     Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
     launch_scales(b.gs, grad_bits_for(b.global_n), s);
@@ -724,11 +738,19 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
 
 // The objective's gradient pairs at `margin` into gpair ([K][gp_stride]), rows outside round `round`'s sample zeroed, max|g| and
 // max h folded into absmax (nullptr: not taken).  dense_g (constant_hessian only): g alone, as float[gp_stride].  The survival
-// objectives have their own kernels (survival.cu); every other objective runs gradient_kernel.
+// objectives have their own kernels (survival.cu), reg:absoluteerror its own (adaptive.cu), which also writes the residuals
+// fl(y - m) into resid (nullptr: not written); every other objective runs gradient_kernel.
 void Booster::launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample,
-                               bool dense_g) {
+                               bool dense_g, float* resid) {
   cudaStream_t s = engine_stream();
   const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
+  if (param_.objective == kAbsoluteError) {
+    AbsErrGradArgs aa{}; aa.margin = margin; aa.label = dm->d_labels.p; aa.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
+    aa.gpair = gpair; aa.resid = resid; aa.absmax = absmax; aa.n = dm->n; aa.row_offset = row_offset; aa.subsample = subsample; aa.seed = param_.seed;
+    aa.iter = (unsigned long long)round; aa.dense_g = dense_g ? 1 : 0;
+    launch_abserr_gradient(aa, s);
+    return;
+  }
   if (objective_is_survival(param_.objective)) {
     B200_CHECK(!dense_g, "the survival objectives write (g,h) pairs");
     SurvivalGradArgs sa{}; sa.margin = margin; sa.label = dm->d_labels.p; sa.lower = dm->d_label_lower.p; sa.upper = dm->d_label_upper.p;
@@ -755,7 +777,7 @@ void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float*
   const int64_t n = dm->n;
   DevBuf<float> d_margin; DevBuf<float2> d_gp; d_margin.alloc((size_t)n * K); d_gp.alloc((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(d_margin.p, margin, sizeof(float) * n * K, cudaMemcpyHostToDevice, s));
-  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample, false);      // always the (g,h) pairs
+  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample, false, nullptr);      // always the (g,h) pairs
   std::vector<float2> h((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(h.data(), d_gp.p, sizeof(float2) * h.size(), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
@@ -785,7 +807,7 @@ TreeBuilder& Booster::builder_for(DMatrix* dm) {
 // (launch_objective) and the tree reads them so (root_mode != 0); this one predicate decides both.  B200XGB_NO_CONSTH turns it off.
 bool Booster::constant_hessian(const DMatrix& dm) const {
   static const bool no_consth = getenv("B200XGB_NO_CONSTH") != nullptr;
-  return !no_consth && param_.objective == kSquaredError && param_.num_class == 1 && dm.weights.empty() &&
+  return !no_consth && (param_.objective == kSquaredError || param_.objective == kAbsoluteError) && param_.num_class == 1 && dm.weights.empty() &&
          param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
 }
 
@@ -802,6 +824,7 @@ TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int 
   b.upload_interaction(interaction_, dm.F); in.n_ic = (int)interaction_.size();
   in.root_mode = !constant_hessian(dm) ? 0 : b.root_h_valid && b.root_h_uid == dm.uid && b.root_h_version == dm.binned_version ? 2 : 1;
   in.world = Comm::get().world();
+  if (objective_is_adaptive(param_.objective)) { in.resid = b.adapt.resid.p; in.adaptive = dm.weights.empty() ? 1 : 2; }
   return in;
 }
 
@@ -843,6 +866,7 @@ int Booster::boosted_rounds() { configure(); return layers(); }
 static std::string default_metric(const TrainParam& p) {
   switch (p.objective) {
     case kSquaredError: case kRegLogistic: return "rmse";
+    case kAbsoluteError: return "mae";
     case kBinaryLogistic: case kLogitRaw: return "logloss";
     case kSquaredLogError: return "rmsle";
     case kPseudoHuber: return "mphe";

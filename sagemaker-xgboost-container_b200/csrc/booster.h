@@ -191,7 +191,8 @@ class Booster {
   void grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_index);
   // h == 1 for every row in every round on dm: the gradients are a dense float g and the trees grow on it (TreeInputs root_mode)
   bool constant_hessian(const DMatrix& dm) const;
-  void launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool dense_g);
+  void launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool dense_g,
+                        float* resid);
   JPtr model_to_json();
   void model_from_json(const JValue& doc);
   JPtr config_to_json();

@@ -446,6 +446,21 @@ int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_
   memcpy(out_mins, c.mins.data(), sizeof(float) * c.mins.size());
   API_END();
 }
+int XGB200SegmentedQuantile(const float* values, const int32_t* segments, const float* weights, bst_ulong n, int n_segments, float alpha,
+                            float* out) {
+  API_BEGIN();
+  B200_CHECK(n < ((bst_ulong)1 << 31), "XGB200SegmentedQuantile: more than 2^31-1 values");
+  for (bst_ulong i = 0; i < n; ++i) B200_CHECK(!std::isnan(values[i]), "XGB200SegmentedQuantile: values must not be NaN (value " + std::to_string(i) + ")");
+  static SelectScratch sc;
+  cudaStream_t s = engine_stream();
+  DevBuf<float> v, w; DevBuf<int> seg;
+  v.alloc(n); seg.alloc(segments ? n : 0); w.alloc(weights ? n : 0);
+  if (n) CUDA_OK(cudaMemcpyAsync(v.p, values, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+  if (n && segments) CUDA_OK(cudaMemcpyAsync(seg.p, segments, sizeof(int) * n, cudaMemcpyHostToDevice, s));
+  if (n && weights) CUDA_OK(cudaMemcpyAsync(w.p, weights, sizeof(float) * n, cudaMemcpyHostToDevice, s));
+  segmented_quantile(v.p, segments ? seg.p : nullptr, weights ? w.p : nullptr, (int64_t)n, (int64_t)n, n_segments, (double)alpha, out, &sc, s);
+  API_END();
+}
 int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class) {
   API_BEGIN();
   Booster* b = BST(handle); const auto& trees = b->trees();

@@ -94,13 +94,16 @@ inline size_t hist_slot_entries(int ngroups, int tw) { return (size_t)ngroups * 
 // ---------------------------------------------------------------------------------------------
 enum Objective : int { kSquaredError = 0, kBinaryLogistic = 1, kRegLogistic = 2, kLogitRaw = 3, kSoftprob = 4, kSoftmax = 5,
                        kSquaredLogError = 6, kPseudoHuber = 7, kPoisson = 8, kGamma = 9, kTweedie = 10, kHinge = 11,
-                       kAft = 12, kCox = 13 };       // survival objectives: own gradient kernels (survival.cu), not gradient_kernel
+                       kAft = 12, kCox = 13,         // survival objectives: own gradient kernels (survival.cu), not gradient_kernel
+                       kAbsoluteError = 14 };        // own gradient kernel and a leaf refresh after every tree (adaptive.cu)
 // prediction transform of an objective (upstream ObjFunction::PredTransform / ProbToMargin): 0 identity, 1 sigmoid / logit,
 // 2 exp / log (count:poisson, reg:gamma, reg:tweedie, survival:aft, survival:cox), 3 step at 0 (binary:hinge; its margin is the raw score)
 enum Transform : int { kTransformNone = 0, kTransformSigmoid = 1, kTransformExp = 2, kTransformHinge = 3 };
 inline bool objective_is_logistic(int o) { return o == kBinaryLogistic || o == kRegLogistic || o == kLogitRaw; }
 inline bool objective_is_log_link(int o) { return o == kPoisson || o == kGamma || o == kTweedie; }
 inline bool objective_is_survival(int o) { return o == kAft || o == kCox; }
+// the objective sets each leaf of a grown tree to a quantile of its rows' residuals (upstream ObjFunction::Task().UpdateTreeLeaf())
+inline bool objective_is_adaptive(int o) { return o == kAbsoluteError; }
 inline int objective_transform(int o) {
   if (o == kBinaryLogistic || o == kRegLogistic) return kTransformSigmoid;
   if (objective_is_log_link(o) || objective_is_survival(o)) return kTransformExp;

@@ -117,6 +117,11 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
   }
 }
 
+float* TreeBuilder::ensure_adaptive() {
+  if (adapt.ensure(n, max_leaves(), cap_nodes)) for (auto& tg : graphs) tg.destroy();
+  return adapt.resid.p;
+}
+
 void TreeBuilder::set_leaf_scale(float v) {
   cudaStream_t s = engine_stream();
   CUDA_OK(cudaMemcpyAsync(leaf_scale.p, &v, sizeof v, cudaMemcpyHostToDevice, s));
@@ -311,9 +316,17 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     launch_subtract(gs, hist_pool.p, slot_stride, next_half, s);
     launch_eval(eval_args(in, L + 1, in.mask ? in.mask + (size_t)(L + 1) * bm.F : nullptr), 1 << (L + 1), s);
   }
-  // prediction cache += leaf values of this tree: one row-order pass over the column-major bins, from the node each row was
-  // routed to (at most one split above its leaf) when the levels were routed
+  // the node each row was routed to (at most one split above its leaf) when the levels were routed
   const uint8_t* start = routed && D >= 2 ? node_of_row.p : nullptr;
+  if (in.adaptive) {             // reg:absoluteerror: each leaf's value becomes fl(q * lr), q the median of its rows' residuals
+    launch_locate_leaves(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, start, g_only ? nullptr : gpair.p + (size_t)k * gp_stride, &adapt, s);
+    SelectArgs sa{}; sa.values = in.resid; sa.seg = adapt.seg.p; sa.h = in.adaptive == 2 ? reinterpret_cast<const float*>(gpair.p + (size_t)k * gp_stride) + 1 : nullptr;
+    sa.h_stride = 2; sa.scales = gs.scales; sa.n = bm.n; sa.nseg = max_leaves(); sa.alpha = 0.5;
+    sa.leaf_nid = adapt.leaf_nid.p; sa.split_cond = ta.split_cond; sa.lr = in.p.eta;
+    segmented_select(sa, &adapt, [&](unsigned long long* p, size_t cnt) { collective([p, cnt, s]() { Comm::get().allreduce_sum_i64(p, cnt, s); }); },
+                     [&](unsigned* p, size_t cnt) { collective([p, cnt, s]() { Comm::get().allreduce_max_u32(p, cnt, s); }); }, s);
+  }
+  // prediction cache += leaf values of this tree: one row-order pass over the column-major bins
   timed(kProfMargin, [&] { launch_update_margin(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, start, in.margin, in.K, k, leaf_scale.p, s); });
   if (profile) prof_margin_rows += bm.n;
   pack_tree_kernel<<<(cap_nodes + 255) / 256, 256, 0, s>>>(ta, gs.n_nodes, packed.p, cap_nodes); ++g_kernel_launches;

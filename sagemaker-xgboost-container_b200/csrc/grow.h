@@ -5,6 +5,7 @@
 #include <string>
 #include <type_traits>
 #include <vector>
+#include "adaptive.h"
 #include "engine.h"
 #include "misc.h"
 #include "tree.h"
@@ -24,11 +25,16 @@ struct TreeInputs {
   int lg_iters, n_ic;                     // grow_policy=lossguide: expansions per tree (0 = depthwise); interaction constraint sets
   int K, k, world;                        // classes, the class of this tree, ranks of the job
   int root_mode;                          // 0 = accumulate G and H, 1 = G and H + snapshot of the root H plane, 2 = G only on top of it
+  // reg:absoluteerror: the round's residuals fl(y - m) by row, and the leaf refresh after the structure is final (adaptive.h):
+  // 0 = none, 1 = quantile of the rows' residuals by count, 2 = by h_q (weighted data)
+  const float* resid;
+  int adaptive;
+  int unused;                             // makes the padding explicit
 };
 static_assert(std::is_trivially_copyable<TreeInputs>::value, "TreeInputs is compared as bytes");
 static_assert(sizeof(BinnedMatrix) == 4 * sizeof(void*) + sizeof(int64_t) + 8 * sizeof(int), "BinnedMatrix has padding bytes");
 static_assert(sizeof(TrainParamDev) == 8 * 4, "TrainParamDev has padding bytes");
-static_assert(sizeof(TreeInputs) == sizeof(BinnedMatrix) + 6 * sizeof(void*) + sizeof(TrainParamDev) + 8 * 4, "TreeInputs has padding bytes");
+static_assert(sizeof(TreeInputs) == sizeof(BinnedMatrix) + 7 * sizeof(void*) + sizeof(TrainParamDev) + 10 * 4, "TreeInputs has padding bytes");
 
 // The tree block, copied to the host in one piece: the node count (padded to 64 B), then `cap` entries each of left, right,
 // parent, split_index, split_bin (int), split_cond, base_weight, loss_chg, sum_hess (float) and default_left (u8).
@@ -96,6 +102,10 @@ struct TreeBuilder {
   PinnedPool pinned; std::vector<cudaEvent_t> free_events;
   std::vector<TreeGraph> graphs;           // per class
   TreeGraph* capturing = nullptr;          // set while enqueue runs under stream capture: collectives cut the capture
+  // reg:absoluteerror: the round's residuals and the leaf refresh's buffers, allocated by ensure_adaptive (only for that objective)
+  SelectScratch adapt;
+  int max_leaves() const { return lg_iters > 0 ? lg_iters + 1 : 1 << max_depth; }
+  float* ensure_adaptive();                // sizes `adapt` for this builder (destroys the captured graphs when a buffer moves); the residual buffer
   // profiling: CUDA events around the launches of each kind and the partition's byte model
   enum ProfKind { kProfRootHist, kProfDeepHist, kProfPartition, kProfMargin, kProfKinds };
   struct ProfEvent { cudaEvent_t a, b; int kind; long long launches; };

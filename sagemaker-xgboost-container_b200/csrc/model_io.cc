@@ -35,7 +35,7 @@ static void objective_params_to_json(JValue& obj, const TrainParam& p) {
     case kPoisson: rp->set("max_delta_step", S(float_repr(p.poisson_max_delta_step))); obj.set("poisson_regression_param", rp); break;
     case kTweedie: rp->set("tweedie_variance_power", S(float_repr(p.tweedie_variance_power))); obj.set("tweedie_regression_param", rp); break;
     case kPseudoHuber: rp->set("huber_slope", S(float_repr(p.huber_slope))); obj.set("pseudo_huber_param", rp); break;
-    case kGamma: case kHinge: case kCox: break;
+    case kGamma: case kHinge: case kCox: case kAbsoluteError: break;
     case kAft: {
       static const char* dist[] = {"normal", "logistic", "extreme"};
       rp->set("aft_loss_distribution", S(dist[p.aft_dist])); rp->set("aft_loss_distribution_scale", S(float_repr(p.aft_sigma)));
