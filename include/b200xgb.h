@@ -170,6 +170,13 @@ XGB_DLL int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64
  * -0.0 counts as +0.0; a NaN value is an error.  out: n_segments floats, NaN for a segment without values. */
 XGB_DLL int XGB200SegmentedQuantile(const float* values, const int32_t* segments, const float* weights, bst_ulong n, int n_segments,
                                     float alpha, float* out);
+/* sampling_method=gradient_based on caller-given pairs (gpair: n x 2 floats (g, h)), with the select and sampling kernels of
+ * training: rag = sqrtf(g^2 + 0.1 h^2), k = max(1, (int64)(float(n) * subsample)) and the threshold u with
+ * sum_i min(1, rag_i / u) = k (0: every row is kept as it is, when k >= the rows with rag > 0); then row i with p = rag_i / u < 1
+ * and a finite rag is kept when rng_uniform(seed, stream, i) < p, as (g / p, h / p), and zeroed otherwise.
+ * *out_threshold = u; out_gpair: n x 2 floats, the sampled pairs. */
+XGB_DLL int XGB200GradientBasedSample(const float* gpair, bst_ulong n, float subsample, unsigned seed, uint64_t stream,
+                                      float* out_threshold, float* out_gpair);
 /* flat tree arrays of the model; any pointer may be NULL. tree_offset has num_trees+1 entries. */
 XGB_DLL int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class);
 XGB_DLL int XGB200BoosterExportModel(BoosterHandle handle, int64_t* tree_offset, int32_t* tree_info, int32_t* left, int32_t* right,
@@ -209,7 +216,9 @@ XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dma
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
 XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
 /* the configured objective's gradient pairs on `dmat` at the given margins (n x num_class, host), with the row sample of boosting
- * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x num_class x 2 floats (g, h) */
+ * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x num_class x 2 floats (g, h).  Under
+ * sampling_method=gradient_based that sample is the one tree 0 of each class takes: each class's own threshold over these
+ * pairs, the draws of the round's uniform sample, kept rows scaled by 1 / p (XGB200GradientBasedSample). */
 XGB_DLL int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair);
 /* CUDA-event stopwatch on the engine's stream: Start records an event, Stop records another, waits, returns ms */
 XGB_DLL int XGB200TimerStart(void);

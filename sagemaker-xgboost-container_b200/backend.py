@@ -392,6 +392,17 @@ class CudaBackend:
                                                      C.c_float(alpha), out.ctypes.data_as(fp)))
         return out
 
+    def gradient_based_sample(self, gpair, subsample, seed=0, stream=0x2000):
+        """sampling_method=gradient_based on the given (n, 2) pairs with the training kernels: (threshold u, sampled pairs (n, 2))
+        (include/b200xgb.h XGB200GradientBasedSample)."""
+        gp = np.ascontiguousarray(gpair, np.float32).reshape(-1, 2)
+        out = np.zeros_like(gp)
+        u = C.c_float()
+        fp = C.POINTER(C.c_float)
+        self._check(self.lib.XGB200GradientBasedSample(gp.ctypes.data_as(fp), c_bst_ulong(len(gp)), C.c_float(subsample), C.c_uint(int(seed)),
+                                                       C.c_uint64(int(stream)), C.byref(u), out.ctypes.data_as(fp)))
+        return np.float32(u.value), out
+
     def booster_export_model(self, h):
         nt, nn = c_bst_ulong(), c_bst_ulong()
         bs = C.c_float()

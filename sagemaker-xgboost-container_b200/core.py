@@ -242,7 +242,7 @@ def _param_items(params):
 _IGNORED_PARAMS = {
     "csv_weights", "verbosity", "verbose", "silent", "nthread", "n_jobs", "predictor", "sketch_eps", "dsplit", "prob_buffer_row",
     "deterministic_histogram", "single_precision_histogram", "updater", "refresh_leaf", "process_type", "device", "gpu_id",
-    "sampling_method", "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
+    "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
     "lambda_bias", "feature_selector", "top_k",
     "disable_default_eval_metric",
     "multi_strategy", "max_cached_hist_node", "random_state",
@@ -282,9 +282,6 @@ def _check_unapplied(k, v):
         return v
     if k == "process_type" and str(v) == "update":
         raise XGBoostError("process_type=update is not implemented by the CUDA hist builder")
-    if k == "sampling_method" and str(v) == "gradient_based":
-        warnings.warn("sampling_method=gradient_based is NOT applied; subsample uses uniform Bernoulli sampling")
-        return _DROP
     if k in _IGNORED_PARAMS:
         return _DROP
     return v

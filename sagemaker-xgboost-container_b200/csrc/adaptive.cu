@@ -242,7 +242,7 @@ __global__ void __launch_bounds__(256) quantile_prep_kernel(const int* segs, con
     int s = segs ? segs[r] : 0;
     if (s >= nseg) { *err = 1; s = -1; }
     if (w) { if (w[r] == 0.f) s = -1; mw = fmaxf(mw, w[r]); }
-    seg[r] = s < 0 ? -1 : s;
+    if (seg) seg[r] = s < 0 ? -1 : s;
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mw = fmaxf(mw, __shfl_xor_sync(0xffffffffu, mw, o));
@@ -256,6 +256,18 @@ __global__ void weight_scale_kernel(const unsigned* absmax, float* scales, int g
   scales[1] = ldexpf(1.0f, grad_bits + 1 - eh);
 }
 
+// sc->scales[1] from the all-reduced largest weight folded into sc->absmax[1]
+static void weight_scale(int64_t global_n, SelectScratch* sc, cudaStream_t s) {
+  if (Comm::get().distributed()) Comm::get().allreduce_max_u32(sc->absmax.p, 2, s);
+  weight_scale_kernel<<<1, 1, 0, s>>>(sc->absmax.p, sc->scales.p, grad_bits_for(global_n)); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+
+void weight_grid(const float* weights, int64_t n, int64_t global_n, SelectScratch* sc, cudaStream_t s) {
+  CUDA_OK(cudaMemsetAsync(sc->absmax.p, 0, 2 * sizeof(unsigned), s));
+  if (n) { quantile_prep_kernel<<<grid_for(n), 256, 0, s>>>(nullptr, weights, n, 1, nullptr, sc->absmax.p, nullptr); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
+  weight_scale(global_n, sc, s);
+}
+
 void segmented_quantile(const float* values, const int* segs, const float* weights, int64_t n, int64_t global_n, int nseg, double alpha,
                         float* out, SelectScratch* sc, cudaStream_t s) {
   B200_CHECK(nseg >= 1 && nseg <= (1 << 24), "segmented quantile: the segment count must be in [1, 2^24]");
@@ -266,10 +278,7 @@ void segmented_quantile(const float* values, const int* segs, const float* weigh
   DevBuf<int> err; err.alloc(1); err.zero(s);
   CUDA_OK(cudaMemsetAsync(sc->absmax.p, 0, 2 * sizeof(unsigned), s));
   if (n) { quantile_prep_kernel<<<grid_for(n), 256, 0, s>>>(segs, weights, n, nseg, sc->seg.p, sc->absmax.p, err.p); ++g_kernel_launches; CUDA_OK(cudaGetLastError()); }
-  if (weights) {
-    if (dist) c.allreduce_max_u32(sc->absmax.p, 2, s);
-    weight_scale_kernel<<<1, 1, 0, s>>>(sc->absmax.p, sc->scales.p, grad_bits_for(global_n)); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
-  }
+  if (weights) weight_scale(global_n, sc, s);
   SelectArgs a{}; a.values = values; a.seg = sc->seg.p; a.h = weights; a.h_stride = 1; a.scales = sc->scales.p; a.n = n; a.nseg = nseg; a.alpha = alpha;
   segmented_select(a, sc, [&](unsigned long long* p, size_t cnt) { if (dist) c.allreduce_sum_i64(p, cnt, s); },
                    [&](unsigned* p, size_t cnt) { if (dist) c.allreduce_max_u32(p, cnt, s); }, s);

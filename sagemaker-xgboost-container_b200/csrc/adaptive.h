@@ -55,6 +55,10 @@ void segmented_select(const SelectArgs& a, SelectScratch* sc, const std::functio
 void launch_locate_leaves(const TreeArrays& t, const int* n_nodes, const uint8_t* bins_col, int64_t n, int has_missing,
                           const uint8_t* node_of_row, const float2* gpair, SelectScratch* sc, cudaStream_t s);
 
+// sc->scales[1]: the fixed-point grid segmented_quantile counts `weights` on (the largest weight over all ranks, `global_n` rows).
+// Training reads it when gradient-based sampling of weighted data weighs the refresh's rows by their instance weight.
+void weight_grid(const float* weights, int64_t n, int64_t global_n, SelectScratch* sc, cudaStream_t s);
+
 // The alpha-quantile of every segment over all ranks' rows (segs nullptr: one segment of every row; weights nullptr: unweighted;
 // rows of weight 0 are left out), on the fixed-point grid of `global_n` rows.  out: nseg floats on the host, NaN when empty.
 void segmented_quantile(const float* values, const int* segs, const float* weights, int64_t n, int64_t global_n, int nseg, double alpha,

@@ -251,6 +251,8 @@ void DMatrix::ensure_binned(int max_bin) {
 // rows of tree j >= 1 of a round from kForestRowStream + 2^20 round + j (index: row); tree 0 keeps 0x2000 + round.
 constexpr uint64_t kDartSkipStream = 0x10000000000ull, kDartOneStream = 0x20000000000ull, kDartTreeStream = 0x30000000000ull;
 constexpr uint64_t kForestRowStream = 0x40000000000ull;
+// the stream tree j of boosting round `round` draws its row sample from (uniform and gradient-based sampling alike)
+static uint64_t row_stream(int round, int j) { return j == 0 ? 0x2000ull + (uint64_t)round : kForestRowStream + ((uint64_t)round << 20) + (uint64_t)j; }
 std::string subset_mask(const std::string& parent, float frac, unsigned seed, uint64_t stream) {
   if (frac >= 1.0f) return parent;
   const int F = (int)parent.size();
@@ -344,6 +346,10 @@ void Booster::configure() {
   }
   B200_CHECK(p.lambda >= 0.0f, "Parameter reg_lambda should be greater equal to 0");
   B200_CHECK(p.subsample > 0.0f && p.subsample <= 1.0f, "Parameter subsample should be in (0, 1]");
+  if (auto sm = raw_params_.find("sampling_method"); sm != raw_params_.end()) {
+    B200_CHECK(sm->second == "uniform" || sm->second == "gradient_based", "Invalid value for parameter sampling_method: " + sm->second + " (uniform, gradient_based)");
+    p.gradient_based = sm->second == "gradient_based" ? 1 : 0;
+  }
   auto tm = raw_params_.find("tree_method");
   if (tm != raw_params_.end()) {
     const std::string& t = tm->second;
@@ -698,6 +704,9 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   // a forest with row sampling draws one row sample per tree: the gradients of every row go to a round buffer first, and each
   // tree's masked copy (and its scales) is made before the tree is grown.  Otherwise every tree of the round shares them.
   const bool per_tree_sample = P > 1 && param_.subsample < 1.0f;
+  // sampling_method=gradient_based: the objective writes every row's pairs, each class's threshold is taken once per round on
+  // them (the P trees of a forest share it and differ in their draws), and each tree keeps its rows by it
+  const bool gbs = gradient_based_sampling();
   // dart forests (a dart model written elsewhere with num_parallel_tree > 1) load and predict, but do not train on
   B200_CHECK(!dart_.on || P == 1, "booster=dart with num_parallel_tree > 1 is not implemented on the CUDA hist path");
   if (!per_tree_sample) forest_gpair_.release();
@@ -707,13 +716,22 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   const bool dense_g = constant_hessian(*dtrain);
   // constant-hessian growth needs subsample >= 1, so a per-tree row sample (which copies (g,h) pairs) never sees dense g
   B200_CHECK(!(dense_g && per_tree_sample), "per-tree row sampling of a constant-hessian round");
+  // likewise constant-hessian growth never meets a gradient-based sample, whose kept rows have h / p != 1
+  B200_CHECK(!(dense_g && gbs), "gradient-based sampling of a constant-hessian round");
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
   // reg:absoluteerror: the round's residuals, read by the leaf refresh of every tree of the round
   float* resid = objective_is_adaptive(param_.objective) ? b.ensure_adaptive() : nullptr;
   if (per_tree_sample) {
     forest_gpair_.ensure((size_t)b.gp_stride * K);
     launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f, false, resid);
+    if (gbs) gradient_based_threshold(forest_gpair_.p, b.gp_stride, dtrain->n, K, param_.subsample, &gbs_, s);
+  } else if (gbs) {          // one tree per class: sampled in place
+    launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, nullptr, 1.0f, false, resid);
+    gradient_based_threshold(b.gpair.p, b.gp_stride, dtrain->n, K, param_.subsample, &gbs_, s);
+    gradient_based_sample(b.gpair.p, b.gpair.p, b.gp_stride, dtrain->n, round, 0, b.gs.absmax);
   } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g, resid);
+  // weighted reg:absoluteerror under gradient-based sampling: the refresh weighs its rows by their instance weight (h is w / p)
+  if (gbs && resid && !dtrain->weights.empty()) weight_grid(dtrain->d_weights.p, dtrain->n, b.global_n, &b.adapt, s);
   if (!per_tree_sample) {
     Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
     launch_scales(b.gs, grad_bits_for(b.global_n), s);
@@ -724,16 +742,25 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
     for (int j = 0; j < P; ++j) {
       if (per_tree_sample) {     // tree j's rows (shared by the K classes): j = 0 draws the stream a single tree draws
         CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
-        SampleArgs sa{}; sa.src = forest_gpair_.p; sa.dst = b.gpair.p; sa.absmax = b.gs.absmax; sa.gp_stride = b.gp_stride; sa.n = dtrain->n;
-        sa.row_offset = (int64_t)Comm::get().rank() << 40; sa.K = K; sa.subsample = param_.subsample; sa.seed = param_.seed;
-        sa.stream = j == 0 ? 0x2000ull + (uint64_t)round : kForestRowStream + ((uint64_t)round << 20) + (uint64_t)j;
-        launch_sample_gpair(sa, s);
+        if (gbs) gradient_based_sample(forest_gpair_.p, b.gpair.p, b.gp_stride, dtrain->n, round, j, b.gs.absmax);
+        else {
+          SampleArgs sa{}; sa.src = forest_gpair_.p; sa.dst = b.gpair.p; sa.absmax = b.gs.absmax; sa.gp_stride = b.gp_stride; sa.n = dtrain->n;
+          sa.row_offset = (int64_t)Comm::get().rank() << 40; sa.K = K; sa.subsample = param_.subsample; sa.seed = param_.seed;
+          sa.stream = row_stream(round, j);
+          launch_sample_gpair(sa, s);
+        }
         Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
         launch_scales(b.gs, grad_bits_for(b.global_n), s);
       }
       grow_one_tree(dtrain, cache, k, iteration_indptr_[round] + k * P + j);
     }
   iteration_indptr_.push_back((int)trees_.size());
+}
+
+void Booster::gradient_based_sample(const float2* src, float2* dst, int64_t gp_stride, int64_t n, int round, int j, unsigned* absmax) {
+  GbsSampleArgs a{}; a.src = src; a.dst = dst; a.absmax = absmax; a.st = gbs_.st.p; a.gp_stride = gp_stride; a.n = n;
+  a.row_offset = (int64_t)Comm::get().rank() << 40; a.K = param_.num_class; a.seed = param_.seed; a.stream = row_stream(round, j);
+  launch_gradient_based_sample(a, engine_stream());
 }
 
 // The objective's gradient pairs at `margin` into gpair ([K][gp_stride]), rows outside round `round`'s sample zeroed, max|g| and
@@ -777,7 +804,12 @@ void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float*
   const int64_t n = dm->n;
   DevBuf<float> d_margin; DevBuf<float2> d_gp; d_margin.alloc((size_t)n * K); d_gp.alloc((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(d_margin.p, margin, sizeof(float) * n * K, cudaMemcpyHostToDevice, s));
-  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, param_.subsample, false, nullptr);      // always the (g,h) pairs
+  const bool gbs = gradient_based_sampling();
+  launch_objective(dm, d_margin.p, round, d_gp.p, n, nullptr, gbs ? 1.0f : param_.subsample, false, nullptr);      // always the (g,h) pairs
+  if (gbs) {                 // the gradient-based sample of tree 0 of each class, as update_one_iter takes it
+    gradient_based_threshold(d_gp.p, n, n, K, param_.subsample, &gbs_, s);
+    gradient_based_sample(d_gp.p, d_gp.p, n, n, round, 0, nullptr);
+  }
   std::vector<float2> h((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(h.data(), d_gp.p, sizeof(float2) * h.size(), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
@@ -824,7 +856,10 @@ TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int 
   b.upload_interaction(interaction_, dm.F); in.n_ic = (int)interaction_.size();
   in.root_mode = !constant_hessian(dm) ? 0 : b.root_h_valid && b.root_h_uid == dm.uid && b.root_h_version == dm.binned_version ? 2 : 1;
   in.world = Comm::get().world();
-  if (objective_is_adaptive(param_.objective)) { in.resid = b.adapt.resid.p; in.adaptive = dm.weights.empty() ? 1 : 2; }
+  if (objective_is_adaptive(param_.objective)) {
+    in.resid = b.adapt.resid.p; in.adaptive = dm.weights.empty() ? 1 : gradient_based_sampling() ? 3 : 2;
+    if (in.adaptive == 3) in.weight = dm.d_weights.p;
+  }
   return in;
 }
 

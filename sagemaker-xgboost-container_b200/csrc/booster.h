@@ -8,6 +8,7 @@
 #include "grow.h"
 #include "json.h"
 #include "misc.h"
+#include "sampling.h"
 #include "survival.h"
 #include "tree.h"
 
@@ -154,6 +155,7 @@ class Booster {
   // class-major.  The only round <-> tree map; always starts with 0 and ends with trees_.size()
   std::vector<int> iteration_indptr_{0};
   DevBuf<float2> forest_gpair_;                 // num_parallel_tree > 1 with subsample < 1: the round's unsampled gradients
+  GbsScratch gbs_;                              // sampling_method=gradient_based: the threshold select's buffers and thresholds
   std::vector<float> weight_drop_;             // parallel to trees_: the tree's weight in every margin (booster=dart; else 1)
   DartParam dart_;
   float dart_new_weight_ = 1.0f;                // weight of the trees the current dart round grows
@@ -191,6 +193,10 @@ class Booster {
   void grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_index);
   // h == 1 for every row in every round on dm: the gradients are a dense float g and the trees grow on it (TreeInputs root_mode)
   bool constant_hessian(const DMatrix& dm) const;
+  // sampling_method=gradient_based applies (subsample < 1): the objective writes every row, the trees sample by threshold
+  bool gradient_based_sampling() const { return param_.gradient_based && param_.subsample < 1.0f; }
+  // tree j of boosting round `round` keeps rows [0, n) of src by the thresholds in gbs_ (launch_gradient_based_sample)
+  void gradient_based_sample(const float2* src, float2* dst, int64_t gp_stride, int64_t n, int round, int j, unsigned* absmax);
   void launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool dense_g,
                         float* resid);
   JPtr model_to_json();

@@ -461,6 +461,24 @@ int XGB200SegmentedQuantile(const float* values, const int32_t* segments, const 
   segmented_quantile(v.p, segments ? seg.p : nullptr, weights ? w.p : nullptr, (int64_t)n, (int64_t)n, n_segments, (double)alpha, out, &sc, s);
   API_END();
 }
+int XGB200GradientBasedSample(const float* gpair, bst_ulong n, float subsample, unsigned seed, uint64_t stream, float* out_threshold, float* out_gpair) {
+  API_BEGIN();
+  B200_CHECK(n < ((bst_ulong)1 << 31), "XGB200GradientBasedSample: more than 2^31-1 rows");
+  B200_CHECK(subsample > 0.0f && subsample <= 1.0f, "XGB200GradientBasedSample: subsample must be in (0, 1]");
+  static GbsScratch sc;
+  cudaStream_t s = engine_stream();
+  DevBuf<float2> gp; gp.alloc(n);
+  if (n) CUDA_OK(cudaMemcpyAsync(gp.p, gpair, sizeof(float2) * n, cudaMemcpyHostToDevice, s));
+  gradient_based_threshold(gp.p, (int64_t)n, (int64_t)n, 1, subsample, &sc, s);
+  GbsSampleArgs a{}; a.src = gp.p; a.dst = gp.p; a.st = sc.st.p; a.gp_stride = (int64_t)n; a.n = (int64_t)n; a.K = 1; a.seed = seed; a.stream = stream;
+  launch_gradient_based_sample(a, s);
+  GbsState st{};
+  CUDA_OK(cudaMemcpyAsync(&st, sc.st.p, sizeof st, cudaMemcpyDeviceToHost, s));
+  if (n) CUDA_OK(cudaMemcpyAsync(out_gpair, gp.p, sizeof(float2) * n, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  if (out_threshold) *out_threshold = st.u;
+  API_END();
+}
 int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class) {
   API_BEGIN();
   Booster* b = BST(handle); const auto& trees = b->trees();

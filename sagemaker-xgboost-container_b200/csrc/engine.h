@@ -119,6 +119,7 @@ struct TrainParam {
   float scale_pos_weight = 1.0f, subsample = 1.0f, colsample_bytree = 1.0f, colsample_bylevel = 1.0f, colsample_bynode = 1.0f;
   unsigned seed = 0;
   int num_parallel_tree = 1;    // trees per class per boosting round (boosted random forests)
+  int gradient_based = 0;       // sampling_method: 0 uniform, 1 gradient_based (sampling.h; only with subsample < 1)
   float huber_slope = 1.0f, tweedie_variance_power = 1.5f, poisson_max_delta_step = 0.7f;   // objective parameters (upstream defaults)
   int aft_dist = 0; float aft_sigma = 1.0f;     // survival:aft: aft_loss_distribution (survival.h AftDist), aft_loss_distribution_scale
 };

@@ -322,6 +322,7 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
     launch_locate_leaves(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, start, g_only ? nullptr : gpair.p + (size_t)k * gp_stride, &adapt, s);
     SelectArgs sa{}; sa.values = in.resid; sa.seg = adapt.seg.p; sa.h = in.adaptive == 2 ? reinterpret_cast<const float*>(gpair.p + (size_t)k * gp_stride) + 1 : nullptr;
     sa.h_stride = 2; sa.scales = gs.scales; sa.n = bm.n; sa.nseg = max_leaves(); sa.alpha = 0.5;
+    if (in.adaptive == 3) { sa.h = in.weight; sa.h_stride = 1; sa.scales = adapt.scales.p; }
     sa.leaf_nid = adapt.leaf_nid.p; sa.split_cond = ta.split_cond; sa.lr = in.p.eta;
     segmented_select(sa, &adapt, [&](unsigned long long* p, size_t cnt) { collective([p, cnt, s]() { Comm::get().allreduce_sum_i64(p, cnt, s); }); },
                      [&](unsigned* p, size_t cnt) { collective([p, cnt, s]() { Comm::get().allreduce_max_u32(p, cnt, s); }); }, s);

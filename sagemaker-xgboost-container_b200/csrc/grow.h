@@ -26,15 +26,16 @@ struct TreeInputs {
   int K, k, world;                        // classes, the class of this tree, ranks of the job
   int root_mode;                          // 0 = accumulate G and H, 1 = G and H + snapshot of the root H plane, 2 = G only on top of it
   // reg:absoluteerror: the round's residuals fl(y - m) by row, and the leaf refresh after the structure is final (adaptive.h):
-  // 0 = none, 1 = quantile of the rows' residuals by count, 2 = by h_q (weighted data)
-  const float* resid;
+  // 0 = none, 1 = quantile of the rows' residuals by count, 2 = by h_q (weighted data), 3 = by the instance weights `weight` on
+  // their own grid (adapt.scales[1], adaptive.h weight_grid): weighted data under gradient-based sampling, whose h is w / p
+  const float* resid; const float* weight;
   int adaptive;
   int unused;                             // makes the padding explicit
 };
 static_assert(std::is_trivially_copyable<TreeInputs>::value, "TreeInputs is compared as bytes");
 static_assert(sizeof(BinnedMatrix) == 4 * sizeof(void*) + sizeof(int64_t) + 8 * sizeof(int), "BinnedMatrix has padding bytes");
 static_assert(sizeof(TrainParamDev) == 8 * 4, "TrainParamDev has padding bytes");
-static_assert(sizeof(TreeInputs) == sizeof(BinnedMatrix) + 7 * sizeof(void*) + sizeof(TrainParamDev) + 10 * 4, "TreeInputs has padding bytes");
+static_assert(sizeof(TreeInputs) == sizeof(BinnedMatrix) + 8 * sizeof(void*) + sizeof(TrainParamDev) + 10 * 4, "TreeInputs has padding bytes");
 
 // The tree block, copied to the host in one piece: the node count (padded to 64 B), then `cap` entries each of left, right,
 // parent, split_index, split_bin (int), split_cond, base_weight, loss_chg, sum_hess (float) and default_left (u8).

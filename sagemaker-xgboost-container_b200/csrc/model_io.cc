@@ -254,7 +254,7 @@ JPtr Booster::config_to_json() {
   f("alpha", param_.alpha); f("colsample_bylevel", param_.colsample_bylevel); f("colsample_bynode", param_.colsample_bynode); f("colsample_bytree", param_.colsample_bytree);
   f("eta", param_.eta); f("gamma", param_.gamma); ttp->set("grow_policy", S(param_.lossguide ? "lossguide" : "depthwise")); f("lambda", param_.lambda); i("max_bin", param_.max_bin);
   f("max_delta_step", param_.max_delta_step); i("max_depth", param_.max_depth); i("max_leaves", param_.max_leaves); f("min_child_weight", param_.min_child_weight);
-  f("subsample", param_.subsample);
+  f("subsample", param_.subsample); ttp->set("sampling_method", S(param_.gradient_based ? "gradient_based" : "uniform"));
   if (!monotone_.empty()) { std::string v = "("; for (size_t j = 0; j < monotone_.size(); ++j) { if (j) v += ","; v += std::to_string(monotone_[j]); } v += ")"; ttp->set("monotone_constraints", S(v)); }
   if (!interaction_.empty()) {
     std::string v = "[";
