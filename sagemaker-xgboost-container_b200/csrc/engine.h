@@ -45,7 +45,7 @@ constexpr int kBins = 256;            // bins per feature (uint8 codes); code 25
 constexpr int kGroupEntries = kBins * kSlots;          // (bin, slot) accumulators per feature group
 constexpr int kMissingBin = 255;
 // Fixed-point grid of the gradients: |g_q| <= 2^bits, h_q <= 2^(bits+1), and a CTA checks its int32 accumulators for overflow
-// every `window` rows with window * 2^bits + 2^24 < 2^31.  Large matrices use 18 bits / 8064 rows; matrices up to 2^20 rows
+// every `window` rows with window * 2^bits = 2^31 - 2^25 (hist.cu kSpillThresholdG / H: what may stay between windows).  Large matrices use 18 bits / 8064 rows; matrices up to 2^20 rows
 // (where one-row leaves with large gradients are common and the extra overflow checks cost nothing measurable) use
 // 21 bits / 1008 rows, which keeps even a single-row leaf within 1e-5 of the double-precision reference.
 constexpr int kGradBits = 18, kWindowRows = 8064;

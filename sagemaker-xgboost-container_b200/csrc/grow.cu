@@ -82,10 +82,13 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
   }
   cap_nodes = (max_nodes + 15) & ~15;
   slot_stride = hist_slot_entries(ngroups, tw);
-  const size_t pool_bytes = pool_slots * slot_stride * sizeof(GH64);
+  const size_t partial_entries = hist_partial_entries(ngroups, tw, engine_num_sms(), max_level_nodes);
+  const size_t pool_bytes = pool_slots * slot_stride * sizeof(GH64) + partial_entries * sizeof(int2);
   size_t free_b = 0, total_b = 0; cudaMemGetInfo(&free_b, &total_b);
-  B200_CHECK(pool_bytes < free_b / 2 + hist_pool.n * sizeof(GH64), "histogram pool for this max_depth / max_leaves / feature count does not fit in device memory");
+  B200_CHECK(pool_bytes < free_b / 2 + hist_pool.n * sizeof(GH64) + hist_partials.n * sizeof(int2),
+             "histogram pool for this max_depth / max_leaves / feature count does not fit in device memory");
   hist_pool.alloc(pool_slots * slot_stride);
+  hist_partials.alloc(partial_entries);
   gpair.alloc((size_t)gp_stride * K + 512); gpair.zero(s); err.alloc(1); tree_index_dev.alloc(1);
   if (!leaf_scale.p) { leaf_scale.alloc(1); set_leaf_scale(1.0f); }
   root_h_cache.alloc(slot_stride);
@@ -166,7 +169,7 @@ HistArgs TreeBuilder::hist_args(const BinnedMatrix& bm, int k) const {
   ha.gpair = gpair.p + (size_t)k * gp_stride;
   ha.build_count = gs.build_count; ha.build_nid = gs.build_nid; ha.build_prefix = gs.build_prefix; ha.seg_begin = gs.seg_begin;
   ha.hist_slot = gs.hist_slot; ha.scales = gs.scales; ha.hist_pool = hist_pool.p; ha.node_sum = gs.node_sum; ha.ngroups = bm.ngroups;
-  ha.accumulate_sum = 1; ha.window_rows = window_rows_for(global_n);
+  ha.partials = hist_partials.p; ha.accumulate_sum = 1; ha.window_rows = window_rows_for(global_n);
   return ha;
 }
 

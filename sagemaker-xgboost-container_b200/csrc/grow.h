@@ -87,6 +87,7 @@ struct TreeBuilder {
   // the partition's two buffer sets: row ids, the gradients (float g alone in the first n floats for constant-hessian objectives)
   // and the 4 tail bytes of each row, by position.  Routed growth (routes()) writes only set 0; set 1 exists only without it.
   DevBuf<GH64> hist_pool; DevBuf<unsigned> ridx[2], scratch;
+  DevBuf<int2> hist_partials;              // the gathered histogram passes' per-segment partials (tree.h HistArgs::partials)
   // gpair: the round's gradients by row, [K][gp_stride] (g,h) pairs, or for constant-hessian growth (TreeInputs root_mode != 0,
   // K == 1) a dense float g[gp_stride] in the same allocation (g_dense)
   DevBuf<float2> gpair, gp[2]; DevBuf<unsigned> tl[2]; DevBuf<int> err, tree_index_dev; DevBuf<unsigned char> ic_path, ic_allowed, ic_sets;

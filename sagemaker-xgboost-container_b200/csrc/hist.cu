@@ -21,8 +21,9 @@
 //                          ids through the partition; g alone for constant-hessian objectives, whose h_q is a constant),
 //                          tail bytes from the pad of the row's line-aligned copy where there is one.
 //  * Gradients are rounded to a power-of-two fixed-point grid (|g_q| <= 2^18, h_q <= 2^19) so a window of 8064 rows per
-//    CTA cannot overflow int32; between windows, accumulators above 2^24 are spilled to the global int64 histogram with
-//    RED.ADD.64 (sparse), and everything is flushed at the end of the CTA's portion.  Sums are exact integers =>
+//    CTA cannot overflow int32; between windows, accumulators above 2^25 (G) / 2^26 (H) are spilled to the global int64 histogram with
+//    RED.ADD.64 (sparse), and everything is flushed at the end of the CTA's portion: by the root kernel with RED.ADD.64, by the
+//    gather kernel with plain stores into a partial slot per (CTA, node) segment that hist_reduce_kernel sums.  Sums are exact integers =>
 //    bit-reproducible for any grid size, block schedule or GPU count; the NCCL all-reduce is order-independent.
 #include <cuda.h>
 #include <cstdlib>
@@ -38,7 +39,12 @@ namespace b200 {
 
 constexpr int kSuperRows = 32;
 constexpr int kMinRowsPerCta = 4096;              // do not pay a flush for fewer rows than this
-constexpr int kSpillThreshold = 1 << 24;
+// Between windows an accumulator is spilled only when the next window could overflow it: a window adds at most
+// window * 2^bits = 2^31 - 2^25 to a G accumulator (int32) and window * 2^(bits+1) = 2^32 - 2^26 to an H accumulator (uint32;
+// engine.h), so whatever stays below 2^25 / 2^26 is safe.  (A constant hessian quantises to h_q = 2^19: an H accumulator
+// reaches 2^24 after 32 rows of one bin, about every window, and 2^26 after 128.)
+constexpr int kSpillThresholdG = 1 << 25;
+constexpr unsigned kSpillThresholdH = 1u << 26;
 constexpr int kPlaneBytes = kGroupEntries * 4;    // 32 KB
 constexpr int kMaxSmem = 232448;                  // 227 KB opt-in limit per CTA
 // root kernel: consumer warps work in teams; a ring stage (tile of kRootRows rows) is consumed by ONE team, warp w of the team
@@ -281,7 +287,7 @@ __device__ __forceinline__ void spill_main(int* smem, int ng_here, GH64* out, bo
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int val = vals[k];
-      const bool sp = last ? (val != 0) : (is_h ? ((unsigned)val >= (unsigned)kSpillThreshold) : (val >= kSpillThreshold || val <= -kSpillThreshold));
+      const bool sp = last ? (val != 0) : (is_h ? ((unsigned)val >= kSpillThresholdH) : (val >= kSpillThresholdG || val <= -kSpillThresholdG));
       if (sp) {
         red_global_s64(is_h ? &o[k].h : &o[k].g, is_h ? (long long)(unsigned)val : (long long)val);
         vals[k] = 0; any = true;
@@ -301,7 +307,7 @@ __device__ __forceinline__ void spill_tail(int* tsm, int tw, int trep, GH64* out
     const bool is_h = idx >= per_plane;
     const int e = is_h ? idx - per_plane : idx;
     const int bin = e / per_bin, slot = e & (tw - 1);
-    const bool sp = last ? true : (is_h ? ((unsigned)val >= (unsigned)kSpillThreshold) : (val >= kSpillThreshold || val <= -kSpillThreshold));
+    const bool sp = last ? true : (is_h ? ((unsigned)val >= kSpillThresholdH) : (val >= kSpillThresholdG || val <= -kSpillThresholdG));
     if (sp) {
       GH64* o = out_tail + bin * tw + slot;
       red_global_s64(is_h ? &o->h : &o->g, is_h ? (long long)(unsigned)val : (long long)val);
@@ -498,6 +504,52 @@ template <bool GPAY> struct Stage<8, GPAY> { unsigned id; typename std::conditio
 // tail planes [bin][trep][tw] of the gather kernel: 32 KB (G + H, trep * tw = 16) fit next to three groups, 64 KB otherwise
 __host__ __device__ constexpr int gather_tail_replicas(int ng) { return ng >= 3 ? 4 : 8; }
 __host__ __device__ constexpr int gather_tail_bytes(int ng) { return ng >= 3 ? 32768 : 65536; }
+// positions per super-tile of the gather kernel (see its lane mapping): 32, 32, 30 for NG = 1, 2, 3
+__host__ __device__ constexpr int gather_super_rows(int ng) { return 32 / (2 * ng) * (2 * ng); }
+
+// Rows of the build list per gather CTA: CTA x < ceff takes positions [x * chunk, min((x + 1) * chunk, T)), chunk a multiple of
+// `sup`.  hist_reduce_kernel repeats it to find the CTAs of a node.
+__device__ __forceinline__ void gather_split(unsigned T, unsigned C, unsigned sup, unsigned& ceff, unsigned& chunk) {
+  ceff = (T + kMinRowsPerCta - 1) / kMinRowsPerCta;
+  ceff = ceff < 1 ? 1 : (ceff > C ? C : ceff);
+  chunk = (T + ceff - 1) / ceff;
+  chunk = (chunk + sup - 1) / sup * sup;
+}
+
+// Final flush of a (CTA, node) segment of the gather kernel: the accumulators go to the segment's own partial slot with plain
+// coalesced 16 B stores, one {g, h} int32 pair per slot entry, and the planes are zeroed for the next segment.  The tail
+// replicas are summed first; a sum that does not fit 32 bits (only when several replicas sit near the spill threshold) goes
+// to the pool with RED.ADD.64 instead, like a spill.
+template <int TWC, int TREP>
+__device__ __forceinline__ void flush_partials(int* smem, int* tsm, int ng_here, bool has_tail, int2* part_main, int2* part_tail, GH64* out_tail,
+                                               int tid, int nthr) {
+  constexpr int kHalf = kGroupEntries / 2;
+#pragma unroll 1          // the gather kernel is register-bound: unrolled, this loop cost the one-group instantiations up to 38 registers
+  for (int i = tid; i < ng_here * kHalf; i += nthr) {
+    const int k = i / kHalf, e = (i - k * kHalf) * 2;
+    int2* G = reinterpret_cast<int2*>(smem + k * 2 * kGroupEntries + e);
+    int2* H = G + kHalf;
+    const int2 g = *G, h = *H;
+    *reinterpret_cast<int4*>(part_main + (size_t)k * kGroupEntries + e) = make_int4(g.x, h.x, g.y, h.y);
+    *G = make_int2(0, 0); *H = make_int2(0, 0);
+  }
+  if (has_tail) {
+    constexpr int kTailPlane = 256 * TWC * TREP;
+    for (int e = tid; e < 256 * TWC; e += nthr) {
+      const int bin = e / TWC, slot = e - bin * TWC;
+      long long g = 0, h = 0;
+#pragma unroll
+      for (int r = 0; r < TREP; ++r) {
+        int* t = tsm + (bin * TREP + r) * TWC + slot;
+        g += t[0]; h += (unsigned)t[kTailPlane];
+        t[0] = 0; t[kTailPlane] = 0;
+      }
+      if (g != (long long)(int)g) { red_global_s64(&out_tail[e].g, g); g = 0; }
+      if (h != (long long)(unsigned)h) { red_global_s64(&out_tail[e].h, h); h = 0; }
+      part_tail[e] = make_int2((int)g, (int)(unsigned)h);
+    }
+  }
+}
 
 // Lane mapping: a row's 32*NG contiguous bytes are fetched by 2*NG adjacent lanes of ONE LDG.128 instruction (the sectors of
 // a row reach the L2 in one request, so DRAM serves them with whole 64 B bursts: requested by separate instructions a 96 B row
@@ -512,6 +564,7 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
   constexpr int NWARPS = NTHREADS / 32;
   constexpr int LPR = 2 * NG, RPI = 32 / LPR, U = 2 * NG;                  // lanes per row, rows per instruction, units per super-tile
   constexpr int SUP = RPI * U;                                             // positions per super-tile: 32, 32, 30
+  static_assert(SUP == gather_super_rows(NG), "hist_reduce_kernel splits the rows with gather_super_rows");
   static_assert(kWindowRowsSmall / (SUP * NWARPS) >= 1, "window too small");
   const unsigned iters_per_window = (unsigned)a.window_rows / (SUP * NWARPS);   // super-tiles per warp between overflow checks
   extern __shared__ __align__(16) int smem[];                              // per group: G[8192] then H[8192]; then the tail planes
@@ -520,12 +573,9 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
   const unsigned T = a.build_prefix[nb];
   if (T == 0) return;
   if (a.rows_counter && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) atomicAdd(a.rows_counter, (unsigned long long)T);
-  const unsigned C = gridDim.x;
-  unsigned ceff = (T + kMinRowsPerCta - 1) / kMinRowsPerCta;
-  ceff = ceff < 1 ? 1 : (ceff > C ? C : ceff);
+  unsigned ceff, chunk;
+  gather_split(T, gridDim.x, SUP, ceff, chunk);
   if (blockIdx.x >= ceff) return;
-  unsigned chunk = (T + ceff - 1) / ceff;
-  chunk = (chunk + SUP - 1) / SUP * SUP;
   unsigned long long r0l = (unsigned long long)blockIdx.x * chunk;
   if (r0l >= T) return;
   unsigned r0 = (unsigned)r0l;
@@ -651,11 +701,54 @@ __global__ void __launch_bounds__(NTHREADS, NG == 1 ? (TW ? 1 : 3) : 1) hist_gat
       }
     }
     __syncthreads();
-    spill_main<2>(smem, ng_here, out_main, true, threadIdx.x, NTHREADS);
-    if (has_tail) spill_tail<2>(smem + NG * 2 * kGroupEntries, TWC, trep, out_tail, true, threadIdx.x, NTHREADS);
+    if (a.partials) {                        // segment b of CTA x: partial slot x + b (unique: a CTA's nodes are a contiguous run)
+      int2* part = a.partials + (size_t)(blockIdx.x + b) * slot_entries;
+      flush_partials<TWC, trep>(smem, smem + NG * 2 * kGroupEntries, ng_here, has_tail, part + (size_t)g0 * kGroupEntries,
+                                part + (size_t)a.ngroups * kGroupEntries, out_tail, threadIdx.x, NTHREADS);
+    } else {
+      spill_main<2>(smem, ng_here, out_main, true, threadIdx.x, NTHREADS);
+      if (has_tail) spill_tail<2>(smem + NG * 2 * kGroupEntries, TWC, trep, out_tail, true, threadIdx.x, NTHREADS);
+    }
     __syncthreads();
     if (a.accumulate_sum && blockIdx.y == 0) flush_node_sum(a.node_sum + nid, accG, accH, lane);
     r0 = nend; ++b;
+  }
+}
+
+// The partial slots of every built node added to its pool slot (which already holds the spills), in ascending CTA order.  Sums
+// of integers: the same bits as the RED.ADD.64 flush in any order.  Node b's rows lie in the gather CTAs x_lo .. x_hi of a
+// launch of C CTAs per group chunk, whose segments for it are partial slots x + b.  A thread takes two entries of a node.
+__global__ void __launch_bounds__(256) hist_reduce_kernel(HistArgs a, unsigned C, unsigned sup) {
+  const int nb = *a.build_count;
+  if (nb <= 0) return;
+  const unsigned T = a.build_prefix[nb];
+  if (T == 0) return;
+  unsigned ceff, chunk;
+  gather_split(T, C, sup, ceff, chunk);
+  const size_t slot_entries = (size_t)a.ngroups * kGroupEntries + (size_t)256 * a.tw;
+  const size_t pairs = slot_entries / 2;
+  for (size_t item = (size_t)blockIdx.x * blockDim.x + threadIdx.x; item < (size_t)nb * pairs; item += (size_t)gridDim.x * blockDim.x) {
+    const int b = (int)(item / pairs);
+    const size_t p = item - (size_t)b * pairs;
+    const unsigned nbeg = a.build_prefix[b], nend = a.build_prefix[b + 1];
+    if (nbeg == nend) continue;
+    const unsigned x_lo = nbeg / chunk, nseg = (nend - 1) / chunk - x_lo + 1;
+    const int4* src = reinterpret_cast<const int4*>(a.partials + (size_t)(x_lo + b) * slot_entries) + p;
+    long long g0 = 0, h0 = 0, g1 = 0, h1 = 0;
+    auto add = [&](const int4& v) { g0 += v.x; h0 += (unsigned)v.y; g1 += v.z; h1 += (unsigned)v.w; };
+    unsigned s = 0;
+    for (; s + 8 <= nseg; s += 8) {                     // eight loads in flight per thread
+      int4 v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = __ldcs(src + (size_t)(s + j) * pairs);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) add(v[j]);
+    }
+    for (; s < nseg; ++s) add(__ldcs(src + (size_t)s * pairs));
+    longlong2* o = reinterpret_cast<longlong2*>(a.hist_pool + (size_t)a.hist_slot[a.build_nid[b]] * slot_entries + 2 * p);
+    longlong2 e0 = o[0], e1 = o[1];
+    e0.x += g0; e0.y += h0; e1.x += g1; e1.y += h1;
+    o[0] = e0; o[1] = e1;
   }
 }
 
@@ -667,6 +760,15 @@ const char* hist_last_kernel() { return g_last_kernel; }
 
 static int chunks_for(int ngroups) { return (ngroups + 2) / 3; }
 static int groups_per_chunk(int ngroups) { const int nc = chunks_for(ngroups); return (ngroups + nc - 1) / nc; }
+// CTAs per group chunk of hist_gather_kernel
+static int gather_grid_x(int ngroups, int tw, int num_sms) {
+  const int nchunks = chunks_for(ngroups);
+  const int per_sm = groups_per_chunk(ngroups) > 1 ? 1 : (tw ? 1 : 3);   // one group: 64 KB of planes (+ 64 KB of replicated tail planes) per CTA
+  return (num_sms * per_sm + nchunks - 1) / nchunks;
+}
+size_t hist_partial_entries(int ngroups, int tw, int num_sms, int max_build) {
+  return ((size_t)gather_grid_x(ngroups, tw, num_sms) + (size_t)max_build) * hist_slot_entries(ngroups, tw);
+}
 
 // Shared-memory plan of hist_root_kernel; returns false when the ring next to the planes would be too shallow to keep
 // every team busy (3 groups of G+H planes = 192 KB: that shape uses the gather kernel for its root pass).
@@ -784,19 +886,24 @@ void launch_hist_build(const HistArgs& a_in, int num_sms, cudaStream_t stream) {
   }
   B200_CHECK(!a.g_only || a.ridx == nullptr, "hist: G-only accumulation is a root-pass mode");
   B200_CHECK(!a.g_only, "hist: the G-only root pass needs the TMA kernel (tensor-map creation failed or B200XGB_NO_TMA is set)");
-  const bool tail = a.tw > 0;
+  // the gathered passes end each (CTA, node) segment with plain stores into its partial slot and one reduce launch sums them;
+  // B200XGB_HIST_RED_FLUSH=1 keeps the RED.ADD.64 flush into the pool (the A/B reference of the tests)
+  static const bool red_flush = getenv("B200XGB_HIST_RED_FLUSH") != nullptr;
+  if (red_flush) a.partials = nullptr;
+  else B200_CHECK(a.partials != nullptr, "hist: the gathered passes need the builder's partial histograms");
   const int ng = a.ng_chunk;
-  if (ng == 1) {
-    const int per_sm = tail ? 1 : 3;          // 64 KB of planes (+ 64 KB of replicated tail planes) per CTA
-    const int gx = (num_sms * per_sm + nchunks - 1) / nchunks;
-    launch_gather<1, 256>(a, gx, nchunks, stream);
-  } else {
-    const int gx = (num_sms + nchunks - 1) / nchunks;
-    if (ng == 2) launch_gather<2, 768>(a, gx, nchunks, stream); else launch_gather<3, 768>(a, gx, nchunks, stream);
-  }
+  const int gx = gather_grid_x(a.ngroups, a.tw, num_sms);
+  if (ng == 1) launch_gather<1, 256>(a, gx, nchunks, stream);
+  else if (ng == 2) launch_gather<2, 768>(a, gx, nchunks, stream);
+  else launch_gather<3, 768>(a, gx, nchunks, stream);
   g_last_kernel = "hist_gather_kernel";
   ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());
+  if (a.partials) {
+    hist_reduce_kernel<<<num_sms * 8, 256, 0, stream>>>(a, (unsigned)gx, (unsigned)gather_super_rows(ng));
+    ++g_kernel_launches;
+    CUDA_OK(cudaGetLastError());
+  }
 }
 
 }  // namespace b200

@@ -80,6 +80,10 @@ struct HistArgs {
   const float* scales;          // sg, sh
   GH64* hist_pool;              // slot stride = hist_slot_entries(ngroups, tw)
   GH64* node_sum;               // per nid, accumulated only when accumulate_sum
+  // hist_gather_kernel's per-segment partial histograms: segment b of CTA x leaves its int32 {g, h} accumulators (h: the bits of
+  // the unsigned H accumulator) in slot entry order at partial slot x + b, and hist_reduce_kernel adds them to the pool;
+  // hist_partial_entries() entries.  B200XGB_HIST_RED_FLUSH=1 flushes with RED.ADD.64 into the pool instead.
+  int2* partials;
   int ngroups;
   int ng_chunk;                 // groups per blockIdx.y chunk (set by the launcher)
   int accumulate_sum;
@@ -96,6 +100,8 @@ void launch_lg_copy_back(const PartArgs& a, unsigned* ridx_dst, void* gp_dst, un
 void launch_zero_build_slots(const GrowState& gs, GH64* pool, size_t slot_entries, int max_build, cudaStream_t s);
 void launch_lg_stage(const GrowState& gs, GH64* pool, size_t slot_entries, int to_stage, cudaStream_t s);
 void launch_hist_build(const HistArgs& a, int num_sms, cudaStream_t stream);
+// entries of HistArgs::partials for builds of at most max_build nodes on num_sms SMs
+size_t hist_partial_entries(int ngroups, int tw, int num_sms, int max_build);
 void hist_configure();     // one-time function attributes (must happen outside stream capture)
 const char* hist_last_kernel();   // name of the kernel variant the last launch used (profiling / tests)
 void launch_init_tree(const GrowState& gs, const TreeArrays& t, unsigned n, cudaStream_t s);   // the root's histogram: slot kLgRootSlot
