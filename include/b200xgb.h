@@ -215,6 +215,10 @@ XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, i
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
 XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
+/* process_type=update: the exact fixed-point (G_q, H_q) sums of every node of every tree being updated, in the node order of the
+ * trees as they were before the update (trees one after another), 2 int64 per node; the nodes of layers not yet updated are 0.
+ * len = 0 before the first update round.  out may be NULL to query len. */
+XGB_DLL int XGB200BoosterGetRefreshSums(BoosterHandle handle, bst_ulong* len, long long* out);
 /* the configured objective's gradient pairs on `dmat` at the given margins (n x num_class, host), with the row sample of boosting
  * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x num_class x 2 floats (g, h).  Under
  * sampling_method=gradient_based that sample is the one tree 0 of each class takes: each class's own threshold over these

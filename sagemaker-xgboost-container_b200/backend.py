@@ -37,6 +37,7 @@ class CudaBackend:
     """Thin, stateless wrapper: one method per C-ABI entry point."""
 
     name = "cuda"
+    supports_process_type_update = True      # refresh / prune of loaded trees (csrc/refresh.cu)
 
     def __init__(self, path=LIB_PATH):
         if not os.path.exists(path):
@@ -496,6 +497,15 @@ class CudaBackend:
         out = np.zeros(n.value, np.float32)
         self._check(self.lib.XGB200BoosterGetTreeWeights(bh, C.byref(n), out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
+
+    def booster_refresh_sums(self, bh):
+        """process_type=update: the int64 (G_q, H_q) of every node of the trees being updated, shape (nodes, 2), in the node order
+        of the trees before the update (include/b200xgb.h XGB200BoosterGetRefreshSums)."""
+        n = c_bst_ulong()
+        self._check(self.lib.XGB200BoosterGetRefreshSums(bh, C.byref(n), None))
+        out = np.zeros(n.value, np.int64)
+        self._check(self.lib.XGB200BoosterGetRefreshSums(bh, C.byref(n), out.ctypes.data_as(C.POINTER(C.c_longlong))))
+        return out.reshape(-1, 2)
 
     def timer_start(self):
         self._check(self.lib.XGB200TimerStart())

@@ -241,7 +241,7 @@ def _param_items(params):
 # (train.py passes the validated hyperparameter dict through, SURVEY.md section 8b "boundary quirks").
 _IGNORED_PARAMS = {
     "csv_weights", "verbosity", "verbose", "silent", "nthread", "n_jobs", "predictor", "sketch_eps", "dsplit", "prob_buffer_row",
-    "deterministic_histogram", "single_precision_histogram", "updater", "refresh_leaf", "process_type", "device", "gpu_id",
+    "deterministic_histogram", "single_precision_histogram", "device", "gpu_id",
     "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
     "lambda_bias", "feature_selector", "top_k",
     "disable_default_eval_metric",
@@ -280,8 +280,13 @@ def _check_unapplied(k, v):
     if k == "tree_method" and str(v) in ("exact", "approx"):
         warnings.warn("tree_method=%s runs the CUDA hist builder (quantile-binned histograms), not xgboost's %s updater" % (v, v))
         return v
-    if k == "process_type" and str(v) == "update":
-        raise XGBoostError("process_type=update is not implemented by the CUDA hist builder")
+    # process_type=update refreshes / prunes the trees of a loaded model (the engine parses process_type, updater and refresh_leaf,
+    # which it ignores under process_type=default); an engine without it must say so rather than grow new trees, and is not sent
+    # the three parameters at all
+    if k in ("process_type", "updater", "refresh_leaf") and not getattr(get_backend(), "supports_process_type_update", False):
+        if k == "process_type" and str(v) == "update":
+            raise XGBoostError("process_type=update is not implemented by this engine")
+        return _DROP
     if k in _IGNORED_PARAMS:
         return _DROP
     return v

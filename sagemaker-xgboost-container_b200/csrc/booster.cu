@@ -420,6 +420,33 @@ void Booster::configure() {
   }
   if (!p.lossguide) B200_CHECK(p.max_depth >= 1, "max_depth=" + std::to_string(p.max_depth) + " (no depth limit) needs grow_policy=lossguide with max_leaves; the depth-wise builder takes max_depth in [1, 16]");
   if (p.max_bin > 256) p.max_bin = 256;            // uint8 bin codes (the Python layer warns)
+  // process_type=update (upstream GBTree): updater is a list of refresh / prune, "refresh,prune" or the "(refresh,prune)" of a
+  // Python list; under process_type=default updater and refresh_leaf are accepted and ignored
+  update_mode_ = false; update_ops_.clear(); update_ops_str_.clear(); refresh_leaf_ = 1;
+  if (auto pt = raw_params_.find("process_type"); pt != raw_params_.end()) {
+    B200_CHECK(pt->second == "default" || pt->second == "update", "Invalid value for parameter process_type: " + pt->second + " (default, update)");
+    update_mode_ = pt->second == "update";
+  }
+  if (update_mode_) {
+    auto up = raw_params_.find("updater");
+    B200_CHECK(up != raw_params_.end(), "process_type=update needs the parameter updater (refresh and/or prune, e.g. updater=refresh,prune)");
+    std::string tok;
+    auto flush = [&]() {
+      if (tok.empty()) return;
+      B200_CHECK(tok == "refresh" || tok == "prune", "Invalid updater under process_type=update: " + tok + " (updater may list refresh and prune only)");
+      update_ops_.push_back(tok == "refresh" ? kOpRefresh : kOpPrune);
+      update_ops_str_ += (update_ops_str_.empty() ? "" : ",") + tok; tok.clear();
+    };
+    for (char ch : up->second) {
+      if (ch == ',' || ch == '(' || ch == ')' || ch == '[' || ch == ']' || ch == '\'' || ch == '"' || std::isspace((unsigned char)ch)) flush();
+      else tok.push_back(ch);
+    }
+    flush();
+    B200_CHECK(!update_ops_.empty(), "process_type=update needs the parameter updater (refresh and/or prune, e.g. updater=refresh,prune)");
+    B200_CHECK(update_ops_.size() <= (size_t)kMaxRefreshOps, "updater lists more than " + std::to_string(kMaxRefreshOps) + " updaters");
+    refresh_leaf_ = geti("refresh_leaf", 1);
+    B200_CHECK(refresh_leaf_ == 0 || refresh_leaf_ == 1, "Parameter refresh_leaf should be 0 or 1");
+  }
   param_ = p;
   configured_ = true;
 }
@@ -661,22 +688,10 @@ static void check_train_width(const DMatrix* dm) {
              std::to_string(dm->F) + ")");
 }
 
-void Booster::update_one_iter(int iter, DMatrix* dtrain) {
-  configure();
-  (void)iter;
-  cudaStream_t s = engine_stream();
-  if (param_.objective == kAft) check_aft_bounds(dtrain); else check_labels(dtrain);
-  B200_CHECK(param_.objective != kCox || !Comm::get().distributed(), "survival:cox is not supported with more than one GPU (world_size > 1): its risk sets span the rows of every rank");
-  if (num_feature_ == 0) num_feature_ = dtrain->F;
-  B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
-             " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
-  B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
-  check_train_width(dtrain);
-  dtrain->ensure_binned(param_.max_bin);
+// label-range errors must surface from update() (the container maps them to UserError, train.py:461-467)
+void Booster::check_label_ranges(const DMatrix* dtrain) {
   const int K = param_.num_class;
-  TreeBuilder& b = builder_for(dtrain);
   if (!labels_checked_) {
-    // label-range errors must surface from update() (the container maps them to UserError, train.py:461-467)
     const std::vector<float>& y = dtrain->labels;
     if (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic || param_.objective == kLogitRaw)
       for (float v : y) B200_CHECK(v >= 0.0f && v <= 1.0f, "Check failed: label must be in [0,1] for logistic regression");
@@ -695,6 +710,24 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
       }
     labels_checked_ = true;
   }
+}
+
+void Booster::update_one_iter(int iter, DMatrix* dtrain) {
+  configure();
+  (void)iter;
+  cudaStream_t s = engine_stream();
+  if (param_.objective == kAft) check_aft_bounds(dtrain); else check_labels(dtrain);
+  B200_CHECK(param_.objective != kCox || !Comm::get().distributed(), "survival:cox is not supported with more than one GPU (world_size > 1): its risk sets span the rows of every rank");
+  if (num_feature_ == 0) num_feature_ = dtrain->F;
+  B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
+             " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
+  B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
+  if (update_mode_) { refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
+  check_train_width(dtrain);
+  dtrain->ensure_binned(param_.max_bin);
+  const int K = param_.num_class;
+  TreeBuilder& b = builder_for(dtrain);
+  check_label_ranges(dtrain);
   estimate_base_score(dtrain);
   PredCache& cache = cache_for(dtrain);
   bring_cache_up_to_date(dtrain, cache);
@@ -887,6 +920,148 @@ void Booster::grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_i
   d_trees_uploaded = 0;                      // offsets/info arrays need a refresh before the next predict
   cache.trees_applied = (int)trees_.size();  // update_margin_kernel already added this tree's leaves (times its weight) to the cache
   cache.weights.push_back(weight);
+}
+
+// ---------------------------------------------------------------------------------------------
+// process_type=update (upstream GBTree::InitUpdater / BoostNewTrees with updater=refresh,prune; DESIGN.md "Refresh and prune")
+// ---------------------------------------------------------------------------------------------
+// The model's layers become the trees to update, packed on the device once; the model keeps base_score, num_feature,
+// num_class and num_parallel_tree and nothing else, and every prediction cache starts over.
+void Booster::begin_update() {
+  cudaStream_t s = engine_stream();
+  sync_model();
+  UpdateState& u = *update_;
+  u.trees = trees_; u.tree_info = tree_info_; u.indptr = iteration_indptr_;
+  bool adjacent = true;
+  for (size_t t = 0; t < u.trees.size(); ++t) {
+    // the refresh walks the nodes reachable from the root as a tree: none of them may be the child of two of them
+    const HostTree& h = u.trees[t];
+    std::vector<char> reached((size_t)h.num_nodes(), 0); reached[0] = 1;
+    for (int i = 0; i < h.num_nodes(); ++i) {
+      if (!reached[i] || h.left[i] < 0) continue;
+      B200_CHECK(!reached[h.left[i]] && !reached[h.right[i]], "process_type=update: tree " + std::to_string(t) + " is not a tree (a node of it has two parents)");
+      reached[h.left[i]] = 1; reached[h.right[i]] = 1;
+      if (h.right[i] != h.left[i] + 1) adjacent = false;
+    }
+  }
+  reset_model();
+  children_adjacent_ = adjacent;                   // the compaction keeps sibling pairs adjacent
+  base_score_estimated_ = true;                    // never re-estimated: the trees to update were fitted on top of it
+  const int nt = (int)u.trees.size();
+  u.node_off.assign(nt + 1, 0); u.block_off.assign(nt, 0);
+  int64_t blk = 0;
+  for (int t = 0; t < nt; ++t) {
+    const int nn = u.trees[t].num_nodes();
+    u.node_off[t + 1] = u.node_off[t] + nn;
+    u.block_off[t] = blk; blk += (int64_t)((tree_block_bytes((size_t)nn) + 255) & ~(size_t)255);
+  }
+  const size_t N = (size_t)u.node_off[nt];
+  u.started = true;
+  if (N == 0) return;
+  std::vector<unsigned char> host(tree_block_bytes(N));
+  const TreeArrays h = tree_block_layout(host.data(), N).t;
+  std::vector<DevNode> dn(N);
+  for (int t = 0; t < nt; ++t) {
+    const HostTree& tr = u.trees[t];
+    for (int i = 0; i < tr.num_nodes(); ++i) {
+      const size_t j = (size_t)u.node_off[t] + i;
+      h.left[j] = tr.left[i]; h.right[j] = tr.right[i]; h.parent[j] = tr.parent[i]; h.split_index[j] = tr.split_index[i];
+      h.split_bin[j] = tr.split_bin[i]; h.default_left[j] = tr.default_left[i]; h.split_cond[j] = tr.split_cond[i];
+      h.base_weight[j] = tr.base_weight[i]; h.loss_chg[j] = tr.loss_chg[i]; h.sum_hess[j] = tr.sum_hess[i];
+      dn[j].cond = tr.split_cond[i]; dn[j].left = tr.left[i]; dn[j].right = tr.right[i];
+      dn[j].fidx_dl = (unsigned)tr.split_index[i] | ((unsigned)tr.default_left[i] << 31);
+    }
+  }
+  u.in_block.alloc(host.size()); u.nodes.alloc(N); u.d_node_off.alloc(nt + 1); u.d_class.alloc(nt); u.d_block_off.alloc(nt);
+  u.sums.alloc(N); u.scratch.alloc(3 * N); u.out_blocks.alloc((size_t)blk);
+  u.sums.zero(s);
+  CUDA_OK(cudaMemcpyAsync(u.in_block.p, host.data(), host.size(), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(u.nodes.p, dn.data(), sizeof(DevNode) * N, cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(u.d_node_off.p, u.node_off.data(), sizeof(int) * (nt + 1), cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(u.d_class.p, u.tree_info.data(), sizeof(int) * nt, cudaMemcpyHostToDevice, s));
+  CUDA_OK(cudaMemcpyAsync(u.d_block_off.p, u.block_off.data(), sizeof(int64_t) * nt, cudaMemcpyHostToDevice, s));
+  Comm::get().sync_stream(s);                     // the host copies go out of scope
+}
+
+// Update round r: the gradients at the margin of the layers refreshed so far, the per-node sums of layer r's trees over every
+// row, then refresh / prune / compaction of each tree on the device, and the trees into the model as grown trees would go.
+void Booster::refresh_one_iter(DMatrix* dtrain) {
+  cudaStream_t s = engine_stream();
+  B200_CHECK(!dart_.on, "process_type=update is not implemented for booster=dart");
+  check_label_ranges(dtrain);
+  if (!update_->started) begin_update();
+  UpdateState& u = *update_;
+  const int round = layers();
+  B200_CHECK(round < u.layers(), "boosting rounds cannot exceed the previous training rounds under process_type=update (the model to update has " +
+             std::to_string(u.layers()) + " rounds)");
+  const int K = param_.num_class;
+  const int t0 = u.indptr[round], t1 = u.indptr[round + 1], T = t1 - t0;
+  for (int t = t0; t < t1; ++t) B200_CHECK(u.tree_info[t] >= 0 && u.tree_info[t] < K, "process_type=update: tree " + std::to_string(t) + " belongs to class " +
+                                           std::to_string(u.tree_info[t]) + " but num_class is " + std::to_string(K));
+  // the fixed-point grid follows the rows of the whole job, as for growth (TreeBuilder::ensure): N GPUs and one agree
+  if (u.global_n_uid != dtrain->uid || u.global_n == 0) {
+    u.global_n = dtrain->n;
+    if (Comm::get().distributed()) {
+      DevBuf<double> dsum; dsum.alloc(1); double v = (double)dtrain->n;
+      CUDA_OK(cudaMemcpyAsync(dsum.p, &v, sizeof v, cudaMemcpyHostToDevice, s));
+      Comm::get().allreduce_sum_f64(dsum.p, 1, s);
+      CUDA_OK(cudaMemcpyAsync(&v, dsum.p, sizeof v, cudaMemcpyDeviceToHost, s));
+      Comm::get().sync_stream(s);
+      u.global_n = (int64_t)v;
+    }
+    u.global_n_uid = dtrain->uid;
+  }
+  PredCache& cache = cache_for(dtrain);
+  bring_cache_up_to_date(dtrain, cache);
+  // every row's (g, h) pairs (the refresher uses every row: no row sampling) and the round's fixed-point scales
+  const int64_t n = dtrain->n;
+  u.gpair.ensure((size_t)std::max<int64_t>(n, 1) * K); u.absmax.ensure(2); u.scales.ensure(4);
+  if (!builder_->err.p) { builder_->err.alloc(1); builder_->err.zero(s); }     // the label-error flag gradient_kernel writes
+  CUDA_OK(cudaMemsetAsync(u.absmax.p, 0, 8, s));
+  launch_objective(dtrain, cache.margin.p, round, u.gpair.p, n, u.absmax.p, 1.0f, false, nullptr);
+  Comm::get().allreduce_max_u32(u.absmax.p, 2, s);
+  GrowState gs{}; gs.absmax = u.absmax.p; gs.scales = u.scales.p;
+  launch_scales(gs, grad_bits_for(u.global_n), s);
+  // the layer's leaf sums, exact int64, all-reduced over the ranks
+  const int base = u.node_off[t0], nl = u.node_off[t1] - base;
+  const size_t N = (size_t)u.node_off.back();
+  CUDA_OK(cudaMemsetAsync(u.sums.p + base, 0, sizeof(GH64) * nl, s));
+  RefreshSumArgs sa{}; sa.X = dtrain->X.p; sa.n = n; sa.F = dtrain->F; sa.nodes = u.nodes.p; sa.tree_node_off = u.d_node_off.p + t0;
+  sa.tree_class = u.d_class.p + t0; sa.T = T; sa.layer_nodes = nl; sa.gpair = u.gpair.p; sa.gp_stride = n; sa.scales = u.scales.p; sa.sums = u.sums.p;
+  launch_refresh_sums(sa, s);
+  Comm::get().allreduce_sum_i64(u.sums.p + base, 2 * (size_t)nl, s);
+  // refresh / prune / compaction, straight into the device model and the trees' blocks
+  reserve_nodes((size_t)nl, 64 * (size_t)nl);
+  RefreshTreeArgs ta{}; ta.in = tree_block_layout(u.in_block.p, N).t; ta.tree_node_off = u.d_node_off.p + t0; ta.T = T; ta.sums = u.sums.p;
+  ta.scales = u.scales.p; ta.p = to_dev(param_); ta.nops = (int)update_ops_.size();
+  for (int i = 0; i < ta.nops; ++i) ta.ops[i] = update_ops_[i];
+  ta.refresh_leaf = refresh_leaf_; ta.scratch = u.scratch.p; ta.total_nodes = (int64_t)N; ta.out_blocks = u.out_blocks.p; ta.block_off = u.d_block_off.p;
+  ta.first_tree = t0; ta.out_nodes = d_nodes.p + d_nodes_used;
+  launch_refresh_trees(ta, s);
+  TreeBuilder& b = *builder_;
+  for (int t = t0; t < t1; ++t) {
+    const size_t nn = (size_t)u.trees[t].num_nodes();
+    if (pending_.size() - (size_t)std::count_if(pending_.begin(), pending_.end(), [](const PendingTree& p) { return p.staging == nullptr; }) >= 512) sync_model();
+    PendingTree pt; pt.cap_nodes = nn; pt.staging = b.pinned.take(tree_block_bytes(nn));
+    if (!b.free_events.empty()) { pt.ready = b.free_events.back(); b.free_events.pop_back(); }
+    else CUDA_OK(cudaEventCreateWithFlags(&pt.ready, cudaEventDisableTiming));
+    CUDA_OK(cudaMemcpyAsync(pt.staging, u.out_blocks.p + u.block_off[t], tree_block_bytes(nn), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaEventRecord(pt.ready, s));
+    append_device_tree(u.tree_info[t], d_nodes_used + (size_t)(u.node_off[t] - base), (int)nn, pt, 1.0f);
+  }
+  d_nodes_used += (size_t)nl;
+  d_trees_uploaded = 0;                      // offsets/info arrays need a refresh before the next predict
+  iteration_indptr_.push_back((int)trees_.size());
+}
+
+void Booster::debug_refresh_sums(std::vector<long long>* out) {
+  const UpdateState& u = *update_;
+  const size_t N = u.node_off.empty() ? 0 : (size_t)u.node_off.back();
+  out->assign(2 * N, 0);
+  if (N == 0 || !u.sums.p) return;
+  cudaStream_t s = engine_stream();
+  CUDA_OK(cudaMemcpyAsync(out->data(), u.sums.p, sizeof(GH64) * N, cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
 }
 
 void Booster::boost_one_iter(DMatrix*, const float*, const float*, size_t) {

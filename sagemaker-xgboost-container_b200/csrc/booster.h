@@ -8,6 +8,7 @@
 #include "grow.h"
 #include "json.h"
 #include "misc.h"
+#include "refresh.h"
 #include "sampling.h"
 #include "survival.h"
 #include "tree.h"
@@ -73,6 +74,21 @@ struct HostTree {
   int num_nodes() const { return (int)left.size(); }
 };
 
+// process_type=update: the trees to update, taken out of the model at the first update round, and the refresh's device buffers
+struct UpdateState {
+  bool started = false;
+  std::vector<HostTree> trees; std::vector<int> tree_info;
+  std::vector<int> indptr{0};                   // layer r = trees [indptr[r], indptr[r + 1])
+  std::vector<int> node_off;                    // [trees + 1]: the trees packed one after another
+  std::vector<int64_t> block_off;               // [trees]: each tree's result block in out_blocks
+  DevBuf<unsigned char> in_block;               // the trees as grow.h tree_block_layout(in_block, total nodes)
+  DevBuf<DevNode> nodes; DevBuf<int> d_node_off, d_class; DevBuf<int64_t> d_block_off;
+  DevBuf<GH64> sums; DevBuf<int> scratch; DevBuf<unsigned char> out_blocks;
+  DevBuf<float2> gpair; DevBuf<unsigned> absmax; DevBuf<float> scales;
+  int64_t global_n = 0; uint64_t global_n_uid = 0;   // rows of the job for the matrix with uid global_n_uid
+  int layers() const { return (int)indptr.size() - 1; }
+};
+
 struct PredCache {
   DevBuf<float> margin; int trees_applied = 0; int64_t n = 0; uint64_t model_version = 0;
   std::vector<float> weights;     // the weight each applied tree was added with (booster=dart changes them after the fact)
@@ -127,6 +143,8 @@ class Booster {
   void set_profile(bool on);
   // the configured objective's gradient pairs at the given host margins [n][K], with round `round`'s row sample; out [n][K][2]
   void debug_gradient(DMatrix* dm, const float* margin, int round, float* out);
+  // process_type=update: the (G_q, H_q) sums of every node of the trees being updated (include/b200xgb.h XGB200BoosterGetRefreshSums)
+  void debug_refresh_sums(std::vector<long long>* out);
   std::string get_profile();                      // JSON, see include/b200xgb.h
   // histogram of one node for kernel-level parity tests / the roofline bench
   // mode: 0 = production choice (TMA root kernel), 1 = gather kernel, 2 = G-only TMA root kernel (H plane stays zero);
@@ -174,8 +192,14 @@ class Booster {
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1
+  // process_type=update: the updaters in order (refresh.h RefreshOp), refresh_leaf, and the trees being updated
+  bool update_mode_ = false; std::vector<int> update_ops_; std::string update_ops_str_; int refresh_leaf_ = 1;
+  std::unique_ptr<UpdateState> update_ = std::make_unique<UpdateState>();
 
   void configure();
+  void check_label_ranges(const DMatrix* dtrain);
+  void begin_update();                               // the model's layers become the trees to update; the model is emptied
+  void refresh_one_iter(DMatrix* dtrain);            // one update round: the next layer refreshed / pruned into the model
   int layers() const { return (int)iteration_indptr_.size() - 1; }
   float base_margin() const;
   void estimate_base_score(DMatrix* dtrain);

@@ -592,6 +592,14 @@ int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out
   if (out) memcpy(out, w.data(), sizeof(float) * w.size());
   API_END();
 }
+int XGB200BoosterGetRefreshSums(BoosterHandle handle, bst_ulong* len, long long* out) {
+  API_BEGIN();
+  std::vector<long long> v;
+  BST(handle)->debug_refresh_sums(&v);
+  if (len) *len = v.size();
+  if (out) memcpy(out, v.data(), sizeof(long long) * v.size());
+  API_END();
+}
 int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair) {
   API_BEGIN();
   B200_CHECK(round >= 0, "XGB200BoosterComputeGradient: round must be >= 0");

@@ -41,7 +41,7 @@ static_assert(sizeof(TreeInputs) == sizeof(BinnedMatrix) + 8 * sizeof(void*) + s
 // parent, split_index, split_bin (int), split_cond, base_weight, loss_chg, sum_hess (float) and default_left (u8).
 inline size_t tree_block_bytes(size_t cap) { return 64 + 9 * 4 * cap + cap; }
 struct TreeBlock { int* n_nodes; TreeArrays t; };
-inline TreeBlock tree_block_layout(void* base, size_t cap) {
+__host__ __device__ inline TreeBlock tree_block_layout(void* base, size_t cap) {     // the tree refresh writes blocks on the device
   int* ip = (int*)((unsigned char*)base + 64); float* fp = (float*)(ip + 5 * cap);
   return {(int*)base, {ip, ip + cap, ip + 2 * cap, ip + 3 * cap, ip + 4 * cap, (unsigned char*)(fp + 4 * cap), fp, fp + cap, fp + 2 * cap, fp + 3 * cap}};
 }

@@ -8,6 +8,7 @@
 #include "engine.h"
 #include "misc.h"
 #include "rng.h"
+#include "traverse.h"
 
 namespace b200 {
 
@@ -225,16 +226,8 @@ __global__ void __launch_bounds__(256) predict_kernel(PredictArgs a) {
   const int nt = a.tree_end - a.tree_begin;
   float acc = (a.K == 1 && a.margin) ? a.margin[r] : 0.f;
   for (int t = a.tree_begin; t < a.tree_end; ++t) {
-    const DevNode* nodes = a.nodes + a.tree_offset[t];
-    int nid = 0;
-    DevNode nd = nodes[0];
-    while (nd.left != -1) {
-      const unsigned f = nd.fidx_dl & 0x7fffffffu;
-      const float v = f < (unsigned)a.F ? __ldg(x + f) : __int_as_float(0x7fc00000);
-      if (isnan(v)) nid = (nd.fidx_dl >> 31) ? nd.left : nd.right;
-      else nid = v < nd.cond ? nd.left : nd.right;
-      nd = nodes[nid];
-    }
+    DevNode nd;
+    const int nid = tree_leaf(a.nodes + a.tree_offset[t], x, a.F, &nd);
     if (a.margin) { if (a.K == 1) acc += nd.cond; else a.margin[r * a.K + a.tree_info[t]] += nd.cond; }
     if (a.leaf) a.leaf[r * nt + (t - a.tree_begin)] = nid;
   }

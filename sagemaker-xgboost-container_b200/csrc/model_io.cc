@@ -117,6 +117,7 @@ template <typename T, typename F> static std::vector<T> num_vec(const JValue& a,
 void Booster::model_from_json(const JValue& doc) {
   const JValue& learner = doc.at("learner");
   reset_model();
+  update_ = std::make_unique<UpdateState>();     // process_type=update starts over from the loaded trees
   attrs.clear();
   if (auto a = learner.get("attributes")) for (auto& kv : a->obj) attrs[kv.first] = kv.second->s;
   feature_names.clear(); feature_types.clear();
@@ -248,13 +249,15 @@ JPtr Booster::config_to_json() {
   learner->set("generic_param", gp);
   JPtr gb = JValue::Object(); gb->set("name", S("gbtree"));
   JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S(std::to_string(param_.num_parallel_tree))); gmp->set("num_trees", S(std::to_string(trees_.size()))); gb->set("gbtree_model_param", gmp);
-  JPtr gtp = JValue::Object(); gtp->set("process_type", S("default")); gtp->set("tree_method", S("hist")); gtp->set("updater", S("grow_b200_hist")); gb->set("gbtree_train_param", gtp);
+  JPtr gtp = JValue::Object(); gtp->set("process_type", S(update_mode_ ? "update" : "default")); gtp->set("tree_method", S("hist"));
+  gtp->set("updater", S(update_mode_ ? update_ops_str_ : "grow_b200_hist")); gb->set("gbtree_train_param", gtp);
   JPtr ttp = JValue::Object();
   auto f = [&](const char* k, float v) { ttp->set(k, S(float_repr(v))); }; auto i = [&](const char* k, int v) { ttp->set(k, S(std::to_string(v))); };
   f("alpha", param_.alpha); f("colsample_bylevel", param_.colsample_bylevel); f("colsample_bynode", param_.colsample_bynode); f("colsample_bytree", param_.colsample_bytree);
   f("eta", param_.eta); f("gamma", param_.gamma); ttp->set("grow_policy", S(param_.lossguide ? "lossguide" : "depthwise")); f("lambda", param_.lambda); i("max_bin", param_.max_bin);
   f("max_delta_step", param_.max_delta_step); i("max_depth", param_.max_depth); i("max_leaves", param_.max_leaves); f("min_child_weight", param_.min_child_weight);
   f("subsample", param_.subsample); ttp->set("sampling_method", S(param_.gradient_based ? "gradient_based" : "uniform"));
+  if (update_mode_) i("refresh_leaf", refresh_leaf_);
   if (!monotone_.empty()) { std::string v = "("; for (size_t j = 0; j < monotone_.size(); ++j) { if (j) v += ","; v += std::to_string(monotone_[j]); } v += ")"; ttp->set("monotone_constraints", S(v)); }
   if (!interaction_.empty()) {
     std::string v = "[";
@@ -296,6 +299,10 @@ void Booster::config_from_json(const JValue& doc) {
       if (auto inner = gb->get("gbtree")) gb = inner;
     }
     if (auto ttp = gb->get("tree_train_param")) for (auto& kv : ttp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+    if (auto gtp = gb->get("gbtree_train_param")) if (auto pt = gtp->get("process_type")) if (pt->type == JValue::kString && pt->s == "update") {
+      raw_params_["process_type"] = "update";          // the default mode's gbtree_train_param names this engine's own updater
+      if (auto up = gtp->get("updater")) if (up->type == JValue::kString) raw_params_["updater"] = up->s;
+    }
     if (auto gmp = gb->get("gbtree_model_param")) if (auto v = gmp->get("num_parallel_tree")) if (v->type == JValue::kString) raw_params_["num_parallel_tree"] = v->s;
   }
   if (auto gp = learner.get("generic_param")) if (auto sd = gp->get("seed")) raw_params_["seed"] = sd->s;
