@@ -141,6 +141,16 @@ XGB_DLL int XGB200DMatrixCreateFromCSVEx(const char* text, bst_ulong len, char d
  * *status: 0 ok; 2 = the body holds something the Python routes treat specially (non-digit index, literal outside the exact
  * fast path, repeated index in a line, trailing empty lines ...): take the host route; 3 = no entry at all (ditto). */
 XGB_DLL int XGB200DMatrixCreateFromLibsvmText(const char* text, bst_ulong len, int whitespace_mode, float absent, int* status, DMatrixHandle* out);
+/* A recordio-protobuf body (application/x-recordio-protobuf: the whole request, or the concatenated files of a training channel)
+ * decoded on the device into the DMatrix that xgb.DMatrix(features, label=labels) holds for the reference's
+ * `features, labels = read_recordio_protobuf(buf)`: encoder.recordio_protobuf_to_dmatrix (serve_utils.py:144-145) and
+ * data_utils.get_recordio_protobuf_dmatrix (data_utils.py:450-453).  features["values"] of every record is a row (dense, or sparse
+ * when its tensor has keys), label["values"] values are concatenated into the "label" info.  *status: 0 = decoded (*out set);
+ * 1 = the reference raises ValueError for this body (bad magic, truncated record, rows of different widths, no record): the
+ * message is what XGBGetLastError() returns; 2 = the body holds an encoding the device path does not decide (unpacked or
+ * repeated fields, merged messages, a repeated "values" key, malformed protobuf ...): decode it on the host.  The return value
+ * is non-zero only for a failure of the library itself. */
+XGB_DLL int XGB200DMatrixCreateFromRecordIO(const char* buf, bst_ulong len, int* status, DMatrixHandle* out);
 XGB_DLL int XGB200CommPeerReduceActive(void);
 /* Columnar training input without a dense float32 matrix on the host (Parquet through pyarrow, pandas frames): `ncols` host
  * buffers of `nrow` items each, col_types[c] in {0 f32, 1 f64, 2 i32, 3 i64, 4 u8, 5 i8, 6 i16, 7 u16, 8 u32, 9 u64, 10 bool};

@@ -147,6 +147,17 @@ class CudaBackend:
         self._check(self.lib.XGB200DMatrixCreateFromLibsvmText(text, C.c_ulong(length), C.c_int(whitespace_mode), C.c_float(absent), C.byref(st), C.byref(h)))
         return (h if st.value == 0 else None), int(st.value)
 
+    def dmatrix_from_recordio(self, buf):
+        """Device-side decode of a recordio-protobuf body (recordio.cu).  Returns (handle, status, message); handle is None
+        unless status == 0, message names the rule the body breaks when status == 1 (include/b200xgb.h)."""
+        body = np.frombuffer(buf, np.uint8)              # bytes / bytearray / memoryview without a copy
+        h = C.c_void_p()
+        st = C.c_int(0)
+        self._check(self.lib.XGB200DMatrixCreateFromRecordIO(C.c_void_p(body.ctypes.data if body.size else None), c_bst_ulong(body.size),
+                                                             C.byref(st), C.byref(h)))
+        message = self.lib.XGBGetLastError().decode("utf-8", "replace") if st.value == 1 else ""
+        return (h if st.value == 0 else None), int(st.value), message
+
     def dmatrix_from_csv(self, payload, delimiter=","):
         """Device-side CSV parse (csv.cu).  Returns (handle, status); handle is None unless status == 0."""
         h = C.c_void_p()

@@ -51,6 +51,8 @@ class DMatrix {
   // label_col / weight_col (-1 = none) become the label / weight info, the others the features in order
   static std::unique_ptr<DMatrix> from_columns(const void* const* cols, const int* types, int ncols, int64_t nrow, int label_col, int weight_col);
   static std::unique_ptr<DMatrix> from_csr(const size_t* indptr, const unsigned* indices, const float* data, size_t nindptr, size_t nelem, size_t ncol);
+  // recordio-protobuf body (recordio.cu): status 0 decoded, 1 the body is invalid (*message names the rule), 2 needs the host route
+  static std::unique_ptr<DMatrix> from_recordio(const char* buf, int64_t len, int* status, std::string* message);
   std::unique_ptr<DMatrix> slice(const int* idx, int64_t len) const;
   void set_float_info(const std::string& field, const float* v, size_t len);
   const std::vector<float>& get_float_info(const std::string& field) const;
@@ -63,6 +65,10 @@ class DMatrix {
  private:
   void bin_with_cuts();
 };
+
+// device half of DMatrix::from_csr (ingest.cu): X (nrow x F) filled with NaN, then row r's entries [d_ptr[r], d_ptr[r + 1]) stored
+// at their indices (an index repeated inside a row keeps its last value); asynchronous on stream s
+void csr_to_dense_device(const unsigned long long* d_ptr, const unsigned* d_idx, const float* d_val, int64_t nrow, int F, float* X, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------------
 // model

@@ -550,6 +550,16 @@ int XGB200DMatrixCreateFromLibsvmText(const char* text, bst_ulong len, int white
   if (st == 0) { auto box = new DMatrixBox(); box->dm = std::move(dm); *out = box; }
   API_END();
 }
+int XGB200DMatrixCreateFromRecordIO(const char* buf, bst_ulong len, int* status, DMatrixHandle* out) {
+  API_BEGIN();
+  B200_CHECK(status != nullptr && out != nullptr && (buf != nullptr || len == 0), "XGB200DMatrixCreateFromRecordIO: NULL argument");
+  std::string msg;
+  auto dm = DMatrix::from_recordio(buf, (int64_t)len, status, &msg);
+  *out = nullptr;
+  if (*status == 0) { auto box = new DMatrixBox(); box->dm = std::move(dm); *out = box; }
+  if (*status == 1) g_last_error = msg;      // the rule the body breaks, for the caller's ValueError
+  API_END();
+}
 int XGB200BuildRootHistogram(BoosterHandle handle, DMatrixHandle dmat, const float* gpair, int repeats, int64_t* out_hist, float* scales, float* out_ms) {
   API_BEGIN();
   DMatrix* dm = DM(dmat);

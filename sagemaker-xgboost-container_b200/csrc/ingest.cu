@@ -73,16 +73,32 @@ __global__ void fill_nan_kernel(float* X, int64_t count) {
   const float nan = __int_as_float(0x7fc00000);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) X[i] = nan;
 }
-// one warp per row: the row's entries land in its own F floats (an index repeated inside a row keeps one of its values)
+// one warp per row: the row's entries land in its own F floats.  An index repeated inside a row keeps the value that comes
+// last in the row: within a 32-entry chunk only the highest lane of each index stores, and chunks are ordered by __syncwarp.
 __global__ void csr_scatter_kernel(const unsigned long long* __restrict__ indptr, const unsigned* __restrict__ indices, const float* __restrict__ vals,
                                    int64_t nrow, int F, float* __restrict__ X) {
   const int lane = threadIdx.x & 31;
   for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < nrow; r += ((int64_t)gridDim.x * blockDim.x) >> 5) {
     const unsigned long long a = indptr[r], z = indptr[r + 1];
-    for (unsigned long long j = a + lane; j < z; j += 32) X[r * F + indices[j]] = vals[j];
+    for (unsigned long long j0 = a; j0 < z; j0 += 32) {
+      const unsigned long long j = j0 + lane;
+      const unsigned c = j < z ? indices[j] : 0xffffffffu;                      // F < 2^31: no real index equals the pad
+      const unsigned same = __match_any_sync(0xffffffffu, c);
+      if (j < z && (same >> lane) == 1u) X[r * F + c] = vals[j];
+      __syncwarp();
+    }
   }
 }
 }  // namespace
+
+void csr_to_dense_device(const unsigned long long* d_ptr, const unsigned* d_idx, const float* d_val, int64_t nrow, int F, float* X, cudaStream_t s) {
+  if (nrow * (int64_t)F <= 0) return;
+  const int sms = engine_num_sms();
+  fill_nan_kernel<<<sms * 8, 256, 0, s>>>(X, nrow * (int64_t)F); ++g_kernel_launches;
+  const int grid = (int)std::min<int64_t>((nrow * 32 + 255) / 256, (int64_t)sms * 16);
+  csr_scatter_kernel<<<std::max(grid, 1), 256, 0, s>>>(d_ptr, d_idx, d_val, nrow, F, X); ++g_kernel_launches;
+  CUDA_OK(cudaGetLastError());
+}
 
 std::unique_ptr<DMatrix> DMatrix::from_columns(const void* const* cols, const int* types, int ncols, int64_t nrow, int label_col, int weight_col) {
   B200_CHECK(ncols >= 0 && nrow >= 0 && nrow < (int64_t)0x7fffffff, "DMatrix: bad shape");
@@ -149,11 +165,7 @@ std::unique_ptr<DMatrix> DMatrix::from_csr(const size_t* indptr, const unsigned*
     CUDA_OK(cudaMemcpyAsync(d_ptr.p, indptr, sizeof(size_t) * nindptr, cudaMemcpyHostToDevice, s));
     if (nelem) { CUDA_OK(cudaMemcpyAsync(d_idx.p, indices, sizeof(unsigned) * nelem, cudaMemcpyHostToDevice, s));
                  CUDA_OK(cudaMemcpyAsync(d_val.p, data, sizeof(float) * nelem, cudaMemcpyHostToDevice, s)); }
-    const int sms = engine_num_sms();
-    fill_nan_kernel<<<sms * 8, 256, 0, s>>>(dm->X.p, (int64_t)(nrow * F)); ++g_kernel_launches;
-    const int grid = (int)std::min<int64_t>(((int64_t)nrow * 32 + 255) / 256, (int64_t)sms * 16);
-    csr_scatter_kernel<<<std::max(grid, 1), 256, 0, s>>>(d_ptr.p, d_idx.p, d_val.p, (int64_t)nrow, (int)F, dm->X.p); ++g_kernel_launches;
-    CUDA_OK(cudaGetLastError());
+    csr_to_dense_device(d_ptr.p, d_idx.p, d_val.p, (int64_t)nrow, (int)F, dm->X.p, s);
     Comm::get().sync_stream(s);                 // the staging buffers above die with this scope
   }
   dm->finish_upload(std::nanf(""));

@@ -162,6 +162,41 @@ def _arrow_columns(table):
     return cols
 
 
+def _is_data_file(file_path, file_name):
+    """data_utils._is_data_file (data_utils.py:120-139): a regular file, not hidden, not an xgboost cache file."""
+    if not os.path.isfile(os.path.join(file_path, file_name)):
+        return False
+    if file_name.startswith(".") or file_name.startswith("_"):
+        return False
+    return not (".cache" in file_name and ("dtrain" in file_name or "dval" in file_name))
+
+
+def recordio_protobuf_to_dmatrix(files_path, is_pipe=False):
+    """recordio-protobuf channel -> DMatrix, or None when the directory holds no data file: what
+    data_utils.get_recordio_protobuf_dmatrix builds (data_utils.py:418-459).  The files, sorted, are read into one buffer
+    (no second copy to join them) that is decoded on the device (csrc/recordio.cu).  Pipe mode is refused, as there."""
+    if is_pipe:
+        raise XGBoostError("Pipe mode for RecordIO-Protobuf is no longer supported. Please use Fast File mode (default) instead. "
+                           "Set input_mode='File' in your SageMaker Estimator or TrainingInput.")
+    from .recordio import recordio_protobuf_to_dmatrix as to_dmatrix
+    if os.path.isfile(files_path):
+        paths = [files_path]
+    else:
+        paths = [os.path.join(files_path, f) for f in sorted(os.listdir(files_path)) if _is_data_file(files_path, f)]
+    if not paths:
+        return None
+    sizes = [os.path.getsize(p) for p in paths]
+    buf = bytearray(sum(sizes))
+    view, at = memoryview(buf), 0
+    for p, size in zip(paths, sizes):
+        with open(p, "rb") as fh:
+            got = fh.readinto(view[at:at + size])
+        if got != size:
+            raise XGBoostError("%s changed size while it was read" % p)
+        at += size
+    return to_dmatrix(buf)
+
+
 def parquet_to_dmatrix(files_path):
     """Parquet channel -> DMatrix, column 0 = label (what data_utils._get_parquet_dmatrix_file_mode builds, data_utils.py:368-390)
     without its host copies (Table -> DataFrame -> ndarray -> data[:, 1:]): the arrow column buffers go to the device as they are

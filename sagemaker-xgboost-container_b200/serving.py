@@ -119,6 +119,13 @@ def libsvm_to_dmatrix(string_like):
     return DMatrix(data)
 
 
+def recordio_protobuf_to_dmatrix(string_like):
+    """encoder.recordio_protobuf_to_dmatrix (encoder.py:90-99): a recordio-protobuf request body (bytes-like) -> DMatrix,
+    decoded on the device (csrc/recordio.cu); bodies the device path hands back take the package's host walker."""
+    from .recordio import recordio_protobuf_to_dmatrix as to_dmatrix
+    return to_dmatrix(string_like)
+
+
 def _predict_one(booster, dtest):
     best_iteration = getattr(booster, "best_ntree_limit", 0)          # serve_utils.py:228-250
     try:
@@ -141,4 +148,4 @@ def predict(model, model_format, dtest, input_content_type, objective=None):
     return _predict_one(model, dtest)
 
 
-__all__ = ["csv_to_dmatrix", "sparse_libsvm_to_dmatrix", "libsvm_to_dmatrix", "predict", "Booster", "DMatrix", "XGBoostError"]
+__all__ = ["csv_to_dmatrix", "sparse_libsvm_to_dmatrix", "libsvm_to_dmatrix", "recordio_protobuf_to_dmatrix", "predict", "Booster", "DMatrix", "XGBoostError"]
