@@ -188,6 +188,7 @@ XGB_DLL int XGB200SegmentedQuantile(const float* values, const int32_t* segments
 XGB_DLL int XGB200GradientBasedSample(const float* gpair, bst_ulong n, float subsample, unsigned seed, uint64_t stream,
                                       float* out_threshold, float* out_gpair);
 /* flat tree arrays of the model; any pointer may be NULL. tree_offset has num_trees+1 entries. */
+/* num_class: the outputs per row (the class count of multi:*, len(quantile_alpha) of reg:quantileerror, else 1) */
 XGB_DLL int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulong* num_nodes, float* base_score, int* num_class);
 XGB_DLL int XGB200BoosterExportModel(BoosterHandle handle, int64_t* tree_offset, int32_t* tree_info, int32_t* left, int32_t* right,
                              int32_t* parent, int32_t* split_index, int32_t* split_bin, uint8_t* default_left,
@@ -221,7 +222,7 @@ XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dma
  * {"kernel": "predict_tiled_kernel" | "predict_kernel", "reason" (why thread-per-row), "has_nan", "tree_begin", "tree_end",
  * "pitch", "chunks": [{"begin","end","node_bytes","rows","threads","smem"}]} (see csrc/predict_plan.h) */
 XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_begin, int iter_end, const char** out_json);
-/* raw margins of the prediction cache the trainer keeps for `dmat` (n x num_class), brought up to date first */
+/* raw margins of the prediction cache the trainer keeps for `dmat` (n x outputs per row), brought up to date first */
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
 XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
@@ -229,8 +230,8 @@ XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, fl
  * trees as they were before the update (trees one after another), 2 int64 per node; the nodes of layers not yet updated are 0.
  * len = 0 before the first update round.  out may be NULL to query len. */
 XGB_DLL int XGB200BoosterGetRefreshSums(BoosterHandle handle, bst_ulong* len, long long* out);
-/* the configured objective's gradient pairs on `dmat` at the given margins (n x num_class, host), with the row sample of boosting
- * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x num_class x 2 floats (g, h).  Under
+/* the configured objective's gradient pairs on `dmat` at the given margins (n x outputs per row, host), with the row sample of boosting
+ * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x outputs x 2 floats (g, h).  Under
  * sampling_method=gradient_based that sample is the one tree 0 of each class takes: each class's own threshold over these
  * pairs, the draws of the round's uniform sample, kept rows scaled by 1 / p (XGB200GradientBasedSample). */
 XGB_DLL int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair);

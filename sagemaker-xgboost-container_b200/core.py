@@ -226,6 +226,8 @@ def _param_items(params):
         items = list(params)
     out = []
     for k, v in items:
+        if isinstance(v, np.ndarray):          # e.g. quantile_alpha=np.array([0.1, 0.5, 0.9]): forwarded as the list would be
+            v = v.tolist() if v.ndim else v.item()
         if k == "eval_metric" and isinstance(v, (list, tuple)):
             out.extend(("eval_metric", m) for m in v)
         elif isinstance(v, (list, tuple)):

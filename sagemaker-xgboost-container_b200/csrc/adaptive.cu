@@ -1,6 +1,8 @@
-// adaptive.cu -- reg:absoluteerror (adaptive.h): the gradient pass, and the leaf refresh after each tree's structure is final:
-// every leaf's value becomes fl(q * lr), q the 0.5-quantile of the residuals of the leaf's rows [UPSTREAM-RECALL:
-// src/objective/regression_obj.cu MeanAbsoluteError, src/objective/adaptive.{h,cc,cu}, src/common/stats.h].
+// adaptive.cu -- reg:absoluteerror and reg:quantileerror (adaptive.h): their gradient passes, the quantile metric, and the leaf
+// refresh after each tree's structure is final: every leaf's value becomes fl(q * lr), q the alpha-quantile (0.5 for absolute
+// error, the tree's target's quantile_alpha entry for quantile error) of the residuals of the leaf's rows [UPSTREAM-RECALL:
+// src/objective/regression_obj.cu MeanAbsoluteError, src/objective/quantile_obj.cu, src/objective/adaptive.{h,cc,cu},
+// src/common/stats.h].
 // q is found by an exact radix select over order-preserving uint32 keys of the residuals, kSelectDigitBits per pass: each pass
 // builds per-segment digit histograms of row counts and h_q (exact int64, all-reduced across ranks), and a pick kernel narrows
 // each segment to one digit.  Nothing depends on row order, timing or the number of ranks (DESIGN.md §3).
@@ -42,6 +44,61 @@ __global__ void __launch_bounds__(256) abserr_gradient_kernel(AbsErrGradArgs a) 
 }
 void launch_abserr_gradient(const AbsErrGradArgs& a, cudaStream_t s) {
   abserr_gradient_kernel<<<grid_for(a.n), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+
+// ---------------------------------------------------------------------------------------------
+// gradient of reg:quantileerror: per target j, d = m - y, g = (d >= 0 ? 1 - alpha_j : -alpha_j) * w, h = w; r = fl(y - m)
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) quantile_gradient_kernel(QuantileGradArgs a) {
+  __shared__ float sg[8], sh[8];
+  for (int j = 0; j < a.Q; ++j) {          // target by target: each folds its own max|g| and max h
+    const float alpha = a.alpha[j];
+    float mg = 0.f, mh = 0.f;
+    for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < a.n; r += (int64_t)gridDim.x * blockDim.x) {
+      const float y = a.label[r], w = a.weight ? a.weight[r] : 1.0f, m = a.margin ? a.margin[r * a.Q + j] : 0.f;
+      const float diff = __fsub_rn(m, y);
+      float g = diff >= 0.f ? __fmul_rn(__fsub_rn(1.0f, alpha), w) : __fmul_rn(-alpha, w), h = w;
+      if (a.subsample < 1.0f && !(rng_uniform(a.seed, 0x2000ull + a.iter, (unsigned long long)(r + a.row_offset)) < a.subsample)) { g = 0.f; h = 0.f; }
+      if (a.resid) a.resid[j * a.n + r] = __fsub_rn(y, m);
+      if (a.dense_g) reinterpret_cast<float*>(a.gpair)[r] = g; else a.gpair[j * a.gp_stride + r] = make_float2(g, h);
+      mg = fmaxf(mg, fabsf(g)); mh = fmaxf(mh, h);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { mg = fmaxf(mg, __shfl_xor_sync(0xffffffffu, mg, o)); mh = fmaxf(mh, __shfl_xor_sync(0xffffffffu, mh, o)); }
+    if ((threadIdx.x & 31) == 0) { sg[threadIdx.x >> 5] = mg; sh[threadIdx.x >> 5] = mh; }
+    __syncthreads();
+    if (threadIdx.x == 0 && a.absmax) {
+      for (int w = 1; w < 8; ++w) { mg = fmaxf(mg, sg[w]); mh = fmaxf(mh, sh[w]); }
+      unsigned* am = a.absmax + (a.per_target ? 2 * j : 0);
+      atomicMax(am, __float_as_uint(mg)); atomicMax(am + 1, __float_as_uint(mh));
+    }
+    __syncthreads();
+  }
+}
+void launch_quantile_gradient(const QuantileGradArgs& a, cudaStream_t s) {
+  B200_CHECK(!a.dense_g || a.Q == 1, "quantile gradient: the dense g layout holds one target");
+  quantile_gradient_kernel<<<grid_for(a.n), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+
+__global__ void __launch_bounds__(256) quantile_metric_kernel(const float* margin, const float* label, const float* weight, const float* alpha,
+                                                              int Q, int64_t n, double* out) {
+  double s = 0, ws = 0;
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    const float y = label[r], w = weight ? weight[r] : 1.0f;
+    for (int j = 0; j < Q; ++j) {
+      const float d = __fsub_rn(y, margin[r * Q + j]), al = alpha[j];
+      const float loss = d >= 0.f ? __fmul_rn(al, d) : __fmul_rn(__fsub_rn(al, 1.0f), d);
+      s += (double)__fmul_rn(loss, w); ws += (double)w;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); ws += __shfl_xor_sync(0xffffffffu, ws, o); }
+  if ((threadIdx.x & 31) == 0) { atomicAdd(out, s); atomicAdd(out + 1, ws); }
+}
+void launch_quantile_metric(const float* margin, const float* label, const float* weight, const float* alpha, int Q, int64_t n, double* out,
+                            cudaStream_t s) {
+  if (n == 0) return;
+  quantile_metric_kernel<<<grid_for(n), 256, 0, s>>>(margin, label, weight, alpha, Q, n, out); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -181,11 +238,11 @@ void segmented_select(const SelectArgs& a, SelectScratch* sc, const std::functio
   select_finish_kernel<<<sgrid, 256, 0, s>>>(a, sc->st.p, sc->inv_min.p, sc->q.p); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 
-bool SelectScratch::ensure(int64_t n, int nseg_, int cap_nodes) {
+bool SelectScratch::ensure(int64_t n, int nseg_, int cap_nodes, int targets) {
   // every buffer a captured tree reads: a graph bakes in their addresses
   const void* before[9] = {hist.p, st.p, inv_min.p, q.p, leaf_nid.p, seg.p, resid.p, leaf_of_node.p, scales.p};
   hist.ensure((size_t)2 * nseg_ * kSelectBuckets); st.ensure(nseg_); inv_min.ensure(nseg_); q.ensure(nseg_); leaf_nid.ensure(nseg_);
-  seg.ensure((size_t)std::max<int64_t>(n, 1)); resid.ensure((size_t)std::max<int64_t>(n, 1)); leaf_of_node.ensure((size_t)std::max(cap_nodes, 1));
+  seg.ensure((size_t)std::max<int64_t>(n, 1)); resid.ensure((size_t)std::max<int64_t>(n, 1) * std::max(targets, 1)); leaf_of_node.ensure((size_t)std::max(cap_nodes, 1));
   absmax.ensure(2); scales.ensure(4);
   nseg = std::max(nseg, nseg_);
   const void* after[9] = {hist.p, st.p, inv_min.p, q.p, leaf_nid.p, seg.p, resid.p, leaf_of_node.p, scales.p};

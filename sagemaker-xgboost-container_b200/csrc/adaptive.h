@@ -1,4 +1,4 @@
-// adaptive.h -- reg:absoluteerror: its gradient pass and the per-leaf quantile refresh of every tree ("adaptive tree",
+// adaptive.h -- reg:absoluteerror and reg:quantileerror: their gradient passes and the per-leaf quantile refresh of every tree ("adaptive tree",
 // upstream src/objective/adaptive.{h,cc,cu} [UPSTREAM-RECALL]), an exact segmented radix select (adaptive.cu, DESIGN.md §3).
 #pragma once
 #include <functional>
@@ -17,6 +17,26 @@ struct AbsErrGradArgs {
 };
 void launch_abserr_gradient(const AbsErrGradArgs& a, cudaStream_t s);
 
+// Gradient pairs of reg:quantileerror for Q targets from one label column: target j of row i gets, with d = fl(m[i][j] - y[i]),
+// ((1 - alpha_j) w, w) when d >= 0 and (-alpha_j w, w) otherwise [UPSTREAM-RECALL: src/objective/quantile_obj.cu], all in
+// float, into gpair[j * gp_stride + i]; margin is [n][Q] row-major, alpha Q floats on the device.  Rows outside the sample
+// (the draw of AbsErrGradArgs, one per row for every target) get (0, 0); resid (may be nullptr) gets fl(y - m[i][j]) at
+// [j * n + i] for every row.  dense_g (Q == 1 only): g alone as float[n].  absmax (may be nullptr): max|g| and max h of every
+// target folded into [0] and [1], or with per_target those of target j into [2 j] and [2 j + 1] (2 Q entries), so that each
+// target's trees can grow on a fixed-point grid of their own.
+struct QuantileGradArgs {
+  const float* margin; const float* label; const float* weight; const float* alpha;   // weight nullptr = 1
+  float2* gpair; float* resid; unsigned* absmax;
+  int64_t n, row_offset, gp_stride;
+  float subsample; unsigned seed; unsigned long long iter; int dense_g, Q, per_target;
+};
+void launch_quantile_gradient(const QuantileGradArgs& a, cudaStream_t s);
+
+// The quantile metric's sums: out[0] += sum_i sum_j fl(w_i * pinball_j(fl(y_i - m[i][j]))), out[1] += Q * sum_i w_i, in double
+// (pinball_j(d) = fl(alpha_j d) for d >= 0, else fl(fl(alpha_j - 1) d)) [UPSTREAM-RECALL: src/metric/elementwise_metric.cu QuantileError]
+void launch_quantile_metric(const float* margin, const float* label, const float* weight, const float* alpha, int Q, int64_t n, double* out,
+                            cudaStream_t s);
+
 // Selection state of one segment (a leaf).  mode 0: no rows; 1: the row of 0-based rank `target` in key order; 2: the first row
 // in key order whose cumulative h_q reaches `target`.  d: upstream Quantile's interpolation weight, < 0 when the rank is clamped
 // to an end (the value alone).  need_v1: the next larger key is not equal to the selected one and comes from the min pass.
@@ -31,10 +51,10 @@ struct SelectScratch {
   DevBuf<SelectSeg> st; DevBuf<unsigned> inv_min; DevBuf<float> q;
   DevBuf<int> seg;                        // per row: its segment, -1 = not selected from
   DevBuf<int> leaf_of_node, leaf_nid;     // training: dense leaf numbering of the tree's nodes
-  DevBuf<float> resid;                    // training: the round's residuals
+  DevBuf<float> resid;                    // training: the round's residuals, [targets][n]
   DevBuf<unsigned> absmax; DevBuf<float> scales;
   int nseg = 0;
-  bool ensure(int64_t n, int nseg, int cap_nodes);      // true when any buffer moved
+  bool ensure(int64_t n, int nseg, int cap_nodes, int targets = 1);      // true when any buffer moved
 };
 
 // The selection proper.  values: per-row floats (-0.0 counts as +0.0, every NaN as one value above +inf); seg: per-row

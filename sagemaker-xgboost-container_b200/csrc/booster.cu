@@ -285,7 +285,8 @@ static const std::map<std::string, int>& objective_table() {
   static const std::map<std::string, int> t = {{"reg:squarederror", kSquaredError}, {"reg:linear", kSquaredError}, {"binary:logistic", kBinaryLogistic},
     {"reg:logistic", kRegLogistic}, {"binary:logitraw", kLogitRaw}, {"multi:softprob", kSoftprob}, {"multi:softmax", kSoftmax},
     {"reg:squaredlogerror", kSquaredLogError}, {"reg:pseudohubererror", kPseudoHuber}, {"count:poisson", kPoisson}, {"reg:gamma", kGamma},
-    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}, {"reg:absoluteerror", kAbsoluteError}};
+    {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}, {"reg:absoluteerror", kAbsoluteError},
+    {"reg:quantileerror", kQuantileError}};
   return t;
 }
 
@@ -293,6 +294,27 @@ void Booster::set_param(const std::string& k, const std::string& v) {
   if (k == "eval_metric") { if (std::find(eval_metrics_.begin(), eval_metrics_.end(), v) == eval_metrics_.end()) eval_metrics_.push_back(v); }
   else raw_params_[k] = v;
   configured_ = false;
+}
+
+// quantile_alpha: "0.5", the "(0.1,0.5,0.9)" of a Python list or tuple, or the "[0.1, 0.5, 0.9]" of a saved config; at least one
+// value, each in [0, 1] [UPSTREAM-RECALL: QuantileLossParam::Validate]
+std::vector<float> parse_quantile_alpha(const std::string& v) {
+  std::vector<float> out; std::string tok;
+  auto flush = [&]() {
+    if (tok.empty()) return;
+    size_t used = 0; float a = 0.0f;
+    try { a = std::stof(tok, &used); } catch (...) { used = 0; }
+    B200_CHECK(used > 0 && used == tok.size(), "Invalid value for parameter quantile_alpha: " + v);
+    B200_CHECK(a >= 0.0f && a <= 1.0f, "quantile_alpha must be in [0, 1] (got " + tok + ")");
+    out.push_back(a); tok.clear();
+  };
+  for (char ch : v) {
+    if (ch == ',' || ch == '(' || ch == ')' || ch == '[' || ch == ']' || std::isspace((unsigned char)ch)) flush();
+    else tok.push_back(ch);
+  }
+  flush();
+  B200_CHECK(!out.empty(), "quantile_alpha must not be empty (got \"" + v + "\")");
+  return out;
 }
 
 void Booster::configure() {
@@ -305,7 +327,7 @@ void Booster::configure() {
   auto ito = raw_params_.find("objective");
   if (ito != raw_params_.end()) objective_name_ = ito->second;
   auto ot = objective_table().find(objective_name_);
-  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:absoluteerror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
+  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:absoluteerror, reg:quantileerror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
   p.objective = ot->second;
   if (objective_name_ == "reg:linear") objective_name_ = "reg:squarederror";
   p.num_class = (p.objective == kSoftprob || p.objective == kSoftmax) ? geti("num_class", 0) : 1;
@@ -323,6 +345,11 @@ void Booster::configure() {
     while (used > 0 && used < it->second.size() && std::isspace((unsigned char)it->second[used])) ++used;
     B200_CHECK(used > 0 && used == it->second.size() && v == std::floor(v) && v >= 1.0 && v <= (double)(1 << 20), "num_parallel_tree must be an integer in [1, 1048576] (got " + it->second + ")");
     p.num_parallel_tree = (int)v;
+  }
+  if (p.objective == kQuantileError) {       // quantile_alpha is read (and checked) only under reg:quantileerror
+    auto qa = raw_params_.find("quantile_alpha");
+    B200_CHECK(qa != raw_params_.end(), "reg:quantileerror needs the parameter quantile_alpha (a value or a list of values in [0, 1])");
+    p.quantile_alpha = parse_quantile_alpha(qa->second);
   }
   p.huber_slope = getf("huber_slope", nullptr, 1.0f); p.tweedie_variance_power = getf("tweedie_variance_power", nullptr, 1.5f);
   B200_CHECK(p.huber_slope != 0.0f, "Check failed: slope != 0.0 (huber_slope)");
@@ -482,6 +509,34 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
     base_score_ = std::isnan(med) ? 0.0f : med;
     return;
   }
+  if (param_.objective == kQuantileError) {
+    // the mean of the labels' alpha_j-quantiles over every rank's rows (weighted when there are weights), times sw / (sw + 1e-6)
+    // with sw the weight sum (the row count without weights), in double [UPSTREAM-RECALL: QuantileRegression::InitEstimation
+    // averages the per-alpha quantiles into one scalar; upstream takes each worker's own quantiles]
+    b.ensure_adaptive(param_.num_outputs());
+    double meanq = 0.0;
+    for (float alpha : param_.quantile_alpha) {
+      float q = 0.0f;
+      segmented_quantile(dtrain->d_labels.p, nullptr, dtrain->weights.empty() ? nullptr : dtrain->d_weights.p, dtrain->n, b.global_n, 1, (double)alpha,
+                         &q, &b.adapt, s);
+      meanq += std::isnan(q) ? 0.0 : (double)q;
+    }
+    meanq /= (double)param_.quantile_alpha.size();
+    double sw = 0.0;
+    if (dtrain->weights.empty()) sw = (double)b.global_n;
+    else {
+      for (float w : dtrain->weights) sw += (double)w;
+      if (Comm::get().distributed()) {
+        dsum_.ensure(4);
+        CUDA_OK(cudaMemcpyAsync(dsum_.p, &sw, sizeof sw, cudaMemcpyHostToDevice, s));
+        Comm::get().allreduce_sum_f64(dsum_.p, 1, s);
+        CUDA_OK(cudaMemcpyAsync(&sw, dsum_.p, sizeof sw, cudaMemcpyDeviceToHost, s));
+        Comm::get().sync_stream(s);
+      }
+    }
+    base_score_ = (float)(meanq * sw / (sw + 1e-6));
+    return;
+  }
   GradArgs ga{}; ga.margin = nullptr; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
   ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = nullptr; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = 1; ga.objective = param_.objective;
   ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = 1.0f; ga.seed = 0; ga.iter = 0; ga.aux = objective_aux(param_);
@@ -565,7 +620,7 @@ void Booster::upload_model() {
 
 PredCache& Booster::cache_for(DMatrix* dm) {
   PredCache& c = caches_[dm->uid];
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   if (c.n != dm->n || c.margin.n != (size_t)dm->n * K) {
     c.n = dm->n; c.margin.alloc((size_t)dm->n * K); c.trees_applied = -1;
   }
@@ -574,7 +629,7 @@ PredCache& Booster::cache_for(DMatrix* dm) {
 
 void Booster::bring_cache_up_to_date(DMatrix* dm, PredCache& c) {
   cudaStream_t s = engine_stream();
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const int nt = (int)trees_.size();
   if (c.trees_applied < 0) {
     if (!dm->base_margin.empty()) {
@@ -637,7 +692,7 @@ std::vector<int> Booster::dart_drop_set(int round) const {
 // the margin the round's gradients read (the cache itself when nothing is dropped).  The new trees' weight goes to the builder.
 float* Booster::dart_begin_round(DMatrix* dtrain, PredCache& c, int round) {
   const std::vector<int> D = dart_drop_set(round);
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const float lr = (float)((double)param_.eta / (double)K);
   float factor = 1.0f; dart_new_weight_ = 1.0f;
   if (!D.empty()) {
@@ -667,7 +722,7 @@ void Booster::dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::v
   CUDA_OK(cudaMemcpyAsync(dart_coef_.p, coef_full.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
   if (m_drop) CUDA_OK(cudaMemcpyAsync(dart_coef_.p + m, coef_drop.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
   DartArgs a{}; a.X = dm->X.p; a.n = dm->n; a.F = dm->F; a.nodes = d_nodes.p; a.tree_offset = d_tree_offset.p; a.tree_info = d_tree_info.p;
-  a.trees = dart_ids_.p; a.ntrees = (int)m; a.K = param_.num_class; a.coef_full = dart_coef_.p; a.coef_drop = dart_coef_.p + m;
+  a.trees = dart_ids_.p; a.ntrees = (int)m; a.K = param_.num_outputs(); a.coef_full = dart_coef_.p; a.coef_drop = dart_coef_.p + m;
   a.m_full = m_full; a.m_drop = m_drop;
   launch_dart_margin(a, s);
   Comm::get().sync_stream(s);            // the host vectors and the list buffers are reused by the next call
@@ -702,6 +757,7 @@ void Booster::check_label_ranges(const DMatrix* dtrain) {
     if (param_.objective == kGamma) for (float v : y) B200_CHECK(v > 0.0f, "GammaRegression: label must be positive.");
     if (param_.objective == kTweedie) for (float v : y) B200_CHECK(v >= 0.0f, "TweedieRegression: label must be nonnegative");
     if (param_.objective == kAbsoluteError) for (float v : y) B200_CHECK(!std::isnan(v), "reg:absoluteerror: label must not be NaN");
+    if (param_.objective == kQuantileError) for (float v : y) B200_CHECK(!std::isnan(v), "reg:quantileerror: label must not be NaN");
     if (param_.objective == kAft)
       for (int64_t i = 0; i < dtrain->n; ++i) {
         const float lo = dtrain->label_lower[i], hi = dtrain->label_upper[i];
@@ -725,7 +781,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   if (update_mode_) { refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
   check_train_width(dtrain);
   dtrain->ensure_binned(param_.max_bin);
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   TreeBuilder& b = builder_for(dtrain);
   check_label_ranges(dtrain);
   estimate_base_score(dtrain);
@@ -752,8 +808,11 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   // likewise constant-hessian growth never meets a gradient-based sample, whose kept rows have h / p != 1
   B200_CHECK(!(dense_g && gbs), "gradient-based sampling of a constant-hessian round");
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
-  // reg:absoluteerror: the round's residuals, read by the leaf refresh of every tree of the round
-  float* resid = objective_is_adaptive(param_.objective) ? b.ensure_adaptive() : nullptr;
+  // reg:quantileerror without a per-tree or gradient-based sample: each target's trees grow on the grid of its own gradients
+  // (upstream quantises each tree's gradients by themselves), so a target's trees do not depend on the other targets
+  const bool per_target_grid = param_.objective == kQuantileError && !per_tree_sample && !gbs;
+  // reg:absoluteerror / reg:quantileerror: the round's residuals of every output, read by the leaf refresh of every tree of the round
+  float* resid = objective_is_adaptive(param_.objective) ? b.ensure_adaptive(K) : nullptr;
   if (per_tree_sample) {
     forest_gpair_.ensure((size_t)b.gp_stride * K);
     launch_objective(dtrain, grad_margin, round, forest_gpair_.p, b.gp_stride, nullptr, 1.0f, false, resid);
@@ -762,10 +821,15 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
     launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, nullptr, 1.0f, false, resid);
     gradient_based_threshold(b.gpair.p, b.gp_stride, dtrain->n, K, param_.subsample, &gbs_, s);
     gradient_based_sample(b.gpair.p, b.gpair.p, b.gp_stride, dtrain->n, round, 0, b.gs.absmax);
+  } else if (per_target_grid) {
+    target_absmax_.ensure(2 * (size_t)K);
+    CUDA_OK(cudaMemsetAsync(target_absmax_.p, 0, 2 * sizeof(unsigned) * K, s));
+    launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, target_absmax_.p, param_.subsample, dense_g, resid, true);
   } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g, resid);
-  // weighted reg:absoluteerror under gradient-based sampling: the refresh weighs its rows by their instance weight (h is w / p)
+  // weighted adaptive objectives under gradient-based sampling: the refresh weighs its rows by their instance weight (h is w / p)
   if (gbs && resid && !dtrain->weights.empty()) weight_grid(dtrain->d_weights.p, dtrain->n, b.global_n, &b.adapt, s);
-  if (!per_tree_sample) {
+  if (per_target_grid) Comm::get().allreduce_max_u32(target_absmax_.p, 2 * (size_t)K, s);
+  else if (!per_tree_sample) {
     Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
     launch_scales(b.gs, grad_bits_for(b.global_n), s);
   }
@@ -784,24 +848,39 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
         }
         Comm::get().allreduce_max_u32(b.gs.absmax, 2, s);
         launch_scales(b.gs, grad_bits_for(b.global_n), s);
+      } else if (per_target_grid && j == 0) {
+        CUDA_OK(cudaMemcpyAsync(b.gs.absmax, target_absmax_.p + 2 * k, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
+        launch_scales(b.gs, grad_bits_for(b.global_n), s);
       }
       grow_one_tree(dtrain, cache, k, iteration_indptr_[round] + k * P + j);
     }
   iteration_indptr_.push_back((int)trees_.size());
 }
 
+// quantile_alpha on the device, uploaded when it differs from what the buffer holds
+const float* Booster::upload_quantile_alpha(const std::vector<float>& alpha) {
+  if (alpha != quantile_alpha_host_ || !quantile_alpha_dev_.p) {
+    cudaStream_t s = engine_stream();
+    quantile_alpha_dev_.alloc(std::max<size_t>(alpha.size(), 1));
+    if (!alpha.empty()) CUDA_OK(cudaMemcpyAsync(quantile_alpha_dev_.p, alpha.data(), sizeof(float) * alpha.size(), cudaMemcpyHostToDevice, s));
+    Comm::get().sync_stream(s);
+    quantile_alpha_host_ = alpha;
+  }
+  return quantile_alpha_dev_.p;
+}
+
 void Booster::gradient_based_sample(const float2* src, float2* dst, int64_t gp_stride, int64_t n, int round, int j, unsigned* absmax) {
   GbsSampleArgs a{}; a.src = src; a.dst = dst; a.absmax = absmax; a.st = gbs_.st.p; a.gp_stride = gp_stride; a.n = n;
-  a.row_offset = (int64_t)Comm::get().rank() << 40; a.K = param_.num_class; a.seed = param_.seed; a.stream = row_stream(round, j);
+  a.row_offset = (int64_t)Comm::get().rank() << 40; a.K = param_.num_outputs(); a.seed = param_.seed; a.stream = row_stream(round, j);
   launch_gradient_based_sample(a, engine_stream());
 }
 
 // The objective's gradient pairs at `margin` into gpair ([K][gp_stride]), rows outside round `round`'s sample zeroed, max|g| and
 // max h folded into absmax (nullptr: not taken).  dense_g (constant_hessian only): g alone, as float[gp_stride].  The survival
-// objectives have their own kernels (survival.cu), reg:absoluteerror its own (adaptive.cu), which also writes the residuals
-// fl(y - m) into resid (nullptr: not written); every other objective runs gradient_kernel.
+// objectives have their own kernels (survival.cu), reg:absoluteerror and reg:quantileerror theirs (adaptive.cu), which also write
+// the residuals fl(y - m) into resid ([K][n]; nullptr: not written); every other objective runs gradient_kernel.
 void Booster::launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample,
-                               bool dense_g, float* resid) {
+                               bool dense_g, float* resid, bool per_target_absmax) {
   cudaStream_t s = engine_stream();
   const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
   if (param_.objective == kAbsoluteError) {
@@ -809,6 +888,14 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
     aa.gpair = gpair; aa.resid = resid; aa.absmax = absmax; aa.n = dm->n; aa.row_offset = row_offset; aa.subsample = subsample; aa.seed = param_.seed;
     aa.iter = (unsigned long long)round; aa.dense_g = dense_g ? 1 : 0;
     launch_abserr_gradient(aa, s);
+    return;
+  }
+  if (param_.objective == kQuantileError) {
+    QuantileGradArgs qa{}; qa.margin = margin; qa.label = dm->d_labels.p; qa.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
+    qa.alpha = quantile_alpha_device(); qa.gpair = gpair; qa.resid = resid; qa.absmax = absmax; qa.n = dm->n; qa.row_offset = row_offset;
+    qa.gp_stride = gp_stride; qa.subsample = subsample; qa.seed = param_.seed; qa.iter = (unsigned long long)round; qa.dense_g = dense_g ? 1 : 0;
+    qa.Q = param_.num_outputs(); qa.per_target = per_target_absmax ? 1 : 0;
+    launch_quantile_gradient(qa, s);
     return;
   }
   if (objective_is_survival(param_.objective)) {
@@ -833,7 +920,7 @@ void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float*
   cudaStream_t s = engine_stream();
   if (param_.objective == kAft) check_aft_bounds(dm); else check_labels(dm);
   dm->ensure_binned(param_.max_bin); builder_for(dm);        // the builder owns the label-error flag gradient_kernel writes
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const int64_t n = dm->n;
   DevBuf<float> d_margin; DevBuf<float2> d_gp; d_margin.alloc((size_t)n * K); d_gp.alloc((size_t)n * K);
   if (n) CUDA_OK(cudaMemcpyAsync(d_margin.p, margin, sizeof(float) * n * K, cudaMemcpyHostToDevice, s));
@@ -864,7 +951,7 @@ static TrainParamDev to_dev(const TrainParam& p) {
 }
 
 TreeBuilder& Booster::builder_for(DMatrix* dm) {
-  builder_->ensure(dm->binned_view(), param_.max_depth, param_.num_class, lossguide_iters(param_), (int)interaction_.size());
+  builder_->ensure(dm->binned_view(), param_.max_depth, param_.num_outputs(), lossguide_iters(param_), (int)interaction_.size());
   return *builder_;
 }
 
@@ -872,7 +959,8 @@ TreeBuilder& Booster::builder_for(DMatrix* dm) {
 // (launch_objective) and the tree reads them so (root_mode != 0); this one predicate decides both.  B200XGB_NO_CONSTH turns it off.
 bool Booster::constant_hessian(const DMatrix& dm) const {
   static const bool no_consth = getenv("B200XGB_NO_CONSTH") != nullptr;
-  return !no_consth && (param_.objective == kSquaredError || param_.objective == kAbsoluteError) && param_.num_class == 1 && dm.weights.empty() &&
+  return !no_consth && (param_.objective == kSquaredError || param_.objective == kAbsoluteError || param_.objective == kQuantileError) &&
+         param_.num_outputs() == 1 && dm.weights.empty() &&
          param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
 }
 
@@ -882,7 +970,7 @@ TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int 
   TreeBuilder& b = *builder_;
   TreeInputs in{};                 // no padding bytes: every byte is zero before the fields are set
   in.bm = dm.binned_view(); in.cut_ptrs = dm.d_cut_ptrs.p; in.cut_vals = dm.d_cut_vals.p; in.min_vals = dm.d_min_vals.p;
-  in.margin = margin; in.K = param_.num_class; in.k = k;
+  in.margin = margin; in.K = param_.num_outputs(); in.k = k;
   in.p = to_dev(param_); in.colsample_bynode = param_.colsample_bynode; in.seed = param_.seed; in.lg_iters = lossguide_iters(param_);
   in.mask = mask.empty() ? nullptr : b.upload_mask(mask, tree_index);
   in.monotone = b.upload_monotone(monotone_, dm.F);
@@ -890,7 +978,9 @@ TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int 
   in.root_mode = !constant_hessian(dm) ? 0 : b.root_h_valid && b.root_h_uid == dm.uid && b.root_h_version == dm.binned_version ? 2 : 1;
   in.world = Comm::get().world();
   if (objective_is_adaptive(param_.objective)) {
-    in.resid = b.adapt.resid.p; in.adaptive = dm.weights.empty() ? 1 : gradient_based_sampling() ? 3 : 2;
+    // output k's residual column and quantile
+    in.resid = b.adapt.resid.p + (size_t)k * dm.n; in.alpha = param_.objective == kQuantileError ? param_.quantile_alpha[k] : 0.5f;
+    in.adaptive = dm.weights.empty() ? 1 : gradient_based_sampling() ? 3 : 2;
     if (in.adaptive == 3) in.weight = dm.d_weights.p;
   }
   return in;
@@ -994,10 +1084,10 @@ void Booster::refresh_one_iter(DMatrix* dtrain) {
   const int round = layers();
   B200_CHECK(round < u.layers(), "boosting rounds cannot exceed the previous training rounds under process_type=update (the model to update has " +
              std::to_string(u.layers()) + " rounds)");
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const int t0 = u.indptr[round], t1 = u.indptr[round + 1], T = t1 - t0;
   for (int t = t0; t < t1; ++t) B200_CHECK(u.tree_info[t] >= 0 && u.tree_info[t] < K, "process_type=update: tree " + std::to_string(t) + " belongs to class " +
-                                           std::to_string(u.tree_info[t]) + " but num_class is " + std::to_string(K));
+                                           std::to_string(u.tree_info[t]) + " but the model has " + std::to_string(K) + " outputs");
   // the fixed-point grid follows the rows of the whole job, as for growth (TreeBuilder::ensure): N GPUs and one agree
   if (u.global_n_uid != dtrain->uid || u.global_n == 0) {
     u.global_n = dtrain->n;
@@ -1077,6 +1167,7 @@ static std::string default_metric(const TrainParam& p) {
   switch (p.objective) {
     case kSquaredError: case kRegLogistic: return "rmse";
     case kAbsoluteError: return "mae";
+    case kQuantileError: return "quantile";
     case kBinaryLogistic: case kLogitRaw: return "logloss";
     case kSquaredLogError: return "rmsle";
     case kPseudoHuber: return "mphe";
@@ -1112,7 +1203,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
       if (mname.rfind("error@", 0) == 0) { base = "error"; ma.threshold = std::stof(mname.substr(6)); }
       if (base == "auc") {
         // validated on hardware against sklearn.metrics.roc_auc_score (tests/test_gpu_parity.py::test_auc_matches_sklearn)
-        B200_CHECK(param_.num_class <= 1, "auc is implemented for binary / regression-style predictions only");
+        B200_CHECK(param_.num_outputs() <= 1, "auc is implemented for binary / regression-style predictions only");
         const int logistic = (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic) ? 1 : 0;
         compute_auc_device(c.margin.p, dm->d_labels.p, dm->weights.empty() ? nullptr : dm->d_weights.p, dm->n, logistic, dsum_.p, s);
         double h3[3];
@@ -1140,8 +1231,18 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         check_labels(dm);
         if (!dm->cox_order.valid) cox_sort(dm->d_labels.p, dm->n, &dm->cox_order, &cox_scratch_, s);
         cox_nloglik(c.margin.p, dm->n, dm->cox_order, &cox_scratch_, dsum_.p, s);
+      } else if (mname == "quantile") {           // pinball loss of every output at its quantile_alpha entry (adaptive.cu)
+        check_labels(dm);
+        B200_CHECK(!param_.quantile_alpha.empty() || raw_params_.count("quantile_alpha"), "the quantile metric needs the parameter quantile_alpha");
+        const std::vector<float> alpha = param_.objective == kQuantileError ? param_.quantile_alpha : parse_quantile_alpha(raw_params_.at("quantile_alpha"));
+        B200_CHECK((int)alpha.size() == param_.num_outputs(), "the quantile metric: the model has " + std::to_string(param_.num_outputs()) +
+                   " outputs per row but quantile_alpha has " + std::to_string(alpha.size()) + " values");
+        CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
+        launch_quantile_metric(c.margin.p, dm->d_labels.p, ma.weight, upload_quantile_alpha(alpha), (int)alpha.size(), dm->n, dsum_.p, s);
       } else {
         if (param_.objective == kAft) check_labels(dm);
+        B200_CHECK(param_.objective != kQuantileError || param_.num_outputs() == 1, "metric " + mname + " reads one output per row; a reg:quantileerror model with " +
+                   std::to_string(param_.num_outputs()) + " outputs is evaluated with the quantile metric");
         if (base == "rmse") ma.metric = kMetricRmse; else if (base == "mse") ma.metric = kMetricRmse; else if (base == "mae") ma.metric = kMetricMae;
         else if (base == "logloss") ma.metric = kMetricLogloss; else if (base == "error") ma.metric = kMetricError;
         else if (base == "merror") ma.metric = kMetricMerror; else if (base == "mlogloss") ma.metric = kMetricMlogloss;
@@ -1150,7 +1251,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         else if (base == "poisson-nloglik") ma.metric = kMetricPoissonNll; else if (base == "gamma-nloglik") ma.metric = kMetricGammaNll;
         else if (base == "gamma-deviance") ma.metric = kMetricGammaDeviance;
         else if (base == "tweedie-nloglik") { ma.metric = kMetricTweedieNll; if (ma.aux == 0.0f) throw Error("tweedie-nloglik needs its variance power: tweedie-nloglik@rho"); }
-        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik)");
+        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, quantile, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik)");
         if (param_.objective == kLogitRaw && (ma.metric == kMetricLogloss || ma.metric == kMetricError)) ma.is_logistic = 1;
         if ((ma.metric == kMetricMerror || ma.metric == kMetricMlogloss)) B200_CHECK(param_.num_class > 1, "Check failed: preds.size() == info.labels_.size() : label and prediction size not match, hint: use merror or mlogloss for multi-class classification");
         CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
@@ -1179,7 +1280,7 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
   configure();
   (void)training;
   cudaStream_t s = engine_stream();
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const int rounds = layers();
   if (iter_end == 0) iter_end = rounds;
   B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end <= rounds, "Invalid iteration range: [" + std::to_string(iter_begin) + ", " + std::to_string(iter_end) + ") for a model with " + std::to_string(rounds) + " rounds");
@@ -1250,7 +1351,7 @@ std::string Booster::debug_eval_root(DMatrix* dm, const long long* hist_fm, long
 void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* out, std::vector<uint64_t>* shape) {
   cudaStream_t s = engine_stream();
   sync_model();
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   const int64_t n = dm->n;
   const int F = std::max(dm->F, num_feature_);
   B200_CHECK(dm->F == F, "pred_contribs: the data has " + std::to_string(dm->F) + " columns, the model uses " + std::to_string(F));
@@ -1303,7 +1404,7 @@ void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* 
 
 PredictArgs Booster::predict_args(DMatrix* dm, int tree_begin, int tree_end) {
   PredictArgs pa{}; pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
-  pa.tree_begin = tree_begin; pa.tree_end = tree_end; pa.K = param_.num_class; pa.margin = nullptr; pa.leaf = nullptr;
+  pa.tree_begin = tree_begin; pa.tree_end = tree_end; pa.K = param_.num_outputs(); pa.margin = nullptr; pa.leaf = nullptr;
   pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
   pa.model_F = num_feature_;
   return pa;
@@ -1324,7 +1425,7 @@ float Booster::debug_predict_kernel_ms(DMatrix* dm, int repeats) {
   configure();
   cudaStream_t s = engine_stream();
   upload_model();
-  const int K = param_.num_class;
+  const int K = param_.num_outputs();
   pred_margin_.ensure((size_t)dm->n * K);
   PredictArgs pa = predict_args(dm, 0, (int)trees_.size());
   pa.margin = pred_margin_.p;
@@ -1347,7 +1448,7 @@ void Booster::cached_margin(DMatrix* dm, std::vector<float>* out) {
   cudaStream_t s = engine_stream();
   PredCache& c = cache_for(dm);
   bring_cache_up_to_date(dm, c);
-  out->resize((size_t)dm->n * param_.num_class);
+  out->resize((size_t)dm->n * param_.num_outputs());
   if (!out->empty()) CUDA_OK(cudaMemcpyAsync(out->data(), c.margin.p, sizeof(float) * out->size(), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
 }

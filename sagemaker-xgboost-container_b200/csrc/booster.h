@@ -201,6 +201,8 @@ class Booster {
   // process_type=update: the updaters in order (refresh.h RefreshOp), refresh_leaf, and the trees being updated
   bool update_mode_ = false; std::vector<int> update_ops_; std::string update_ops_str_; int refresh_leaf_ = 1;
   std::unique_ptr<UpdateState> update_ = std::make_unique<UpdateState>();
+  DevBuf<float> quantile_alpha_dev_; std::vector<float> quantile_alpha_host_;   // reg:quantileerror / the quantile metric: alpha on the device
+  DevBuf<unsigned> target_absmax_;              // reg:quantileerror: each target's max|g| and max h ([2 Q]), for a grid per target
 
   void configure();
   void check_label_ranges(const DMatrix* dtrain);
@@ -228,7 +230,9 @@ class Booster {
   // tree j of boosting round `round` keeps rows [0, n) of src by the thresholds in gbs_ (launch_gradient_based_sample)
   void gradient_based_sample(const float2* src, float2* dst, int64_t gp_stride, int64_t n, int round, int j, unsigned* absmax);
   void launch_objective(DMatrix* dm, const float* margin, int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool dense_g,
-                        float* resid);
+                        float* resid, bool per_target_absmax = false);
+  const float* upload_quantile_alpha(const std::vector<float>& alpha);       // the device copy of alpha
+  const float* quantile_alpha_device() { return upload_quantile_alpha(param_.quantile_alpha); }
   JPtr model_to_json();
   void model_from_json(const JValue& doc);
   JPtr config_to_json();
@@ -236,6 +240,8 @@ class Booster {
   void reset_model();
 };
 
+// quantile_alpha in any of its accepted forms (booster.cu); raises on a malformed, empty or out-of-range value
+std::vector<float> parse_quantile_alpha(const std::string& v);
 std::string colsample_mask(unsigned seed, int tree_index, int F, float frac);   // bytes, 1 = feature usable
 std::string subset_mask(const std::string& parent, float frac, unsigned seed, uint64_t stream);
 

@@ -484,7 +484,7 @@ int XGB200BoosterModelShape(BoosterHandle handle, bst_ulong* num_trees, bst_ulon
   Booster* b = BST(handle); const auto& trees = b->trees();
   size_t nn = 0; for (auto& t : trees) nn += t.left.size();
   if (num_trees) *num_trees = trees.size(); if (num_nodes) *num_nodes = nn; if (base_score) *base_score = b->base_score();
-  if (num_class) *num_class = b->param().num_class;
+  if (num_class) *num_class = b->param().num_outputs();          // classes, or the outputs of a reg:quantileerror model
   API_END();
 }
 int XGB200BoosterExportModel(BoosterHandle handle, int64_t* tree_offset, int32_t* tree_info, int32_t* left, int32_t* right, int32_t* parent,

@@ -95,7 +95,8 @@ inline size_t hist_slot_entries(int ngroups, int tw) { return (size_t)ngroups * 
 enum Objective : int { kSquaredError = 0, kBinaryLogistic = 1, kRegLogistic = 2, kLogitRaw = 3, kSoftprob = 4, kSoftmax = 5,
                        kSquaredLogError = 6, kPseudoHuber = 7, kPoisson = 8, kGamma = 9, kTweedie = 10, kHinge = 11,
                        kAft = 12, kCox = 13,         // survival objectives: own gradient kernels (survival.cu), not gradient_kernel
-                       kAbsoluteError = 14 };        // own gradient kernel and a leaf refresh after every tree (adaptive.cu)
+                       kAbsoluteError = 14,          // own gradient kernel and a leaf refresh after every tree (adaptive.cu)
+                       kQuantileError = 15 };        // likewise, one output (and one tree per round) per quantile_alpha
 // prediction transform of an objective (upstream ObjFunction::PredTransform / ProbToMargin): 0 identity, 1 sigmoid / logit,
 // 2 exp / log (count:poisson, reg:gamma, reg:tweedie, survival:aft, survival:cox), 3 step at 0 (binary:hinge; its margin is the raw score)
 enum Transform : int { kTransformNone = 0, kTransformSigmoid = 1, kTransformExp = 2, kTransformHinge = 3 };
@@ -103,7 +104,7 @@ inline bool objective_is_logistic(int o) { return o == kBinaryLogistic || o == k
 inline bool objective_is_log_link(int o) { return o == kPoisson || o == kGamma || o == kTweedie; }
 inline bool objective_is_survival(int o) { return o == kAft || o == kCox; }
 // the objective sets each leaf of a grown tree to a quantile of its rows' residuals (upstream ObjFunction::Task().UpdateTreeLeaf())
-inline bool objective_is_adaptive(int o) { return o == kAbsoluteError; }
+inline bool objective_is_adaptive(int o) { return o == kAbsoluteError || o == kQuantileError; }
 inline int objective_transform(int o) {
   if (o == kBinaryLogistic || o == kRegLogistic) return kTransformSigmoid;
   if (objective_is_log_link(o) || objective_is_survival(o)) return kTransformExp;
@@ -122,6 +123,10 @@ struct TrainParam {
   int gradient_based = 0;       // sampling_method: 0 uniform, 1 gradient_based (sampling.h; only with subsample < 1)
   float huber_slope = 1.0f, tweedie_variance_power = 1.5f, poisson_max_delta_step = 0.7f;   // objective parameters (upstream defaults)
   int aft_dist = 0; float aft_sigma = 1.0f;     // survival:aft: aft_loss_distribution (survival.h AftDist), aft_loss_distribution_scale
+  std::vector<float> quantile_alpha;            // reg:quantileerror: one output per entry (empty for every other objective)
+  // Outputs per row: margin columns, trees per round and layer (times num_parallel_tree), prediction columns.  num_class
+  // itself is the class count of multi:* (softmax, merror / mlogloss) and 1 otherwise.
+  int num_outputs() const { return objective == kQuantileError ? (int)quantile_alpha.size() : num_class; }
 };
 
 // ---------------------------------------------------------------------------------------------

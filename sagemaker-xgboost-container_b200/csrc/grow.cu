@@ -120,8 +120,8 @@ void TreeBuilder::ensure(const BinnedMatrix& bm, int max_depth_, int K, int lg_i
   }
 }
 
-float* TreeBuilder::ensure_adaptive() {
-  if (adapt.ensure(n, max_leaves(), cap_nodes)) for (auto& tg : graphs) tg.destroy();
+float* TreeBuilder::ensure_adaptive(int targets) {
+  if (adapt.ensure(n, max_leaves(), cap_nodes, targets)) for (auto& tg : graphs) tg.destroy();
   return adapt.resid.p;
 }
 
@@ -321,10 +321,10 @@ void TreeBuilder::enqueue(const TreeInputs& in) {
   }
   // the node each row was routed to (at most one split above its leaf) when the levels were routed
   const uint8_t* start = routed && D >= 2 ? node_of_row.p : nullptr;
-  if (in.adaptive) {             // reg:absoluteerror: each leaf's value becomes fl(q * lr), q the median of its rows' residuals
+  if (in.adaptive) {             // each leaf's value becomes fl(q * lr), q the alpha-quantile of its rows' residuals
     launch_locate_leaves(ta, gs.n_nodes, bm.bins_col, bm.n, bm.has_missing, start, g_only ? nullptr : gpair.p + (size_t)k * gp_stride, &adapt, s);
     SelectArgs sa{}; sa.values = in.resid; sa.seg = adapt.seg.p; sa.h = in.adaptive == 2 ? reinterpret_cast<const float*>(gpair.p + (size_t)k * gp_stride) + 1 : nullptr;
-    sa.h_stride = 2; sa.scales = gs.scales; sa.n = bm.n; sa.nseg = max_leaves(); sa.alpha = 0.5;
+    sa.h_stride = 2; sa.scales = gs.scales; sa.n = bm.n; sa.nseg = max_leaves(); sa.alpha = (double)in.alpha;
     if (in.adaptive == 3) { sa.h = in.weight; sa.h_stride = 1; sa.scales = adapt.scales.p; }
     sa.leaf_nid = adapt.leaf_nid.p; sa.split_cond = ta.split_cond; sa.lr = in.p.eta;
     segmented_select(sa, &adapt, [&](unsigned long long* p, size_t cnt) { collective([p, cnt, s]() { Comm::get().allreduce_sum_i64(p, cnt, s); }); },

@@ -25,12 +25,13 @@ struct TreeInputs {
   int lg_iters, n_ic;                     // grow_policy=lossguide: expansions per tree (0 = depthwise); interaction constraint sets
   int K, k, world;                        // classes, the class of this tree, ranks of the job
   int root_mode;                          // 0 = accumulate G and H, 1 = G and H + snapshot of the root H plane, 2 = G only on top of it
-  // reg:absoluteerror: the round's residuals fl(y - m) by row, and the leaf refresh after the structure is final (adaptive.h):
-  // 0 = none, 1 = quantile of the rows' residuals by count, 2 = by h_q (weighted data), 3 = by the instance weights `weight` on
-  // their own grid (adapt.scales[1], adaptive.h weight_grid): weighted data under gradient-based sampling, whose h is w / p
+  // reg:absoluteerror / reg:quantileerror: the round's residuals fl(y - m) by row of this tree's output, and the leaf refresh
+  // after the structure is final (adaptive.h): 0 = none, 1 = alpha-quantile of the rows' residuals by count, 2 = by h_q
+  // (weighted data), 3 = by the instance weights `weight` on their own grid (adapt.scales[1], adaptive.h weight_grid): weighted
+  // data under gradient-based sampling, whose h is w / p.  alpha: 0.5 for absolute error, the target's quantile_alpha entry.
   const float* resid; const float* weight;
   int adaptive;
-  int unused;                             // makes the padding explicit
+  float alpha;
 };
 static_assert(std::is_trivially_copyable<TreeInputs>::value, "TreeInputs is compared as bytes");
 static_assert(sizeof(BinnedMatrix) == 4 * sizeof(void*) + sizeof(int64_t) + 8 * sizeof(int), "BinnedMatrix has padding bytes");
@@ -104,10 +105,13 @@ struct TreeBuilder {
   PinnedPool pinned; std::vector<cudaEvent_t> free_events;
   std::vector<TreeGraph> graphs;           // per class
   TreeGraph* capturing = nullptr;          // set while enqueue runs under stream capture: collectives cut the capture
-  // reg:absoluteerror: the round's residuals and the leaf refresh's buffers, allocated by ensure_adaptive (only for that objective)
+  // reg:absoluteerror / reg:quantileerror: the round's residuals and the leaf refresh's buffers, allocated by ensure_adaptive
+  // (only for those objectives)
   SelectScratch adapt;
   int max_leaves() const { return lg_iters > 0 ? lg_iters + 1 : 1 << max_depth; }
-  float* ensure_adaptive();                // sizes `adapt` for this builder (destroys the captured graphs when a buffer moves); the residual buffer
+  // sizes `adapt` for this builder and `targets` residual columns of n rows (destroys the captured graphs when a buffer moves);
+  // the residual buffer
+  float* ensure_adaptive(int targets = 1);
   // profiling: CUDA events around the launches of each kind and the partition's byte model
   enum ProfKind { kProfRootHist, kProfDeepHist, kProfPartition, kProfMargin, kProfKinds };
   struct ProfEvent { cudaEvent_t a, b; int kind; long long launches; };

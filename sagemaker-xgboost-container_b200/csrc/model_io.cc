@@ -20,12 +20,27 @@ static std::string float_repr(float v) {       // shortest round-trip, xgboost s
   return mant + "E" + std::to_string(ex);
 }
 static JPtr S(const std::string& s) { return JValue::Str(s); }
+// reg:quantileerror's block into raw parameters (read back, and checked, only under that objective by configure)
+static void quantile_params_from_json(const JValue& obj, std::map<std::string, std::string>* raw) {
+  if (auto qp = obj.get("quantile_loss_param")) if (auto v = qp->get("quantile_alpha")) if (v->type == JValue::kString) (*raw)["quantile_alpha"] = v->s;
+}
 // the AFT parameter block into raw parameters (read back, and range-checked, only under survival:aft by configure)
 static void aft_params_from_json(const JValue& obj, std::map<std::string, std::string>* raw) {
   auto ap = obj.get("aft_loss_param");
   if (!ap) return;
   if (auto v = ap->get("aft_loss_distribution")) (*raw)["aft_loss_distribution"] = v->s;
   if (auto v = ap->get("aft_loss_distribution_scale")) (*raw)["aft_loss_distribution_scale"] = v->type == JValue::kString ? v->s : float_repr((float)v->as_double());
+}
+
+// quantile_alpha as "[0.1, 0.5, 0.9]": each value in the fewest %g digits that read back to the same float
+static std::string alpha_repr(const std::vector<float>& a) {
+  std::string out = "[";
+  for (size_t i = 0; i < a.size(); ++i) {
+    char b[48];
+    for (int p = 1; p <= 9; ++p) { snprintf(b, sizeof b, "%.*g", p, (double)a[i]); if (std::strtof(b, nullptr) == a[i]) break; }
+    out += (i ? ", " : "") + std::string(b);
+  }
+  return out + "]";
 }
 
 // per-objective parameter block of the model / config documents (upstream ObjFunction::SaveConfig)
@@ -36,6 +51,7 @@ static void objective_params_to_json(JValue& obj, const TrainParam& p) {
     case kTweedie: rp->set("tweedie_variance_power", S(float_repr(p.tweedie_variance_power))); obj.set("tweedie_regression_param", rp); break;
     case kPseudoHuber: rp->set("huber_slope", S(float_repr(p.huber_slope))); obj.set("pseudo_huber_param", rp); break;
     case kGamma: case kHinge: case kCox: case kAbsoluteError: break;
+    case kQuantileError: rp->set("quantile_alpha", S(alpha_repr(p.quantile_alpha))); obj.set("quantile_loss_param", rp); break;   // [UPSTREAM-RECALL]
     case kAft: {
       static const char* dist[] = {"normal", "logistic", "extreme"};
       rp->set("aft_loss_distribution", S(dist[p.aft_dist])); rp->set("aft_loss_distribution_scale", S(float_repr(p.aft_sigma)));
@@ -46,7 +62,7 @@ static void objective_params_to_json(JValue& obj, const TrainParam& p) {
 
 JPtr Booster::model_to_json() {
   configure(); sync_model();
-  const int K = param_.num_class;
+  const int K = param_.num_class;           // classes; the outputs of a quantile model go to num_target
   JPtr doc = JValue::Object();
   JPtr learner = JValue::Object();
   JPtr attributes = JValue::Object();
@@ -92,7 +108,8 @@ JPtr Booster::model_to_json() {
   // scalar form = the 3.0.x schema this document is stamped with (3.1+ writes the bracketed vector "[1.0E1]", which the
   // reader below accepts as well: the reference's own fixture is a [3,2,0] file)
   lmp->set("base_score", S(float_repr(base_score_))); lmp->set("boost_from_average", S("1"));
-  lmp->set("num_class", S(std::to_string(K > 1 ? K : 0))); lmp->set("num_feature", S(std::to_string(num_feature_))); lmp->set("num_target", S("1"));
+  lmp->set("num_class", S(std::to_string(K > 1 ? K : 0))); lmp->set("num_feature", S(std::to_string(num_feature_)));
+  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : 1)));
   learner->set("learner_model_param", lmp);
   JPtr obj = JValue::Object(); obj->set("name", S(objective_name_));
   if (param_.objective == kSoftprob || param_.objective == kSoftmax) { JPtr sp = JValue::Object(); sp->set("num_class", S(std::to_string(K))); obj->set("softmax_multiclass_param", sp); }
@@ -131,6 +148,7 @@ void Booster::model_from_json(const JValue& doc) {
   if (auto tp = obj.get("tweedie_regression_param")) if (auto v = tp->get("tweedie_variance_power")) raw_params_["tweedie_variance_power"] = std::to_string(v->as_double());
   if (auto hp = obj.get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = std::to_string(v->as_double());
   aft_params_from_json(obj, &raw_params_);
+  quantile_params_from_json(obj, &raw_params_);
   const JValue& lmp = learner.at("learner_model_param");
   num_feature_ = (int)lmp.at("num_feature").as_int();
   int nc = lmp.has("num_class") ? (int)lmp.at("num_class").as_int() : 0;
@@ -151,6 +169,13 @@ void Booster::model_from_json(const JValue& doc) {
   const JValue& tinfo = model.at("tree_info");
   B200_CHECK(trees.type == JValue::kArray && tinfo.length() == trees.arr.size(), "model: tree_info does not have one entry per tree");
   int K = std::max(1, nc); if (nc <= 1) if (auto sp = obj.get("softmax_multiclass_param")) K = std::max(1, (int)sp->at("num_class").as_int());
+  if (objective_name_ == "reg:quantileerror") {   // one output per quantile_alpha entry: num_target of them
+    const int nt = lmp.has("num_target") ? (int)lmp.at("num_target").as_int() : 1;
+    auto qa = raw_params_.find("quantile_alpha");
+    B200_CHECK(qa != raw_params_.end(), "model: a reg:quantileerror model needs objective.quantile_loss_param.quantile_alpha");
+    B200_CHECK((int)parse_quantile_alpha(qa->second).size() == nt, "model: num_target is " + std::to_string(nt) + " but quantile_alpha is " + qa->second);
+    K = std::max(1, nt);
+  }
   for (size_t t = 0; t < trees.arr.size(); ++t) { const double g = tinfo.num_at(t); B200_CHECK(g >= 0 && g < K, "model: tree_info entry out of range"); }
   // the layer layout: iteration_indptr when the document has it (2.x / 3.x), else K * num_parallel_tree trees per round (1.x)
   int P = 1;
@@ -276,7 +301,8 @@ JPtr Booster::config_to_json() {
   }
   learner->set("gradient_booster", gb);
   JPtr lmp = JValue::Object(); lmp->set("base_score", S(float_repr(base_score_))); lmp->set("boost_from_average", S("1"));
-  lmp->set("num_class", S(std::to_string(param_.num_class > 1 ? param_.num_class : 0))); lmp->set("num_feature", S(std::to_string(num_feature_))); lmp->set("num_target", S("1"));
+  lmp->set("num_class", S(std::to_string(param_.num_class > 1 ? param_.num_class : 0))); lmp->set("num_feature", S(std::to_string(num_feature_)));
+  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : 1)));
   learner->set("learner_model_param", lmp);
   JPtr ltp = JValue::Object(); ltp->set("booster", S(dart_.on ? "dart" : "gbtree")); ltp->set("disable_default_eval_metric", S("0")); ltp->set("multi_strategy", S("one_output_per_tree")); ltp->set("objective", S(objective_name_));
   learner->set("learner_train_param", ltp);
@@ -314,6 +340,7 @@ void Booster::config_from_json(const JValue& doc) {
     if (auto tp = o->get("tweedie_regression_param")) if (auto v = tp->get("tweedie_variance_power")) raw_params_["tweedie_variance_power"] = v->s;
     if (auto hp = o->get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = v->s;
     aft_params_from_json(*o, &raw_params_);
+    quantile_params_from_json(*o, &raw_params_);
   }
   if (auto m = learner.get("metrics")) { eval_metrics_.clear(); for (auto& x : m->arr) eval_metrics_.push_back(x->at("name").s); }
   configured_ = false;
