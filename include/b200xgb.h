@@ -46,10 +46,12 @@ XGB_DLL int XGBuildInfo(const char** out);
 /* upstream's Python package passes ndarray inputs as `__array_interface__` JSON ({"data":[ptr,ro],"shape":[n,m],"typestr":"<f4"}),
  * config {"missing": NaN, "nthread": 0}; data_utils.py:384 (Parquet -> numpy), encoder.py:52 (CSV payload) reach it */
 XGB_DLL int XGDMatrixCreateFromDense(const char* data, const char* config, DMatrixHandle* out);
-/* labels / weights / base_margin from an array interface (DMatrix(label=...), data_utils.py:384) */
+/* labels / weights / base_margin from an array interface (DMatrix(label=...), data_utils.py:384); "group" (query group sizes) and
+ * "qid" (one query id per row, non-decreasing; groups are its runs) from DMatrix(group=...) / DMatrix(qid=...) / set_info */
 XGB_DLL int XGDMatrixSetInfoFromInterface(DMatrixHandle handle, const char* field, const char* data);
 /* {"uri": "<path>?format=csv&label_column=0[&weight_column=1][&delimiter=,]" | "<path>?format=libsvm"}: data_utils.py:309-313,361;
- * a directory means every regular file in it (data_utils.py:520-545); CSV text is parsed on the device */
+ * a directory means every regular file in it (data_utils.py:520-545); CSV text is parsed on the device; libsvm qid:<id> tokens
+ * become the query groups (the runs of equal consecutive qid over the files in order) */
 XGB_DLL int XGDMatrixCreateFromURI(const char* config, DMatrixHandle* out);
 XGB_DLL int XGDMatrixCreateFromMat(const float* data, bst_ulong nrow, bst_ulong ncol, float missing, DMatrixHandle* out);
 /* CSR; num_col = 0 means "infer from the indices" (libsvm loader: indices kept as-is, data_utils.py:348-365) */
@@ -66,6 +68,14 @@ XGB_DLL int XGDMatrixNumCol(DMatrixHandle handle, bst_ulong* out);
 XGB_DLL int XGDMatrixSetFloatInfo(DMatrixHandle handle, const char* field, const float* array, bst_ulong len);
 XGB_DLL int XGDMatrixGetFloatInfo(DMatrixHandle handle, const char* field, bst_ulong* out_len, const float** out_dptr); /* train.py:394-396 get_label */
 XGB_DLL int XGDMatrixSliceDMatrix(DMatrixHandle handle, const int* idxset, bst_ulong len, DMatrixHandle* out);          /* train.py:410-411 */
+/* DMatrix.slice(rindex, allow_groups): with query groups, allow_groups != 0 and idxset listing whole groups (the slice keeps them) */
+XGB_DLL int XGDMatrixSliceDMatrixEx(DMatrixHandle handle, const int* idxset, bst_ulong len, DMatrixHandle* out, int allow_groups);
+/* query groups (rank:pairwise / rank:ndcg / rank:map, the ndcg / map metrics; DMatrix.set_group / set_uint_info / get_uint_info /
+ * get_group): field "group_ptr" (len = groups + 1, from 0 to num_row) or "group" (the sizes); Get returns "group_ptr", empty
+ * without groups */
+XGB_DLL int XGDMatrixSetUIntInfo(DMatrixHandle handle, const char* field, const unsigned* array, bst_ulong len);
+XGB_DLL int XGDMatrixGetUIntInfo(DMatrixHandle handle, const char* field, bst_ulong* out_len, const unsigned** out_dptr);
+XGB_DLL int XGDMatrixSetGroup(DMatrixHandle handle, const unsigned* group, bst_ulong len);
 /* field: "feature_name" | "feature_type" */
 XGB_DLL int XGDMatrixSetStrFeatureInfo(DMatrixHandle handle, const char* field, const char** features, bst_ulong size);
 XGB_DLL int XGDMatrixGetStrFeatureInfo(DMatrixHandle handle, const char* field, bst_ulong* size, const char*** out_features);

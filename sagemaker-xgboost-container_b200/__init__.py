@@ -11,7 +11,7 @@ from . import callback, collective, core, dask, sklearn, tracker, training  # no
 from .backend import XGBoostError, get_backend  # noqa: F401
 from .core import Booster, DMatrix  # noqa: F401
 from .training import cv, train  # noqa: F401
-from .sklearn import XGBClassifier, XGBModel, XGBRegressor, XGBRFClassifier, XGBRFRegressor  # noqa: F401
+from .sklearn import XGBClassifier, XGBModel, XGBRanker, XGBRegressor, XGBRFClassifier, XGBRFRegressor  # noqa: F401
 
 __version__ = "3.0.5"        # API level mirrored (docker/3.0-5/base/Dockerfile.cpu:33 pins xgboost==3.0.5)
 

@@ -38,6 +38,7 @@ class CudaBackend:
 
     name = "cuda"
     supports_process_type_update = True      # refresh / prune of loaded trees (csrc/refresh.cu)
+    supports_ranking = True                  # query groups, rank:* objectives, ndcg / map metrics (csrc/rank.cu)
 
     def __init__(self, path=LIB_PATH):
         if not os.path.exists(path):
@@ -199,11 +200,34 @@ class CudaBackend:
             return np.zeros(0, np.float32)
         return np.ctypeslib.as_array(ptr, shape=(n.value,)).copy()
 
-    def dmatrix_slice(self, h, idx):
+    def dmatrix_slice(self, h, idx, allow_groups=False):
         idx = np.ascontiguousarray(idx, dtype=np.int32)
         out = C.c_void_p()
-        self._check(self.lib.XGDMatrixSliceDMatrix(h, idx.ctypes.data_as(C.POINTER(C.c_int)), c_bst_ulong(len(idx)), C.byref(out)))
+        self._check(self.lib.XGDMatrixSliceDMatrixEx(h, idx.ctypes.data_as(C.POINTER(C.c_int)), c_bst_ulong(len(idx)), C.byref(out),
+                                                     C.c_int(1 if allow_groups else 0)))
         return out
+
+    def dmatrix_set_info_interface(self, h, field, arr):
+        """XGDMatrixSetInfoFromInterface with a 1-D host array (upstream's route for "group" and "qid")."""
+        arr = np.ascontiguousarray(arr).reshape(-1)
+        iface = {"data": [int(arr.ctypes.data), True], "shape": [int(arr.size)], "typestr": arr.dtype.str, "version": 3}
+        self._check(self.lib.XGDMatrixSetInfoFromInterface(h, _cstr(field), _cstr(json.dumps(iface))))
+
+    def dmatrix_set_uint_info(self, h, field, arr):
+        arr = np.ascontiguousarray(arr, dtype=np.uint32).reshape(-1)
+        self._check(self.lib.XGDMatrixSetUIntInfo(h, _cstr(field), arr.ctypes.data_as(C.POINTER(C.c_uint)), c_bst_ulong(arr.size)))
+
+    def dmatrix_set_group(self, h, sizes):
+        arr = np.ascontiguousarray(sizes, dtype=np.uint32).reshape(-1)
+        self._check(self.lib.XGDMatrixSetGroup(h, arr.ctypes.data_as(C.POINTER(C.c_uint)), c_bst_ulong(arr.size)))
+
+    def dmatrix_get_uint_info(self, h, field):
+        n = c_bst_ulong()
+        ptr = C.POINTER(C.c_uint)()
+        self._check(self.lib.XGDMatrixGetUIntInfo(h, _cstr(field), C.byref(n), C.byref(ptr)))
+        if n.value == 0:
+            return np.zeros(0, np.uint32)
+        return np.ctypeslib.as_array(ptr, shape=(n.value,)).copy()
 
     def dmatrix_set_str_info(self, h, field, values):
         values = list(values or [])

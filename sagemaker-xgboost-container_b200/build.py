@@ -14,12 +14,12 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "lib", "libb200xgb.so")
-SOURCES = ["hist.cu", "tree.cu", "misc.cu", "quantile.cu", "auc.cu", "shap.cu", "dart.cu", "survival.cu", "adaptive.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
+SOURCES = ["hist.cu", "tree.cu", "misc.cu", "quantile.cu", "auc.cu", "shap.cu", "dart.cu", "survival.cu", "rank.cu", "adaptive.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
          "-diag-suppress", "177", "-I", os.path.join(HERE, "..", "include")]
-# survival.cu computes its objectives in double: no fused multiply-adds, so they round like a host restatement of the formulas
-EXTRA_FLAGS = {"survival.cu": ["--fmad=false"]}
+# survival.cu and rank.cu compute their objectives in double: no fused multiply-adds, so they round like a host restatement of the formulas
+EXTRA_FLAGS = {"survival.cu": ["--fmad=false"], "rank.cu": ["--fmad=false"]}
 
 
 def _newest_header():

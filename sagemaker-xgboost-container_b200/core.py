@@ -35,7 +35,7 @@ class DMatrix:
                  feature_weights=None, enable_categorical=False, data_split_mode=None):
         self.handle = None
         if group is not None or qid is not None:
-            raise XGBoostError("ranking (group/qid) data is not supported on the CUDA hist path")
+            _check_ranking_backend()
         if enable_categorical:
             raise XGBoostError("categorical features are not supported on the CUDA hist path")
         be = get_backend()
@@ -43,7 +43,10 @@ class DMatrix:
         if isinstance(data, (str, os.PathLike)) and self._try_device_csv(os.fspath(data), be):
             pass
         elif isinstance(data, (str, os.PathLike)):
-            X, y, w = load_uri(os.fspath(data))
+            X, y, w, q = load_uri(os.fspath(data), with_qid=True)
+            if q is not None and qid is None and group is None:
+                _check_ranking_backend()
+                qid = q
             if _is_scipy_sparse(X):
                 self.handle = be.dmatrix_from_csr(X.indptr, X.indices, X.data, X.shape[1])
             else:
@@ -87,6 +90,10 @@ class DMatrix:
             self.set_float_info("label_lower_bound", label_lower_bound)
         if label_upper_bound is not None:
             self.set_float_info("label_upper_bound", label_upper_bound)
+        if group is not None:
+            self.set_group(group)
+        if qid is not None:
+            self.set_info(qid=qid)
         if feature_names is not None:
             self.feature_names = feature_names
         if feature_types is not None:
@@ -164,8 +171,31 @@ class DMatrix:
     def get_base_margin(self):
         return self.get_float_info("base_margin")
 
+    # ---- query groups (rank:* objectives, ndcg / map metrics); under groups a weight is one per group
+    def set_group(self, group):
+        _check_ranking_backend()
+        get_backend().dmatrix_set_group(self.handle, np.asarray(group, dtype=np.uint32))
+
+    def set_uint_info(self, field, data):
+        _check_ranking_backend()
+        get_backend().dmatrix_set_uint_info(self.handle, field, np.asarray(data, dtype=np.uint32))
+
+    def get_uint_info(self, field):
+        be = get_backend()
+        return be.dmatrix_get_uint_info(self.handle, field) if getattr(be, "supports_ranking", False) else np.zeros(0, np.uint32)
+
+    def get_group(self):
+        ptr = self.get_uint_info("group_ptr")
+        return np.diff(ptr).astype(np.uint32) if len(ptr) else np.zeros(0, np.uint32)
+
     def set_info(self, *, label=None, weight=None, base_margin=None, label_lower_bound=None, label_upper_bound=None, feature_names=None,
-                 feature_types=None, **kwargs):
+                 feature_types=None, group=None, qid=None, **kwargs):
+        if group is not None:
+            self.set_group(group)
+        if qid is not None:
+            _check_ranking_backend()
+            q = np.asarray(qid)
+            get_backend().dmatrix_set_info_interface(self.handle, "qid", q if q.dtype.kind in "iu" else q.astype(np.float64))
         if label is not None:
             self.set_label(label)
         if weight is not None:
@@ -186,8 +216,9 @@ class DMatrix:
 
     def slice(self, rindex, allow_groups=False):
         idx = np.asarray(list(rindex) if not isinstance(rindex, np.ndarray) else rindex, dtype=np.int32)
-        res = DMatrix._from_handle(get_backend().dmatrix_slice(self.handle, idx))
-        return res
+        be = get_backend()
+        h = be.dmatrix_slice(self.handle, idx, allow_groups=True) if allow_groups else be.dmatrix_slice(self.handle, idx)
+        return DMatrix._from_handle(h)
 
     @property
     def feature_names(self):
@@ -212,6 +243,11 @@ class DMatrix:
     @feature_types.setter
     def feature_types(self, types):
         get_backend().dmatrix_set_str_info(self.handle, "feature_type", list(types) if types else [])
+
+
+def _check_ranking_backend():
+    if not getattr(get_backend(), "supports_ranking", False):
+        raise XGBoostError("query groups (group / qid) and the rank:* objectives are not implemented by this engine")
 
 
 def _param_items(params):
@@ -289,6 +325,8 @@ def _check_unapplied(k, v):
         if k == "process_type" and str(v) == "update":
             raise XGBoostError("process_type=update is not implemented by this engine")
         return _DROP
+    if k == "objective" and str(v).startswith("rank:"):
+        _check_ranking_backend()
     if k in _IGNORED_PARAMS:
         return _DROP
     return v

@@ -95,8 +95,21 @@ __global__ void gather_rows_kernel(const float* X, int F, const int* idx, int64_
   }
 }
 
-std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len) const {
+std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len, bool allow_groups) const {
   for (int64_t i = 0; i < len; ++i) B200_CHECK(idx[i] >= 0 && idx[i] < n, "DMatrix.slice: row index out of range");
+  // with query groups: idx must list whole groups, each one's rows in order; the slice keeps those groups (and their weights)
+  std::vector<unsigned> ptr; std::vector<int> groups;
+  if (!group_ptr.empty()) {
+    B200_CHECK(allow_groups, "DMatrix.slice: the matrix has query groups; slice it by whole groups with allow_groups=True");
+    ptr.push_back(0);
+    for (int64_t i = 0; i < len;) {
+      const int g = (int)(std::upper_bound(group_ptr.begin(), group_ptr.end(), (unsigned)idx[i]) - group_ptr.begin()) - 1;
+      const int64_t size = (int64_t)group_ptr[g + 1] - group_ptr[g];
+      B200_CHECK(idx[i] == (int)group_ptr[g] && i + size <= len, "DMatrix.slice: with allow_groups=True the rows must be whole query groups");
+      for (int64_t j = 0; j < size; ++j) B200_CHECK(idx[i + j] == (int)(group_ptr[g] + j), "DMatrix.slice: with allow_groups=True the rows must be whole query groups");
+      groups.push_back(g); i += size; ptr.push_back((unsigned)i);
+    }
+  }
   auto dm = std::make_unique<DMatrix>();
   dm->n = len; dm->F = F; dm->has_missing = has_missing;
   dm->feature_names = feature_names; dm->feature_types = feature_types;
@@ -113,7 +126,14 @@ std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len) const {
   auto take = [&](const std::vector<float>& src, size_t per_row) { std::vector<float> o; if (src.empty()) return o; o.resize(len * per_row);
     for (int64_t i = 0; i < len; ++i) for (size_t k = 0; k < per_row; ++k) o[i * per_row + k] = src[(size_t)idx[i] * per_row + k]; return o; };
   if (!labels.empty()) { auto v = take(labels, 1); dm->set_float_info("label", v.data(), v.size()); }
-  if (!weights.empty()) { auto v = take(weights, 1); dm->set_float_info("weight", v.data(), v.size()); }
+  if (!group_ptr.empty()) {
+    dm->set_group_ptr(ptr);
+    if (!weights.empty()) {
+      B200_CHECK(weights.size() == group_ptr.size() - 1, "DMatrix.slice: a matrix with query groups needs one weight per group");
+      std::vector<float> v; for (int g : groups) v.push_back(weights[g]);
+      dm->set_float_info("weight", v.data(), v.size());
+    }
+  } else if (!weights.empty()) { auto v = take(weights, 1); dm->set_float_info("weight", v.data(), v.size()); }
   if (!label_lower.empty()) { auto v = take(label_lower, 1); dm->set_float_info("label_lower_bound", v.data(), v.size()); }
   if (!label_upper.empty()) { auto v = take(label_upper, 1); dm->set_float_info("label_upper_bound", v.data(), v.size()); }
   if (!base_margin.empty() && n > 0) { size_t per = base_margin.size() / n; auto v = take(base_margin, per); dm->set_float_info("base_margin", v.data(), v.size()); }
@@ -126,16 +146,46 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
     h.assign(v, v + len); d.alloc(len);
     if (len) { CUDA_OK(cudaMemcpyAsync(d.p, h.data(), sizeof(float) * len, cudaMemcpyHostToDevice, s)); Comm::get().sync_stream(s); }
   };
-  if (field == "label") { put(labels, d_labels); cox_order.valid = false; }
+  if (field == "label") { put(labels, d_labels); cox_order.valid = false; rank_groups.valid = false; }
   else if (field == "label_lower_bound") put(label_lower, d_label_lower);      // survival:aft; the bins do not depend on them
   else if (field == "label_upper_bound") put(label_upper, d_label_upper);
   else if (field == "weight") {
     for (size_t i = 0; i < len; ++i) B200_CHECK(v[i] >= 0 && !std::isnan(v[i]), "Weights must be positive values.");
     put(weights, d_weights);
     binned = false;      // weighted quantiles depend on the weights
+    rank_groups.valid = false;
   }
   else if (field == "base_margin") put(base_margin, d_base_margin);
   else throw Error("Unknown float field name: " + field);
+}
+
+void DMatrix::set_group_ptr(std::vector<unsigned> ptr) {
+  B200_CHECK(!ptr.empty() && ptr[0] == 0, "group_ptr must start at 0");
+  for (size_t g = 1; g < ptr.size(); ++g) B200_CHECK(ptr[g] >= ptr[g - 1], "group_ptr must not decrease");
+  B200_CHECK((int64_t)ptr.back() == n, "the query groups cover " + std::to_string(ptr.back()) + " rows but the DMatrix has " + std::to_string(n) +
+             " (group sizes must add up to num_row)");
+  group_ptr = ptr.size() > 1 ? std::move(ptr) : std::vector<unsigned>{};
+  rank_groups.valid = false;
+  binned = binned && weights.empty();       // the sketch reads per-group weights row by row
+}
+
+void DMatrix::set_group_sizes(const unsigned* sizes, size_t len) {
+  std::vector<unsigned> ptr{0};
+  uint64_t at = 0;
+  for (size_t g = 0; g < len; ++g) { at += sizes[g]; B200_CHECK(at <= (uint64_t)n, "the query group sizes add up to more than the " + std::to_string(n) + " rows of the DMatrix"); ptr.push_back((unsigned)at); }
+  set_group_ptr(std::move(ptr));
+}
+
+void DMatrix::set_qid(const int64_t* qid, size_t len) {
+  B200_CHECK((int64_t)len == n, "qid must have one entry per row (" + std::to_string(n) + " rows, " + std::to_string(len) + " qid)");
+  std::vector<unsigned> ptr{0};
+  for (size_t i = 1; i < len; ++i) {
+    B200_CHECK(qid[i] >= qid[i - 1], "qid must be sorted in non-decreasing order (row " + std::to_string(i) + ": " + std::to_string(qid[i]) + " after " +
+               std::to_string(qid[i - 1]) + ")");
+    if (qid[i] != qid[i - 1]) ptr.push_back((unsigned)i);
+  }
+  if (len) ptr.push_back((unsigned)len);
+  set_group_ptr(std::move(ptr));
 }
 
 const std::vector<float>& DMatrix::get_float_info(const std::string& field) const {
@@ -190,8 +240,21 @@ void DMatrix::ensure_binned(int max_bin) {
   B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
   cudaStream_t s = engine_stream();
   Comm& comm = Comm::get();
+  // weights per query group weigh each row of the group in the sketch
+  DevBuf<float> row_w;
+  const float* w = weights.empty() ? nullptr : d_weights.p;
+  if (w && (int64_t)weights.size() != n) {
+    B200_CHECK(!group_ptr.empty() && weights.size() == group_ptr.size() - 1, "weights must have one entry per row, or one per query group (" +
+               std::to_string(n) + " rows, " + std::to_string(weights.size()) + " weights)");
+    std::vector<float> h((size_t)n);
+    for (size_t g = 0; g + 1 < group_ptr.size(); ++g) std::fill(h.begin() + group_ptr[g], h.begin() + group_ptr[g + 1], weights[g]);
+    row_w.alloc((size_t)n);
+    CUDA_OK(cudaMemcpyAsync(row_w.p, h.data(), sizeof(float) * n, cudaMemcpyHostToDevice, s));
+    comm.sync_stream(s);
+    w = row_w.p;
+  }
   if (!comm.distributed()) {
-    compute_cuts_device(X.p, n, F, weights.empty() ? nullptr : d_weights.p, max_bin, has_missing, &cuts, s);
+    compute_cuts_device(X.p, n, F, w, max_bin, has_missing, &cuts, s);
   } else {
     // every rank summarises its shard (exact when a feature has <= cap distinct values), the summaries are
     // all-gathered and merged, and every rank derives the same cuts.
@@ -205,7 +268,7 @@ void DMatrix::ensure_binned(int max_bin) {
       has_missing = v != 0;
     }
     std::vector<FeatureSummary> local;
-    compute_summaries_device(X.p, n, F, weights.empty() ? nullptr : d_weights.p, cap, &local, s);
+    compute_summaries_device(X.p, n, F, w, cap, &local, s);
     const size_t per_feat = (size_t)(cap + 2);
     const size_t rec = per_feat * (sizeof(float) + sizeof(double)) + sizeof(double);   // vals, weights, count
     std::vector<unsigned char> sendbuf((size_t)F * rec, 0);
@@ -251,6 +314,9 @@ void DMatrix::ensure_binned(int max_bin) {
 // rows of tree j >= 1 of a round from kForestRowStream + 2^20 round + j (index: row); tree 0 keeps 0x2000 + round.
 constexpr uint64_t kDartSkipStream = 0x10000000000ull, kDartOneStream = 0x20000000000ull, kDartTreeStream = 0x30000000000ull;
 constexpr uint64_t kForestRowStream = 0x40000000000ull;
+// lambdarank_pair_method=mean: draw j of a document of round `round` comes from kRankPairStream + 2^20 round + j (index: row + rank
+// offset, as the subsample draw), so lambdarank_num_pair_per_sample is at most 2^20 under mean
+constexpr uint64_t kRankPairStream = 0x50000000000ull;
 // the stream tree j of boosting round `round` draws its row sample from (uniform and gradient-based sampling alike)
 static uint64_t row_stream(int round, int j) { return j == 0 ? 0x2000ull + (uint64_t)round : kForestRowStream + ((uint64_t)round << 20) + (uint64_t)j; }
 std::string subset_mask(const std::string& parent, float frac, unsigned seed, uint64_t stream) {
@@ -286,7 +352,7 @@ static const std::map<std::string, int>& objective_table() {
     {"reg:logistic", kRegLogistic}, {"binary:logitraw", kLogitRaw}, {"multi:softprob", kSoftprob}, {"multi:softmax", kSoftmax},
     {"reg:squaredlogerror", kSquaredLogError}, {"reg:pseudohubererror", kPseudoHuber}, {"count:poisson", kPoisson}, {"reg:gamma", kGamma},
     {"reg:tweedie", kTweedie}, {"binary:hinge", kHinge}, {"survival:aft", kAft}, {"survival:cox", kCox}, {"reg:absoluteerror", kAbsoluteError},
-    {"reg:quantileerror", kQuantileError}};
+    {"reg:quantileerror", kQuantileError}, {"rank:pairwise", kRankPairwise}, {"rank:ndcg", kRankNdcg}, {"rank:map", kRankMap}};
   return t;
 }
 
@@ -327,7 +393,7 @@ void Booster::configure() {
   auto ito = raw_params_.find("objective");
   if (ito != raw_params_.end()) objective_name_ = ito->second;
   auto ot = objective_table().find(objective_name_);
-  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:absoluteerror, reg:quantileerror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox)");
+  B200_CHECK(ot != objective_table().end(), "Unknown objective function: `" + objective_name_ + "` (supported on the CUDA hist path: reg:squarederror, reg:linear, reg:logistic, reg:squaredlogerror, reg:pseudohubererror, reg:absoluteerror, reg:quantileerror, reg:gamma, reg:tweedie, count:poisson, binary:logistic, binary:logitraw, binary:hinge, multi:softprob, multi:softmax, survival:aft, survival:cox, rank:pairwise, rank:ndcg, rank:map)");
   p.objective = ot->second;
   if (objective_name_ == "reg:linear") objective_name_ = "reg:squarederror";
   p.num_class = (p.objective == kSoftprob || p.objective == kSoftmax) ? geti("num_class", 0) : 1;
@@ -363,6 +429,33 @@ void Booster::configure() {
     }
     p.aft_sigma = getf("aft_loss_distribution_scale", nullptr, 1.0f);
     B200_CHECK(p.aft_sigma > 0.0f && std::isfinite(p.aft_sigma), "aft_loss_distribution_scale must be a finite number > 0 (got " + std::to_string(p.aft_sigma) + ")");
+  }
+  if (objective_is_rank(p.objective)) {     // the LambdaRank parameters are read (and checked) only under rank:*
+    auto getb = [&](const char* a, int def) {
+      auto it = raw_params_.find(a); if (it == raw_params_.end()) return def;
+      std::string v = it->second; for (char& ch : v) ch = (char)std::tolower((unsigned char)ch);
+      if (v == "1" || v == "true") return 1;
+      if (v == "0" || v == "false") return 0;
+      throw Error(std::string("Invalid value for parameter ") + a + ": " + it->second + " (true or false)");
+    };
+    if (auto pm = raw_params_.find("lambdarank_pair_method"); pm != raw_params_.end()) {
+      B200_CHECK(pm->second == "topk" || pm->second == "mean", "Invalid value for parameter lambdarank_pair_method: " + pm->second + " (topk, mean)");
+      p.rank_mean = pm->second == "mean" ? 1 : 0;
+    }
+    if (p.rank_mean) p.rank_k = 1;
+    if (auto kp = raw_params_.find("lambdarank_num_pair_per_sample"); kp != raw_params_.end()) {
+      double v = 0.0; size_t used = 0;
+      try { v = std::stod(kp->second, &used); } catch (...) { used = 0; }
+      B200_CHECK(used > 0 && used == kp->second.size() && v == std::floor(v) && v >= 1.0 && v <= 2147483647.0,
+                 "lambdarank_num_pair_per_sample must be an integer >= 1 (got " + kp->second + ")");
+      p.rank_k = (int)v;
+    }
+    p.rank_exp_gain = getb("ndcg_exp_gain", 1); p.rank_normalization = getb("lambdarank_normalization", 1);
+    p.rank_score_normalization = getb("lambdarank_score_normalization", 1);
+    p.rank_unbiased = getb("lambdarank_unbiased", 0);
+    B200_CHECK(!p.rank_mean || p.rank_k <= (1 << 20), "lambdarank_num_pair_per_sample must be <= 1048576 under lambdarank_pair_method=mean");
+    p.rank_bias_norm = getf("lambdarank_bias_norm", nullptr, 2.0f);
+    B200_CHECK(p.rank_bias_norm >= 0.0f, "lambdarank_bias_norm must be >= 0");
   }
   // count:poisson: max_delta_step defaults to 0.7 for the objective's hessian AND the tree's leaf clipping (upstream learner.cc sets
   // the shared parameter when the user did not)
@@ -495,7 +588,7 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
   if (param_.objective == kSoftprob || param_.objective == kSoftmax) { base_score_ = 0.5f; return; }
   // 3.0.x fits the intercept for the RegLossObj family only; the log-link objectives and binary:hinge keep the 0.5 default
   // [UPSTREAM-RECALL: src/objective/init_estimation.cc; later releases changed the GLM objectives]
-  if (objective_is_log_link(param_.objective) || param_.objective == kHinge || objective_is_survival(param_.objective)) { base_score_ = 0.5f; return; }
+  if (objective_is_log_link(param_.objective) || param_.objective == kHinge || objective_is_survival(param_.objective) || objective_is_rank(param_.objective)) { base_score_ = 0.5f; return; }
   cudaStream_t s = engine_stream();
   TreeBuilder& b = *builder_;
   if (param_.objective == kAbsoluteError) {
@@ -738,6 +831,11 @@ static void check_aft_bounds(const DMatrix* dm) {
              "survival:aft needs label_lower_bound and label_upper_bound with one entry per row (" + std::to_string(dm->n) + " rows, " +
              std::to_string(dm->label_lower.size()) + " lower and " + std::to_string(dm->label_upper.size()) + " upper bounds)");
 }
+// every objective and metric but the ranking ones reads one weight per row
+static void check_row_weights(const DMatrix* dm) {
+  B200_CHECK(dm->weights.empty() || (int64_t)dm->weights.size() == dm->n, "weights must have one entry per row (" + std::to_string(dm->n) + " rows, " +
+             std::to_string(dm->weights.size()) + " weights); one weight per query group is read by the rank:* objectives and the ndcg / map metrics only");
+}
 static void check_train_width(const DMatrix* dm) {
   B200_CHECK(dm->F <= kMaxTrainFeatures, "the CUDA hist builder trains on at most " + std::to_string(kMaxTrainFeatures) + " features (the data has " +
              std::to_string(dm->F) + ")");
@@ -758,6 +856,12 @@ void Booster::check_label_ranges(const DMatrix* dtrain) {
     if (param_.objective == kTweedie) for (float v : y) B200_CHECK(v >= 0.0f, "TweedieRegression: label must be nonnegative");
     if (param_.objective == kAbsoluteError) for (float v : y) B200_CHECK(!std::isnan(v), "reg:absoluteerror: label must not be NaN");
     if (param_.objective == kQuantileError) for (float v : y) B200_CHECK(!std::isnan(v), "reg:quantileerror: label must not be NaN");
+    if (objective_is_rank(param_.objective)) for (float v : y) B200_CHECK(!std::isnan(v), objective_name_ + ": label must not be NaN");
+    if (param_.objective == kRankNdcg) for (float v : y) {
+      B200_CHECK(v >= 0.0f, "rank:ndcg: label must be >= 0 (got " + std::to_string(v) + ")");
+      B200_CHECK(!param_.rank_exp_gain || v <= 31.0f, "rank:ndcg: label must be <= 31 with ndcg_exp_gain=true (got " + std::to_string(v) + "); set ndcg_exp_gain=false for larger relevance degrees");
+    }
+    if (param_.objective == kRankMap) for (float v : y) B200_CHECK(v == 0.0f || v == 1.0f, "rank:map: label must be 0 or 1 (got " + std::to_string(v) + ")");
     if (param_.objective == kAft)
       for (int64_t i = 0; i < dtrain->n; ++i) {
         const float lo = dtrain->label_lower[i], hi = dtrain->label_upper[i];
@@ -778,6 +882,8 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
              " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
   B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
+  if (objective_is_rank(param_.objective)) rank_groups(dtrain, objective_name_.c_str());
+  else check_row_weights(dtrain);
   if (update_mode_) { refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
   check_train_width(dtrain);
   dtrain->ensure_binned(param_.max_bin);
@@ -898,6 +1004,31 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
     launch_quantile_gradient(qa, s);
     return;
   }
+  if (objective_is_rank(param_.objective)) {
+    B200_CHECK(!dense_g, "the ranking objectives write (g,h) pairs");
+    B200_CHECK(!param_.rank_unbiased, "lambdarank_unbiased=true (position debiasing) is not implemented on the CUDA hist path; a model trained with it loads and predicts");
+    const RankGroups& rg = rank_groups(dm, objective_name_.c_str());
+    RankGradArgs ra{}; ra.margin = margin; ra.label = dm->d_labels.p; ra.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
+    // w_g * (groups / sum of w_g), both totals over every rank.  Every rank enters the all-reduce, with or without weights (an
+    // empty shard has no groups), and all of them or none must have weights.
+    double t[3] = {dm->n > 0 ? (double)rg.G : 0.0, 0.0, ra.weight ? 1.0 : 0.0};
+    for (float w : dm->weights) t[1] += (double)w;
+    if (Comm::get().distributed()) {
+      dsum_.ensure(4);
+      CUDA_OK(cudaMemcpyAsync(dsum_.p, t, sizeof t, cudaMemcpyHostToDevice, s));
+      Comm::get().allreduce_sum_f64(dsum_.p, 3, s);
+      CUDA_OK(cudaMemcpyAsync(t, dsum_.p, sizeof t, cudaMemcpyDeviceToHost, s));
+      Comm::get().sync_stream(s);
+      B200_CHECK(t[2] == 0.0 || t[2] == (double)Comm::get().world(), std::string(objective_name_) + ": every rank's DMatrix or none must have weights");
+    }
+    ra.wscale = t[2] > 0.0 && t[1] > 0.0 ? t[0] / t[1] : 1.0;
+    ra.gpair = gpair; ra.absmax = absmax; ra.n = dm->n; ra.row_offset = row_offset; ra.subsample = subsample; ra.seed = param_.seed;
+    ra.iter = (unsigned long long)round; ra.objective = param_.objective; ra.k = param_.rank_k; ra.exp_gain = param_.rank_exp_gain;
+    ra.normalization = param_.rank_normalization; ra.score_normalization = param_.rank_score_normalization;
+    ra.mean = param_.rank_mean; ra.pair_stream = kRankPairStream + ((uint64_t)round << 20);
+    launch_rank_gradient(ra, rg, &rank_scratch_, s);
+    return;
+  }
   if (objective_is_survival(param_.objective)) {
     B200_CHECK(!dense_g, "the survival objectives write (g,h) pairs");
     SurvivalGradArgs sa{}; sa.margin = margin; sa.label = dm->d_labels.p; sa.lower = dm->d_label_lower.p; sa.upper = dm->d_label_upper.p;
@@ -913,6 +1044,16 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
   ga.objective = param_.objective; ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = subsample; ga.seed = param_.seed;
   ga.iter = (unsigned long long)round; ga.aux = objective_aux(param_); ga.dense_g = dense_g ? 1 : 0;
   launch_gradient(ga, s);
+}
+
+// dm's query groups on the device (one group of all rows without groups), built on first use; what (an objective or metric)
+// reads one weight per group
+const RankGroups& Booster::rank_groups(DMatrix* dm, const char* what) {
+  check_labels(dm);
+  B200_CHECK(dm->weights.empty() || (int64_t)dm->weights.size() == dm->num_groups(), std::string(what) + " reads one weight per query group: the DMatrix has " +
+             std::to_string(dm->num_groups()) + " groups but " + std::to_string(dm->weights.size()) + " weights");
+  if (!dm->rank_groups.valid) rank_groups_build(dm->group_ptr, dm->d_labels.p, dm->n, &dm->rank_groups, &rank_scratch_, engine_stream());
+  return dm->rank_groups;
 }
 
 void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float* out) {
@@ -1177,8 +1318,26 @@ static std::string default_metric(const TrainParam& p) {
     case kHinge: return "error";
     case kAft: return "aft-nloglik";
     case kCox: return "cox-nloglik";
+    case kRankPairwise: case kRankNdcg: return p.rank_mean ? "ndcg" : "ndcg@" + std::to_string(p.rank_k);
+    case kRankMap: return p.rank_mean ? "map" : "map@" + std::to_string(p.rank_k);
     default: return "mlogloss";
   }
+}
+
+// ndcg, ndcg@k, ndcg-, ndcg@k-, map, map@k, map-, map@k- (k = 0: the whole group; '-' scores a group without relevant documents 0)
+static bool parse_rank_metric(const std::string& name, int* map, int* k, int* minus) {
+  std::string s = name;
+  if (s.rfind("ndcg", 0) == 0) { *map = 0; s = s.substr(4); }
+  else if (s.rfind("map", 0) == 0 && (s.size() == 3 || s[3] == '@' || s[3] == '-')) { *map = 1; s = s.substr(3); }
+  else return false;
+  *minus = 0; *k = 0;
+  if (!s.empty() && s.back() == '-') { *minus = 1; s.pop_back(); }
+  if (s.empty()) return true;
+  B200_CHECK(s[0] == '@' && s.size() > 1 && s.find_first_not_of("0123456789", 1) == std::string::npos && s.size() < 11,
+             "Invalid ranking metric " + name + " (ndcg, ndcg@k, ndcg-, ndcg@k-, map, map@k, map-, map@k-)");
+  *k = std::stoi(s.substr(1));
+  B200_CHECK(*k >= 1, "Invalid ranking metric " + name + ": k must be >= 1");
+  return true;
 }
 
 std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, const std::vector<std::string>& names) {
@@ -1201,9 +1360,24 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
       std::string base = mname;
       if (mname.rfind("tweedie-nloglik@", 0) == 0) { base = "tweedie-nloglik"; ma.aux = std::stof(mname.substr(16)); B200_CHECK(ma.aux >= 1.0f && ma.aux < 2.0f, "tweedie variance power must be in interval [1, 2)"); }
       if (mname.rfind("error@", 0) == 0) { base = "error"; ma.threshold = std::stof(mname.substr(6)); }
+      int rank_map = 0, rank_k = 0, rank_minus = 0;
+      if (parse_rank_metric(mname, &rank_map, &rank_k, &rank_minus)) {     // ndcg / map over the query groups (rank.cu)
+        const RankGroups& rg = rank_groups(dm, mname.c_str());
+        rank_metric(c.margin.p, dm->d_labels.p, ma.weight, rg, rank_map, rank_k, param_.rank_exp_gain, rank_minus, &rank_scratch_, dsum_.p, s);
+        Comm::get().allreduce_sum_f64(dsum_.p, 2, s);
+        double h[2];
+        CUDA_OK(cudaMemcpyAsync(h, dsum_.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        Comm::get().sync_stream(s);
+        char buf[64]; snprintf(buf, sizeof buf, "%.17g", h[1] > 0.0 ? h[0] / h[1] : 0.0);
+        out += "\t" + names[i] + "-" + mname + ":" + buf;
+        continue;
+      }
+      B200_CHECK(mname.rfind("pre@", 0) != 0 && mname != "pre", "metric " + mname + ": the pre / pre@k ranking metric is not implemented on the CUDA hist path (ndcg and map are)");
+      check_row_weights(dm);
       if (base == "auc") {
         // validated on hardware against sklearn.metrics.roc_auc_score (tests/test_gpu_parity.py::test_auc_matches_sklearn)
         B200_CHECK(param_.num_outputs() <= 1, "auc is implemented for binary / regression-style predictions only");
+        B200_CHECK(!objective_is_rank(param_.objective) || dm->group_ptr.empty(), "auc under a rank:* objective on a DMatrix with query groups (ranking AUC) is not implemented on the CUDA hist path");
         const int logistic = (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic) ? 1 : 0;
         compute_auc_device(c.margin.p, dm->d_labels.p, dm->weights.empty() ? nullptr : dm->d_weights.p, dm->n, logistic, dsum_.p, s);
         double h3[3];
@@ -1251,7 +1425,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         else if (base == "poisson-nloglik") ma.metric = kMetricPoissonNll; else if (base == "gamma-nloglik") ma.metric = kMetricGammaNll;
         else if (base == "gamma-deviance") ma.metric = kMetricGammaDeviance;
         else if (base == "tweedie-nloglik") { ma.metric = kMetricTweedieNll; if (ma.aux == 0.0f) throw Error("tweedie-nloglik needs its variance power: tweedie-nloglik@rho"); }
-        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, quantile, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik)");
+        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, quantile, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik, ndcg, ndcg@k, map, map@k)");
         if (param_.objective == kLogitRaw && (ma.metric == kMetricLogloss || ma.metric == kMetricError)) ma.is_logistic = 1;
         if ((ma.metric == kMetricMerror || ma.metric == kMetricMlogloss)) B200_CHECK(param_.num_class > 1, "Check failed: preds.size() == info.labels_.size() : label and prediction size not match, hint: use merror or mlogloss for multi-class classification");
         CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));

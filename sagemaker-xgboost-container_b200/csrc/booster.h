@@ -8,6 +8,7 @@
 #include "grow.h"
 #include "json.h"
 #include "misc.h"
+#include "rank.h"
 #include "refresh.h"
 #include "sampling.h"
 #include "survival.h"
@@ -28,6 +29,9 @@ class DMatrix {
   std::vector<float> label_lower, label_upper;         // survival:aft interval bounds (label_lower_bound / label_upper_bound)
   DevBuf<float> d_label_lower, d_label_upper;
   CoxOrder cox_order;                                 // survival:cox: the rows sorted by |label|, built on first use, reset with the labels
+  // query groups: group g is rows [group_ptr[g], group_ptr[g + 1]) (empty: no groups); under groups a weight is one per group
+  std::vector<unsigned> group_ptr;
+  RankGroups rank_groups;                             // their device layout, built on first use, reset with the labels, groups or weights
   std::vector<std::string> feature_names, feature_types;
   // binned representation (built on first use as a training matrix)
   bool binned = false; int binned_max_bin = 0;
@@ -53,8 +57,13 @@ class DMatrix {
   static std::unique_ptr<DMatrix> from_csr(const size_t* indptr, const unsigned* indices, const float* data, size_t nindptr, size_t nelem, size_t ncol);
   // recordio-protobuf body (recordio.cu): status 0 decoded, 1 the body is invalid (*message names the rule), 2 needs the host route
   static std::unique_ptr<DMatrix> from_recordio(const char* buf, int64_t len, int* status, std::string* message);
-  std::unique_ptr<DMatrix> slice(const int* idx, int64_t len) const;
+  // allow_groups: a matrix with groups may be sliced by whole groups, which the slice carries
+  std::unique_ptr<DMatrix> slice(const int* idx, int64_t len, bool allow_groups = false) const;
   void set_float_info(const std::string& field, const float* v, size_t len);
+  void set_group_ptr(std::vector<unsigned> ptr);      // validated: starts at 0, non-decreasing, ends at n
+  void set_group_sizes(const unsigned* sizes, size_t len);
+  void set_qid(const int64_t* qid, size_t len);       // groups are the runs of equal consecutive qid; qid must not decrease
+  int64_t num_groups() const { return group_ptr.empty() ? 1 : (int64_t)group_ptr.size() - 1; }
   const std::vector<float>& get_float_info(const std::string& field) const;
   void ensure_binned(int max_bin);
   void set_cuts(const HostCuts& c);                   // external cuts (shared with the oracle in tests)
@@ -195,6 +204,7 @@ class Booster {
   std::unique_ptr<TreeBuilder> builder_ = std::make_unique<TreeBuilder>();   // its device buffers are sized by builder_for
   DevBuf<double> dsum_;                         // device sums of the metrics and of the base-score stump
   CoxScratch cox_scratch_;                      // survival:cox: per-round scratch of the gradient and of cox-nloglik
+  RankScratch rank_scratch_;                    // rank:* and the ndcg / map metrics: per-call scratch
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1
@@ -206,6 +216,7 @@ class Booster {
 
   void configure();
   void check_label_ranges(const DMatrix* dtrain);
+  const RankGroups& rank_groups(DMatrix* dm, const char* what);   // dm's groups on the device; checks one weight per group
   void begin_update();                               // the model's layers become the trees to update; the model is emptied
   void refresh_one_iter(DMatrix* dtrain);            // one update round: the next layer refreshed / pruned into the model
   int layers() const { return (int)iteration_indptr_.size() - 1; }

@@ -124,11 +124,37 @@ int XGDMatrixCreateFromDense(const char* data, const char* config, DMatrixHandle
   *out = guard.release();
   API_END();
 }
+namespace {
+// query ids / group sizes: integral values only
+std::vector<int64_t> to_int64(const HostArray& h, const char* field) {
+  const size_t cnt = (size_t)h.n * h.m;
+  std::vector<int64_t> v(cnt);
+  const std::string& t = h.typestr;
+#define CONV(T) { const T* p = static_cast<const T*>(h.ptr); for (size_t i = 0; i < cnt; ++i) v[i] = (int64_t)p[i]; }
+#define CONVF(T) { const T* p = static_cast<const T*>(h.ptr); for (size_t i = 0; i < cnt; ++i) { \
+    B200_CHECK(std::isfinite(p[i]) && p[i] == std::floor(p[i]) && std::fabs((double)p[i]) < 9e18, std::string(field) + " must hold integers"); v[i] = (int64_t)p[i]; } }
+  if (t == "<i4") CONV(int32_t) else if (t == "<i8") CONV(int64_t) else if (t == "<u4") CONV(uint32_t) else if (t == "<u8") CONV(uint64_t)
+  else if (t == "<i2") CONV(int16_t) else if (t == "<u2") CONV(uint16_t) else if (t == "|i1") CONV(int8_t) else if (t == "|u1") CONV(uint8_t)
+  else if (t == "<f4") CONVF(float) else if (t == "<f8") CONVF(double)
+  else throw Error(std::string("array interface: unsupported typestr ") + t + " for " + field);
+#undef CONV
+#undef CONVF
+  return v;
+}
+std::vector<unsigned> to_group_sizes(const std::vector<int64_t>& v) {
+  std::vector<unsigned> out;
+  for (int64_t x : v) { B200_CHECK(x >= 0 && x <= 0x7fffffff, "group sizes must be in [0, 2^31)"); out.push_back((unsigned)x); }
+  return out;
+}
+}  // namespace
+
 int XGDMatrixSetInfoFromInterface(DMatrixHandle handle, const char* field, const char* data) {
   API_BEGIN();
   HostArray h = parse_array_interface(data);
-  std::vector<float> v = to_float32(h);
-  DM(handle)->set_float_info(field, v.data(), v.size());
+  const std::string f(field);
+  if (f == "qid") { std::vector<int64_t> q = to_int64(h, field); DM(handle)->set_qid(q.data(), q.size()); }
+  else if (f == "group") { std::vector<unsigned> g = to_group_sizes(to_int64(h, field)); DM(handle)->set_group_sizes(g.data(), g.size()); }
+  else { std::vector<float> v = to_float32(h); DM(handle)->set_float_info(field, v.data(), v.size()); }
   API_END();
 }
 
@@ -189,6 +215,7 @@ int XGDMatrixCreateFromURI(const char* config, DMatrixHandle* out) {
     if (st != 0) throw Error("CSV contains a field the device parser cannot decide exactly (blank line, > 19 digits or malformed number)");
   } else if (fmt == "libsvm") {
     std::vector<size_t> indptr{0}; std::vector<unsigned> indices; std::vector<float> vals, labels;
+    std::vector<int64_t> qid; size_t qid_rows = 0;     // rows that carry a qid token; all or none must
     for (auto& f : files) {
       std::ifstream in(f); std::string line;
       while (std::getline(in, line)) {
@@ -199,7 +226,13 @@ int XGDMatrixCreateFromURI(const char* config, DMatrixHandle* out) {
         while (ls >> tok) {
           size_t c = tok.find(':');
           if (c == std::string::npos) throw Error("Invalid libsvm token " + tok + " in " + f);
-          if (tok.compare(0, 4, "qid:") == 0) continue;
+          if (tok.compare(0, 4, "qid:") == 0) {
+            size_t used = 0; long long v = 0;
+            try { v = std::stoll(tok.substr(4), &used); } catch (...) { used = 0; }
+            B200_CHECK(used > 0 && used == tok.size() - 4 && qid.size() < labels.size(), "Invalid libsvm token " + tok + " in " + f);
+            qid.resize(labels.size() - 1, 0); qid.push_back(v); ++qid_rows;
+            continue;
+          }
           indices.push_back((unsigned)std::stoul(tok.substr(0, c))); vals.push_back(std::stof(tok.substr(c + 1)));
         }
         indptr.push_back(indices.size());
@@ -208,6 +241,10 @@ int XGDMatrixCreateFromURI(const char* config, DMatrixHandle* out) {
     if (labels.empty()) throw Error("libsvm input is empty");
     box->dm = DMatrix::from_csr(indptr.data(), indices.data(), vals.data(), indptr.size(), indices.size(), 0);
     box->dm->set_float_info("label", labels.data(), labels.size());
+    if (qid_rows) {
+      B200_CHECK(qid_rows == labels.size(), "libsvm input: " + std::to_string(qid_rows) + " of " + std::to_string(labels.size()) + " rows have a qid token; all or none must");
+      box->dm->set_qid(qid.data(), qid.size());
+    }
   } else throw Error("Unknown data format in URI: " + fmt);
   *out = guard.release();
   API_END();
@@ -229,6 +266,28 @@ int XGDMatrixSliceDMatrix(DMatrixHandle handle, const int* idxset, bst_ulong len
   *out = guard.release();
   API_END();
 }
+int XGDMatrixSliceDMatrixEx(DMatrixHandle handle, const int* idxset, bst_ulong len, DMatrixHandle* out, int allow_groups) {
+  API_BEGIN();
+  auto box = new DMatrixBox(); std::unique_ptr<DMatrixBox> guard(box);
+  box->dm = DM(handle)->slice(idxset, (int64_t)len, allow_groups != 0);
+  *out = guard.release();
+  API_END();
+}
+int XGDMatrixSetUIntInfo(DMatrixHandle handle, const char* field, const unsigned* array, bst_ulong len) {
+  API_BEGIN();
+  const std::string f(field);
+  if (f == "group_ptr") DM(handle)->set_group_ptr(std::vector<unsigned>(array, array + len));
+  else if (f == "group") DM(handle)->set_group_sizes(array, (size_t)len);
+  else throw Error("Unknown uint field name: " + f + " (group_ptr, group)");
+  API_END();
+}
+int XGDMatrixGetUIntInfo(DMatrixHandle handle, const char* field, bst_ulong* out_len, const unsigned** out_dptr) {
+  API_BEGIN();
+  B200_CHECK(std::string(field) == "group_ptr", std::string("Unknown uint field name: ") + field + " (group_ptr)");
+  const std::vector<unsigned>& v = DM(handle)->group_ptr; *out_len = v.size(); *out_dptr = v.data();
+  API_END();
+}
+int XGDMatrixSetGroup(DMatrixHandle handle, const unsigned* group, bst_ulong len) { API_BEGIN(); DM(handle)->set_group_sizes(group, (size_t)len); API_END(); }
 int XGDMatrixSetStrFeatureInfo(DMatrixHandle handle, const char* field, const char** features, bst_ulong size) {
   API_BEGIN();
   DMatrix* dm = DM(handle);
@@ -437,6 +496,7 @@ int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_
   DMatrix* dm = DM(handle);
   B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
   B200_CHECK(n_ranges >= 1 && row_bounds[0] == 0 && row_bounds[n_ranges] == dm->n, "XGB200DMatrixRankCuts: the ranges must cover the rows");
+  B200_CHECK(dm->weights.empty() || (int64_t)dm->weights.size() == dm->n, "XGB200DMatrixRankCuts: the weights must be one per row");
   for (int r = 0; r < n_ranges; ++r) B200_CHECK(row_bounds[r] <= row_bounds[r + 1], "XGB200DMatrixRankCuts: row_bounds must not decrease");
   HostCuts c;
   compute_rank_cuts_device(dm->X.p, dm->F, dm->weights.empty() ? nullptr : dm->d_weights.p, row_bounds, n_ranges, max_bin, dm->has_missing, &c,

@@ -96,7 +96,8 @@ enum Objective : int { kSquaredError = 0, kBinaryLogistic = 1, kRegLogistic = 2,
                        kSquaredLogError = 6, kPseudoHuber = 7, kPoisson = 8, kGamma = 9, kTweedie = 10, kHinge = 11,
                        kAft = 12, kCox = 13,         // survival objectives: own gradient kernels (survival.cu), not gradient_kernel
                        kAbsoluteError = 14,          // own gradient kernel and a leaf refresh after every tree (adaptive.cu)
-                       kQuantileError = 15 };        // likewise, one output (and one tree per round) per quantile_alpha
+                       kQuantileError = 15,          // likewise, one output (and one tree per round) per quantile_alpha
+                       kRankPairwise = 16, kRankNdcg = 17, kRankMap = 18 };   // over query groups: own gradient kernels (rank.cu)
 // prediction transform of an objective (upstream ObjFunction::PredTransform / ProbToMargin): 0 identity, 1 sigmoid / logit,
 // 2 exp / log (count:poisson, reg:gamma, reg:tweedie, survival:aft, survival:cox), 3 step at 0 (binary:hinge; its margin is the raw score)
 enum Transform : int { kTransformNone = 0, kTransformSigmoid = 1, kTransformExp = 2, kTransformHinge = 3 };
@@ -105,6 +106,7 @@ inline bool objective_is_log_link(int o) { return o == kPoisson || o == kGamma |
 inline bool objective_is_survival(int o) { return o == kAft || o == kCox; }
 // the objective sets each leaf of a grown tree to a quantile of its rows' residuals (upstream ObjFunction::Task().UpdateTreeLeaf())
 inline bool objective_is_adaptive(int o) { return o == kAbsoluteError || o == kQuantileError; }
+inline bool objective_is_rank(int o) { return o == kRankPairwise || o == kRankNdcg || o == kRankMap; }
 inline int objective_transform(int o) {
   if (o == kBinaryLogistic || o == kRegLogistic) return kTransformSigmoid;
   if (objective_is_log_link(o) || objective_is_survival(o)) return kTransformExp;
@@ -124,6 +126,10 @@ struct TrainParam {
   float huber_slope = 1.0f, tweedie_variance_power = 1.5f, poisson_max_delta_step = 0.7f;   // objective parameters (upstream defaults)
   int aft_dist = 0; float aft_sigma = 1.0f;     // survival:aft: aft_loss_distribution (survival.h AftDist), aft_loss_distribution_scale
   std::vector<float> quantile_alpha;            // reg:quantileerror: one output per entry (empty for every other objective)
+  // rank:* (upstream LambdaRankParam): lambdarank_num_pair_per_sample (the topk truncation K), ndcg_exp_gain,
+  // lambdarank_normalization, lambdarank_score_normalization, lambdarank_bias_norm (inert: lambdarank_unbiased is rejected)
+  // lambdarank_unbiased=true is read and written, and a model with it predicts, but it does not train
+  int rank_mean = 0, rank_unbiased = 0, rank_k = 32, rank_exp_gain = 1, rank_normalization = 1, rank_score_normalization = 1; float rank_bias_norm = 2.0f;
   // Outputs per row: margin columns, trees per round and layer (times num_parallel_tree), prediction columns.  num_class
   // itself is the class count of multi:* (softmax, merror / mlogloss) and 1 otherwise.
   int num_outputs() const { return objective == kQuantileError ? (int)quantile_alpha.size() : num_class; }

@@ -32,6 +32,21 @@ static void aft_params_from_json(const JValue& obj, std::map<std::string, std::s
   if (auto v = ap->get("aft_loss_distribution_scale")) (*raw)["aft_loss_distribution_scale"] = v->type == JValue::kString ? v->s : float_repr((float)v->as_double());
 }
 
+// rank:*'s lambdarank_param block into raw parameters (read, and checked, only under those objectives by configure); a field a
+// document leaves out keeps its default
+static const char* kLambdaRankFields[] = {"lambdarank_pair_method", "lambdarank_num_pair_per_sample", "lambdarank_unbiased", "lambdarank_bias_norm",
+                                          "ndcg_exp_gain", "lambdarank_normalization", "lambdarank_score_normalization"};
+static void rank_params_from_json(const JValue& obj, std::map<std::string, std::string>* raw) {
+  auto lp = obj.get("lambdarank_param");
+  if (!lp) return;
+  for (const char* f : kLambdaRankFields)
+    if (auto v = lp->get(f)) {
+      if (v->type == JValue::kString) (*raw)[f] = v->s;
+      else if (v->type == JValue::kBool) (*raw)[f] = v->b ? "1" : "0";
+      else (*raw)[f] = float_repr((float)v->as_double());
+    }
+}
+
 // quantile_alpha as "[0.1, 0.5, 0.9]": each value in the fewest %g digits that read back to the same float
 static std::string alpha_repr(const std::vector<float>& a) {
   std::string out = "[";
@@ -52,6 +67,11 @@ static void objective_params_to_json(JValue& obj, const TrainParam& p) {
     case kPseudoHuber: rp->set("huber_slope", S(float_repr(p.huber_slope))); obj.set("pseudo_huber_param", rp); break;
     case kGamma: case kHinge: case kCox: case kAbsoluteError: break;
     case kQuantileError: rp->set("quantile_alpha", S(alpha_repr(p.quantile_alpha))); obj.set("quantile_loss_param", rp); break;   // [UPSTREAM-RECALL]
+    case kRankPairwise: case kRankNdcg: case kRankMap: {      // every value a string, as upstream writes them [UPSTREAM-RECALL]
+      const std::string v[] = {p.rank_mean ? "mean" : "topk", std::to_string(p.rank_k), p.rank_unbiased ? "1" : "0", float_repr(p.rank_bias_norm), p.rank_exp_gain ? "1" : "0",
+                               p.rank_normalization ? "1" : "0", p.rank_score_normalization ? "1" : "0"};
+      for (int i = 0; i < 7; ++i) rp->set(kLambdaRankFields[i], S(v[i]));
+      obj.set("lambdarank_param", rp); break; }
     case kAft: {
       static const char* dist[] = {"normal", "logistic", "extreme"};
       rp->set("aft_loss_distribution", S(dist[p.aft_dist])); rp->set("aft_loss_distribution_scale", S(float_repr(p.aft_sigma)));
@@ -149,6 +169,7 @@ void Booster::model_from_json(const JValue& doc) {
   if (auto hp = obj.get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = std::to_string(v->as_double());
   aft_params_from_json(obj, &raw_params_);
   quantile_params_from_json(obj, &raw_params_);
+  rank_params_from_json(obj, &raw_params_);
   const JValue& lmp = learner.at("learner_model_param");
   num_feature_ = (int)lmp.at("num_feature").as_int();
   int nc = lmp.has("num_class") ? (int)lmp.at("num_class").as_int() : 0;
@@ -341,6 +362,7 @@ void Booster::config_from_json(const JValue& doc) {
     if (auto hp = o->get("pseudo_huber_param")) if (auto v = hp->get("huber_slope")) raw_params_["huber_slope"] = v->s;
     aft_params_from_json(*o, &raw_params_);
     quantile_params_from_json(*o, &raw_params_);
+    rank_params_from_json(*o, &raw_params_);
   }
   if (auto m = learner.get("metrics")) { eval_metrics_.clear(); for (auto& x : m->arr) eval_metrics_.push_back(x->at("name").s); }
   configured_ = false;

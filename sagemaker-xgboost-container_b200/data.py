@@ -67,8 +67,22 @@ def _load_csv(files, q):
     return data, y, w
 
 
+def _has_qid(fh, chunk=1 << 22):
+    """Whether the rest of the file holds a `qid:` token, read in fixed-size chunks (a token split by a chunk edge is kept whole by
+    carrying the last three bytes over)."""
+    tail = b""
+    while True:
+        block = fh.read(chunk)
+        if not block:
+            return False
+        if b"qid:" in tail + block[:3] or b"qid:" in block:
+            return True
+        tail = block[-3:]
+
+
 def _load_libsvm_fast(files):
-    """C parser of scikit-learn when the files are plain `label idx:val ...` lines (no per-row weights / qid)."""
+    """C parser of scikit-learn when the files are plain `label idx:val ...` lines (no per-row weights / qid: that parser would
+    drop a qid token on any line, so a file with one anywhere goes to the plain loop)."""
     try:
         from sklearn.datasets import load_svmlight_files
     except ImportError:
@@ -76,7 +90,9 @@ def _load_libsvm_fast(files):
     for f in files:
         with open(f, "rb") as fh:
             head = fh.readline().split(b"#", 1)[0].split()
-        if not head or b":" in head[0] or any(t.startswith(b"qid:") for t in head[1:2]):
+            if not head or b":" in head[0] or _has_qid(fh):
+                return None
+        if any(t.startswith(b"qid:") for t in head[1:]):
             return None
     try:
         out = load_svmlight_files(files, dtype=np.float32, zero_based=True)
@@ -90,12 +106,14 @@ def _load_libsvm_fast(files):
     return X, np.concatenate(ys).astype(np.float32), None
 
 
-def _load_libsvm(files, q):
+def _load_libsvm(files, q, with_qid=False):
+    """-> (CSR features, labels, weights | None), plus the qid of every row (int64, or None without qid tokens) with with_qid.
+    A file with qid tokens must carry one on every line; the query groups are the runs of equal consecutive qid."""
     import scipy.sparse as sp
     fast = _load_libsvm_fast(files)
     if fast is not None:
-        return fast
-    labels, weights, rows_ptr, cols, vals = [], [], [0], [], []
+        return fast + (None,) if with_qid else fast
+    labels, weights, rows_ptr, cols, vals, qids = [], [], [0], [], [], []
     has_weight = False
     for f in files:
         with open(f, "rb") as fh:
@@ -116,6 +134,12 @@ def _load_libsvm(files, q):
                 for tok in parts[1:]:
                     k, _, v = tok.partition(b":")
                     if k == b"qid":
+                        if len(qids) >= len(labels):
+                            raise XGBoostError("Invalid libsvm token %r in %s: a second qid on the line" % (tok, f))
+                        try:
+                            qids.extend([None] * (len(labels) - 1 - len(qids)) + [int(v)])
+                        except ValueError:
+                            raise XGBoostError("Invalid libsvm token %r in %s" % (tok, f))
                         continue
                     try:
                         cols.append(int(k))
@@ -127,11 +151,16 @@ def _load_libsvm(files, q):
         raise XGBoostError("libsvm input is empty")
     ncol = (max(cols) + 1) if cols else 0
     X = sp.csr_matrix((np.asarray(vals, np.float32), np.asarray(cols, np.int32), np.asarray(rows_ptr, np.int64)), shape=(len(labels), ncol))
-    return X, np.asarray(labels, np.float32), (np.asarray(weights, np.float32) if has_weight else None)
+    out = (X, np.asarray(labels, np.float32), (np.asarray(weights, np.float32) if has_weight else None))
+    n_qid = sum(1 for x in qids if x is not None)
+    if n_qid and n_qid != len(labels):
+        raise XGBoostError("libsvm input: %d of %d rows have a qid token; all or none must" % (n_qid, len(labels)))
+    return out + (np.asarray(qids, np.int64) if n_qid else None,) if with_qid else out
 
 
-def load_uri(uri):
-    """-> (features: ndarray | scipy CSR, label | None, weight | None)"""
+def load_uri(uri, with_qid=False):
+    """-> (features: ndarray | scipy CSR, label | None, weight | None), plus the per-row qid of a libsvm input (None without qid
+    tokens, and for CSV) with with_qid"""
     path, q = parse_uri(uri)
     fmt = q.get("format")
     if fmt is None:
@@ -139,9 +168,10 @@ def load_uri(uri):
         fmt = "csv" if ext == ".csv" else "libsvm"
     files = _list_files(path)
     if fmt == "csv":
-        return _load_csv(files, q)
+        out = _load_csv(files, q)
+        return out + (None,) if with_qid else out
     if fmt == "libsvm":
-        return _load_libsvm(files, q)
+        return _load_libsvm(files, q, with_qid)
     raise XGBoostError("Unknown data format in URI: %s" % fmt)
 
 

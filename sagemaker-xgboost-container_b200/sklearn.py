@@ -1,4 +1,4 @@
-"""scikit-learn style wrappers (`XGBRegressor`, `XGBClassifier`) over `train()` -- the subset of `xgboost.sklearn` that
+"""scikit-learn style wrappers (`XGBRegressor`, `XGBClassifier`, `XGBRanker`) over `train()` -- the subset of `xgboost.sklearn` that
 script-mode customer code in the container's test resources uses (test/resources/boston/single_machine_customer_script.py:54).
 """
 import json
@@ -157,6 +157,40 @@ class XGBClassifier(XGBModel):
             return XGBModel.predict(self, X, True, validate_features, base_margin, iteration_range)
         p = self.predict_proba(X, validate_features, base_margin, iteration_range)
         return np.argmax(p, axis=1)
+
+
+class XGBRanker(XGBModel):
+    """Learning to rank over query groups: the rows of each query are given by `group` (sizes) or `qid` (one id per row, sorted),
+    `sample_weight` holds one weight per group, and `predict` returns the ranking scores (margins)."""
+    _default_objective = "rank:ndcg"
+
+    def _ranking_dmatrix(self, X, y, group, qid, sample_weight=None, base_margin=None):
+        if (group is None) == (qid is None):
+            raise ValueError("XGBRanker needs exactly one of group and qid for every matrix it trains or evaluates on")
+        return DMatrix(X, label=y, weight=sample_weight, base_margin=base_margin, missing=self.missing, group=group, qid=qid)
+
+    def fit(self, X, y, *, group=None, qid=None, sample_weight=None, base_margin=None, eval_set=None, eval_group=None, eval_qid=None,
+            verbose=False, xgb_model=None, sample_weight_eval_set=None):
+        params = self.get_xgb_params()
+        if not str(params["objective"]).startswith("rank:"):
+            raise ValueError("XGBRanker takes a rank:* objective (got %s)" % params["objective"])
+        dtrain = self._ranking_dmatrix(X, y, group, qid, sample_weight, base_margin)
+        evals = []
+        for i, (Xe, ye) in enumerate(eval_set or []):
+            ge = eval_group[i] if eval_group is not None else None
+            qe = eval_qid[i] if eval_qid is not None else None
+            we = sample_weight_eval_set[i] if sample_weight_eval_set else None
+            evals.append((self._ranking_dmatrix(Xe, ye, ge, qe, we), "validation_%d" % i))
+        self.evals_result_ = {}
+        model = xgb_model.get_booster() if isinstance(xgb_model, XGBModel) else xgb_model
+        self._Booster = train(params, dtrain, self.get_num_boosting_rounds(), evals=evals, early_stopping_rounds=self.early_stopping_rounds,
+                              evals_result=self.evals_result_, custom_metric=self.eval_metric if callable(self.eval_metric) else None,
+                              verbose_eval=verbose, xgb_model=model, callbacks=self.callbacks)
+        self.n_features_in_ = dtrain.num_col()
+        return self
+
+    def predict(self, X, output_margin=False, validate_features=True, base_margin=None, iteration_range=None):
+        return XGBModel.predict(self, X, True, validate_features, base_margin, iteration_range)
 
 
 class _RandomForest:
