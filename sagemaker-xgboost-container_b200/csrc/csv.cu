@@ -7,16 +7,21 @@
 // fields, a field is what Python's float() accepts (decimal, exponent, inf/nan in any case).  Values take the same two
 // roundings: text -> nearest double (Clinger's exact fast path: <= 19 significant digits below 2^53 and |exp10| <= 22,
 // one IEEE multiply or divide) -> nearest float32 (what xgb.DMatrix does with a float64 array).  A field outside the fast
-// path (or malformed) raises a flag and the caller falls back to the host parser, so results never differ.
+// path (or malformed) raises a flag and the caller falls back to the host parser, so results never differ.  The byte-level
+// code (field literals, newline count, libsvm token walk) is in text_parse.h, shared with a CPU sweep of the tests.
 //
-// Kernels: (1) newline positions (flag + CUB select), (2) one thread per row walks its fields.  Text is read once from
-// HBM (L1-cached byte loads; rows are short and contiguous per thread).
+// Kernels: (1) newline count, (2) newline positions (CUB select), (3) one thread per row walks its fields.  Text is read
+// once from HBM (L1-cached byte loads; rows are short and contiguous per thread).  The row table of (2) has as many entries
+// as (1) counted only if the two agree: the parse kernels compare the select's own count with it before they read a row
+// bound, and on a mismatch write kRowTableMismatch and return.  The host raises on that code (a device bug, not a body the
+// host route should see), without an extra synchronisation.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cub/cub.cuh>
 #include <cstring>
 #include "booster.h"
+#include "text_parse.h"
 
 namespace b200 {
 
@@ -25,69 +30,26 @@ struct IsNewline {
   __host__ __device__ bool operator()(const int64_t& i) const { return text[i] == '\n'; }
 };
 
-__device__ __forceinline__ bool is_space(char c) { return c == ' ' || c == '\t' || c == '\r'; }
+// err code of a row table whose select count differs from the newline count (never a property of the body)
+constexpr int kRowTableMismatch = 16;
 
-__device__ __forceinline__ char lower(char c) { return (c >= 'A' && c <= 'Z') ? (char)(c + 32) : c; }
-
-// parse [p, e) as a Python-float literal; returns false when the token is malformed or needs the slow path
-__device__ bool parse_field(const char* p, const char* e, float* out) {
-  while (p < e && is_space(*p)) ++p;
-  while (e > p && is_space(e[-1])) --e;
-  if (p == e) { *out = __int_as_float(0x7fc00000); return true; }                 // empty field -> NaN (encoder.py:31-32)
-  bool neg = false;
-  if (*p == '+' || *p == '-') { neg = *p == '-'; ++p; if (p == e) return false; }
-  const int len = (int)(e - p);
-  if (len == 3 && lower(p[0]) == 'n' && lower(p[1]) == 'a' && lower(p[2]) == 'n') { *out = __int_as_float(0x7fc00000); return true; }
-  if ((len == 3 && lower(p[0]) == 'i' && lower(p[1]) == 'n' && lower(p[2]) == 'f') ||
-      (len == 8 && lower(p[0]) == 'i' && lower(p[1]) == 'n' && lower(p[2]) == 'f' && lower(p[3]) == 'i' && lower(p[4]) == 'n' && lower(p[5]) == 'i' &&
-       lower(p[6]) == 't' && lower(p[7]) == 'y')) { *out = neg ? __int_as_float(0xff800000) : __int_as_float(0x7f800000); return true; }
-  unsigned long long mant = 0; int digits = 0, sig = 0, exp10 = 0; bool any = false, dropped = false;
-  while (p < e && *p >= '0' && *p <= '9') {
-    any = true;
-    if (sig < 19) { mant = mant * 10ull + (unsigned)(*p - '0'); if (mant != 0) ++sig; } else { ++exp10; if (*p != '0') dropped = true; }
-    ++p; ++digits;
-  }
-  if (p < e && *p == '.') {
-    ++p;
-    while (p < e && *p >= '0' && *p <= '9') {
-      any = true;
-      if (sig < 19) { mant = mant * 10ull + (unsigned)(*p - '0'); if (mant != 0) ++sig; --exp10; } else if (*p != '0') dropped = true;
-      ++p;
-    }
-  }
-  if (!any) return false;
-  if (p < e && (*p == 'e' || *p == 'E')) {
-    ++p; bool eneg = false;
-    if (p < e && (*p == '+' || *p == '-')) { eneg = *p == '-'; ++p; }
-    if (p == e) return false;
-    int ev = 0;
-    while (p < e && *p >= '0' && *p <= '9') { if (ev < 100000) ev = ev * 10 + (*p - '0'); ++p; }
-    exp10 += eneg ? -ev : ev;
-  }
-  if (p != e) return false;                                                       // trailing junk (Python's float() would raise)
-  if (mant == 0) { *out = neg ? -0.0f : 0.0f; return true; }
-  if (dropped || mant >= (1ull << 53) || exp10 > 22 || exp10 < -22) return false;   // outside the exact fast path: host parser decides
-  const double p10[23] = {1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
-  double d = (double)mant;                                                        // exact: mant < 2^53
-  d = exp10 >= 0 ? d * p10[exp10] : d / p10[-exp10];                              // one correctly rounded IEEE operation
-  *out = (float)(neg ? -d : d);
-  return true;
-}
-
-// one thread per row: row r covers [start, end) where start = r ? nl[r-1] + 1 : 0 and end = r < n-1 ? nl[r] : len
-__global__ void __launch_bounds__(256) csv_parse_kernel(const char* text, int64_t len, const int64_t* nl, int64_t n, int F, char delim, float* out, int* err) {
+// one thread per row: row r covers [start, end) where start = r ? nl[r-1] + 1 : 0 and end = r < n-1 ? nl[r] : len;
+// num_nl is the select's count of the entries it wrote into nl
+__global__ void __launch_bounds__(256) csv_parse_kernel(const char* text, int64_t len, const int64_t* nl, const long long* num_nl, int64_t n, int F,
+                                                        char delim, float* out, int* err) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
+  if (*num_nl != n - 1) { if (r == 0) atomicMax(err, kRowTableMismatch); return; }
   const char* p = text + (r ? nl[r - 1] + 1 : 0);
   const char* e = text + (r < n - 1 ? nl[r] : len);
   float* o = out + r * F;
   int f = 0;
   const char* tok = p;
   for (const char* q = p;; ++q) {
-    if (q == e || *q == delim) {
+    if (q >= e || *q == delim) {
       if (f < F) { float v; if (!parse_field(tok, q, &v)) { atomicMax(err, 2); v = 0.f; } o[f] = v; }
       ++f; tok = q + 1;
-      if (q == e) break;
+      if (q >= e) break;
     }
   }
   if (f != F) atomicMax(err, 1);                                                   // ragged row
@@ -103,8 +65,7 @@ __global__ void __launch_bounds__(256) count_newlines_kernel(const char* text, i
     const unsigned ws[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const unsigned x = ws[k] ^ 0x0a0a0a0au;                                     // zero byte <=> '\n'
-      c += __popc(((x - 0x01010101u) & ~x & 0x80808080u));
+      c += newlines_in_word(ws[k]);
     }
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) for (int64_t i = nvec * 16; i < len; ++i) c += text[i] == '\n';
@@ -121,6 +82,44 @@ __global__ void fill_value_kernel(float* X, int64_t count, float v) {
 struct CsvScratch { DevBuf<char> text; DevBuf<int64_t> nl; DevBuf<unsigned char> tmp; DevBuf<unsigned long long> cnt; DevBuf<int> err; };
 static CsvScratch& csv_scratch() { static thread_local CsvScratch s; return s; }
 
+// the select's count of newline positions, in device memory (zero when no select ran: nnl == 0)
+static const long long* newline_select_count(CsvScratch& sc) { return reinterpret_cast<const long long*>(sc.cnt.p + 1); }
+
+// newline count, then (for nnl > 0) their positions into sc.nl; the count is on the host when this returns.  lap(stage)
+// after each of the two steps (profiling).
+template <class Lap>
+static unsigned long long newline_table(CsvScratch& sc, int64_t len, cudaStream_t s, Lap&& lap) {
+  CUDA_OK(cudaMemsetAsync(sc.cnt.p, 0, 16, s));
+  count_newlines_kernel<<<engine_num_sms() * 8, 256, 0, s>>>(sc.text.p, len, sc.cnt.p); ++g_kernel_launches;
+  CUDA_OK(cudaGetLastError());
+  unsigned long long nnl = 0;
+  CUDA_OK(cudaMemcpyAsync(&nnl, sc.cnt.p, sizeof(nnl), cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  lap("count newlines");
+  sc.nl.ensure((size_t)nnl + 1);
+  if (nnl > 0) {                                                                   // positions of the newlines, in order
+    cub::CountingInputIterator<int64_t> idx(0);
+    IsNewline pred{sc.text.p};
+    size_t tmp_bytes = 0;
+    long long* d_num = reinterpret_cast<long long*>(sc.cnt.p + 1);
+    CUDA_OK(cub::DeviceSelect::If(nullptr, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
+    sc.tmp.ensure(tmp_bytes);
+    CUDA_OK(cub::DeviceSelect::If(sc.tmp.p, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
+    ++g_kernel_launches;
+  }
+  lap("newline positions");
+  return nnl;
+}
+
+// a parse kernel found the row table inconsistent with the newline count: a device bug, so no host-route fallback
+[[noreturn]] static void raise_row_table_mismatch(CsvScratch& sc, unsigned long long nnl, cudaStream_t s) {
+  long long selected = 0;
+  CUDA_OK(cudaMemcpyAsync(&selected, newline_select_count(sc), sizeof selected, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  throw Error("text parser: the newline count (" + std::to_string(nnl) + ") differs from the newline positions found (" +
+              std::to_string(selected) + ")");
+}
+
 // returns 0 = ok, 1 = ragged rows, 2 = a field outside the exact fast path / malformed (caller falls back to the host parser)
 int parse_csv_device(const char* h_text, int64_t len, char delim, int F, int64_t* n_rows_out, DevBuf<float>* X, cudaStream_t s) {
   CsvScratch& sc = csv_scratch();
@@ -136,36 +135,20 @@ int parse_csv_device(const char* h_text, int64_t len, char delim, int F, int64_t
   sc.text.ensure((size_t)len + 16); sc.cnt.ensure(2); sc.err.ensure(1);
   CUDA_OK(cudaMemcpyAsync(sc.text.p, h_text, (size_t)len, cudaMemcpyHostToDevice, s));
   lap("h2d of the text");
-  CUDA_OK(cudaMemsetAsync(sc.cnt.p, 0, 16, s));
   CUDA_OK(cudaMemsetAsync(sc.err.p, 0, 4, s));
-  count_newlines_kernel<<<engine_num_sms() * 8, 256, 0, s>>>(sc.text.p, len, sc.cnt.p); ++g_kernel_launches;
-  CUDA_OK(cudaGetLastError());
-  unsigned long long nnl = 0;
-  CUDA_OK(cudaMemcpyAsync(&nnl, sc.cnt.p, sizeof(nnl), cudaMemcpyDeviceToHost, s));
-  CUDA_OK(cudaStreamSynchronize(s));
-  lap("count newlines");
+  const unsigned long long nnl = newline_table(sc, len, s, lap);
   const int64_t n = (int64_t)nnl + 1;
   *n_rows_out = n;
-  sc.nl.ensure((size_t)nnl + 1);
-  if (nnl > 0) {                                                                   // positions of the newlines, in order
-    cub::CountingInputIterator<int64_t> idx(0);
-    IsNewline pred{sc.text.p};
-    size_t tmp_bytes = 0;
-    long long* d_num = reinterpret_cast<long long*>(sc.cnt.p + 1);
-    CUDA_OK(cub::DeviceSelect::If(nullptr, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
-    sc.tmp.ensure(tmp_bytes);
-    CUDA_OK(cub::DeviceSelect::If(sc.tmp.p, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
-    ++g_kernel_launches;
-  }
-  lap("newline positions");
   X->alloc((size_t)n * F);
   lap("alloc X");
-  csv_parse_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(sc.text.p, len, sc.nl.p, n, F, delim, X->p, sc.err.p); ++g_kernel_launches;
+  csv_parse_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(sc.text.p, len, sc.nl.p, newline_select_count(sc), n, F, delim, X->p, sc.err.p);
+  ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());
   int err = 0;
   CUDA_OK(cudaMemcpyAsync(&err, sc.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
   lap("parse kernel");
+  if (err == kRowTableMismatch) raise_row_table_mismatch(sc, nnl, s);
   return err;
 }
 
@@ -180,39 +163,25 @@ int parse_csv_device(const char* h_text, int64_t len, char delim, int F, int64_t
 struct LibsvmRange { int min_idx, max_idx; unsigned long long entries; int err; int last_row_entries; };
 
 template <bool kFill>
-__global__ void __launch_bounds__(256) libsvm_kernel(const char* text, int64_t len, const int64_t* nl, int64_t n, LibsvmRange* rg, int whitespace_mode,
-                                                     float* X, int F, int shift, float absent) {
+__global__ void __launch_bounds__(256) libsvm_kernel(const char* text, int64_t len, const int64_t* nl, const long long* num_nl, int64_t n, LibsvmRange* rg,
+                                                     int whitespace_mode, float* X, int F, int shift, float absent) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
+  if (*num_nl != n - 1) { if (r == 0) atomicMax(&rg->err, kRowTableMismatch); return; }
   const char* p = text + (r ? nl[r - 1] + 1 : 0);
   const char* e = text + (r < n - 1 ? nl[r] : len);
-  int lo = 0x7fffffff, hi = -1, cnt = 0; bool bad = false;
-  const char* q = p;
-  while (q < e) {
-    // token = run of non-separator characters; serve_utils splits on ' ' only, the encoder on any whitespace
-    while (q < e && (*q == ' ' || (whitespace_mode && (*q == '\t' || *q == '\r' || *q == '\f' || *q == '\v')))) ++q;
-    const char* t = q;
-    while (q < e && !(*q == ' ' || (whitespace_mode && (*q == '\t' || *q == '\r' || *q == '\f' || *q == '\v')))) ++q;
-    if (t == q) break;
-    const char* c = t; while (c < q && *c != ':') ++c;
-    if (c == q) continue;                                                        // no colon: the label (or junk both routes ignore)
-    int idx = 0; bool ok = c > t && (c - t) <= 9;
-    for (const char* d = t; d < c && ok; ++d) { if (*d < '0' || *d > '9') ok = false; else idx = idx * 10 + (*d - '0'); }
-    const char* v = c + 1;
-    for (const char* d = v; d < q && ok; ++d) if (*d == ':' || *d == '_') ok = false;       // second colon / digit separators: host decides
-    float val = 0.f;
-    if (ok) { if (v == q || !parse_field(v, q, &val)) ok = false; else if (v < q && (is_space(*v) || is_space(q[-1]))) ok = false; }
-    if (!ok) { bad = true; continue; }
+  int lo = 0x7fffffff, hi = -1, cnt = 0;
+  const bool good = libsvm_line(p, e, whitespace_mode, [&](int idx, float val) {
     ++cnt; lo = min(lo, idx); hi = max(hi, idx);
-    if (kFill) {
-      float* slot = X + r * F + (idx - shift);
-      // serve_utils' COO -> CSR conversion SUMS an index repeated inside a line (the encoder's dict keeps the last one, which is
-      // what this sequential walk does): with NaN as the fill value a slot that is no longer NaN has been written before
-      if (!whitespace_mode && (val != val || *slot == *slot)) bad = true;
-      *slot = val;
-    }
-  }
-  if (bad) atomicMax(&rg->err, 2);
+    if (!kFill) return true;
+    float* slot = X + r * F + (idx - shift);
+    // serve_utils' COO -> CSR conversion SUMS an index repeated inside a line (the encoder's dict keeps the last one, which is
+    // what this sequential walk does): with NaN as the fill value a slot that is no longer NaN has been written before
+    const bool fresh = whitespace_mode || (val == val && *slot != *slot);
+    *slot = val;
+    return fresh;
+  });
+  if (!good) atomicMax(&rg->err, 2);
   if (!kFill) {
     if (cnt) { atomicMin(&rg->min_idx, lo); atomicMax(&rg->max_idx, hi); atomicAdd(&rg->entries, (unsigned long long)cnt); }
     if (r == n - 1) rg->last_row_entries = cnt;
@@ -224,34 +193,19 @@ int parse_libsvm_device(const char* h_text, int64_t len, int whitespace_mode, fl
   CsvScratch& sc = csv_scratch();
   sc.text.ensure((size_t)len + 16); sc.cnt.ensure(2); sc.err.ensure(16);
   CUDA_OK(cudaMemcpyAsync(sc.text.p, h_text, (size_t)len, cudaMemcpyHostToDevice, s));
-  CUDA_OK(cudaMemsetAsync(sc.cnt.p, 0, 16, s));
-  count_newlines_kernel<<<engine_num_sms() * 8, 256, 0, s>>>(sc.text.p, len, sc.cnt.p); ++g_kernel_launches;
-  CUDA_OK(cudaGetLastError());
-  unsigned long long nnl = 0;
-  CUDA_OK(cudaMemcpyAsync(&nnl, sc.cnt.p, sizeof(nnl), cudaMemcpyDeviceToHost, s));
-  CUDA_OK(cudaStreamSynchronize(s));
+  const unsigned long long nnl = newline_table(sc, len, s, [](const char*) {});
   const int64_t n = (int64_t)nnl + 1;
-  sc.nl.ensure((size_t)nnl + 1);
-  if (nnl > 0) {
-    cub::CountingInputIterator<int64_t> idx(0);
-    IsNewline pred{sc.text.p};
-    size_t tmp_bytes = 0;
-    long long* d_num = reinterpret_cast<long long*>(sc.cnt.p + 1);
-    CUDA_OK(cub::DeviceSelect::If(nullptr, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
-    sc.tmp.ensure(tmp_bytes);
-    CUDA_OK(cub::DeviceSelect::If(sc.tmp.p, tmp_bytes, idx, sc.nl.p, d_num, len, pred, s));
-    ++g_kernel_launches;
-  }
   static_assert(sizeof(LibsvmRange) <= 16 * sizeof(int), "range block lives in the err scratch");
   LibsvmRange* rg = reinterpret_cast<LibsvmRange*>(sc.err.p);
   LibsvmRange init{0x7fffffff, -1, 0ull, 0, 0};
   CUDA_OK(cudaMemcpyAsync(rg, &init, sizeof init, cudaMemcpyHostToDevice, s));
   const unsigned grid = (unsigned)((n + 255) / 256);
-  libsvm_kernel<false><<<grid, 256, 0, s>>>(sc.text.p, len, sc.nl.p, n, rg, whitespace_mode, nullptr, 0, 0, absent); ++g_kernel_launches;
+  libsvm_kernel<false><<<grid, 256, 0, s>>>(sc.text.p, len, sc.nl.p, newline_select_count(sc), n, rg, whitespace_mode, nullptr, 0, 0, absent); ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());
   LibsvmRange h{};
   CUDA_OK(cudaMemcpyAsync(&h, rg, sizeof h, cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));
+  if (h.err == kRowTableMismatch) raise_row_table_mismatch(sc, nnl, s);
   if (h.err != 0) return 2;
   if (h.entries == 0) return 3;
   if (!whitespace_mode && h.last_row_entries == 0) return 2;      // csr_matrix((data, (row, col))) infers its row count: trailing empty lines vanish there
@@ -260,7 +214,7 @@ int parse_libsvm_device(const char* h_text, int64_t len, int whitespace_mode, fl
   B200_CHECK((double)n * (double)F < 4e9, "libsvm body: the dense matrix would exceed 4e9 entries");
   X->alloc((size_t)n * F);
   fill_value_kernel<<<engine_num_sms() * 8, 256, 0, s>>>(X->p, (int64_t)n * F, absent); ++g_kernel_launches;
-  libsvm_kernel<true><<<grid, 256, 0, s>>>(sc.text.p, len, sc.nl.p, n, rg, whitespace_mode, X->p, F, shift, absent); ++g_kernel_launches;
+  libsvm_kernel<true><<<grid, 256, 0, s>>>(sc.text.p, len, sc.nl.p, newline_select_count(sc), n, rg, whitespace_mode, X->p, F, shift, absent); ++g_kernel_launches;
   CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaMemcpyAsync(&h, rg, sizeof h, cudaMemcpyDeviceToHost, s));
   CUDA_OK(cudaStreamSynchronize(s));

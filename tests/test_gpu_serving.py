@@ -22,25 +22,47 @@ def _device_matrix(xgb, payload):
     return be.dmatrix_get_raw(d.handle).reshape(n, F), d
 
 
-def test_csv_payload_device_parse_is_bit_identical_to_the_container_route(xgb):
-    rng = np.random.default_rng(7)
+def _mixed_body(formats, specials, seed=7):
+    rng = np.random.default_rng(seed)
     n, F = 20000, 28
     X = rng.standard_normal((n, F)) * np.exp(rng.uniform(-20, 20, size=(n, F)))
     lines = []
     for r in range(n):
-        fmt = ["%.6g", "%.17g", "%.3e", "%d", "%.9f"][r % 5]
+        fmt = formats[r % len(formats)]
         vals = [(fmt % (int(v) if fmt == "%d" else v)) for v in X[r]]
         if r % 97 == 0:
             vals[r % F] = ""                     # empty field -> NaN
         if r % 101 == 0:
-            vals[(r + 3) % F] = ["nan", "NaN", "inf", "-inf", "+1.5", " 2.5 ", "-0", "1e-45", "3.4028235e38", "1e39"][(r // 101) % 10]
+            vals[(r + 3) % F] = specials[(r // 101) % len(specials)]
         lines.append(",".join(vals))
-    payload = "\n".join(lines)
-    got, d = _device_matrix(xgb, payload)
-    ref = _reference_route(payload)
+    return "\n".join(lines)
+
+
+def _assert_same(got, ref):
     assert got.shape == ref.shape
-    assert np.array_equal(got.view(np.uint32)[~np.isnan(ref)], ref.view(np.uint32)[~np.isnan(ref)])          # bit-exact, incl. -0, denormals, inf
+    assert np.array_equal(got.view(np.uint32)[~np.isnan(ref)], ref.view(np.uint32)[~np.isnan(ref)])          # bit-exact, incl. -0, inf
     assert np.array_equal(np.isnan(got), np.isnan(ref))
+
+
+def test_csv_payload_device_parse_is_bit_identical_to_the_container_route(xgb):
+    """Every field inside the exact fast path: the device must take the whole body (status 0), not hand it to the host route."""
+    payload = _mixed_body(["%.6g", "%.9g", "%.3e", "%d", "%.4f"], ["nan", "NaN", "inf", "-inf", "+1.5", " 2.5 ", "-0", "1e-22", "1E+05", ".5"])
+    be = xgb.get_backend()
+    h, st = be.dmatrix_from_csv(payload, ",")
+    assert st == 0
+    d = xgb.DMatrix._from_handle(h)
+    _assert_same(be.dmatrix_get_raw(d.handle).reshape(d.num_row(), d.num_col()), _reference_route(payload))
+
+
+def test_csv_payload_outside_the_fast_path_takes_the_host_route_bit_identically(xgb):
+    """%.17g and %.9f fields (mantissas >= 2^53, exponents beyond +-22) and literals that overflow float32: status 2 on the
+    device, then the container's own route through serving.csv_to_dmatrix."""
+    payload = _mixed_body(["%.6g", "%.17g", "%.3e", "%d", "%.9f"], ["nan", "inf", "-0", "1e-45", "3.4028235e38", "1e39"])
+    h, st = xgb.get_backend().dmatrix_from_csv(payload, ",")
+    assert st == 2 and h is None
+    got, _ = _device_matrix(xgb, payload)
+    with np.errstate(over="ignore"):
+        _assert_same(got, _reference_route(payload))
 
 
 def test_csv_semicolon_single_row_and_single_column(xgb):
