@@ -1,6 +1,7 @@
 // auc.cu -- binary ROC-AUC on the device (sort based), checked on hardware against sklearn.metrics.roc_auc_score
-// (tests/test_gpu_parity.py::test_auc_matches_sklearn).  `auc` is the one metric of the container's HPO list that the container does not compute
-// itself (algorithm_mode/train_utils.py:45-76 routes accuracy/f1/rmse/mae... to feval, `auc` stays native).
+// (tests/test_gpu_parity.py::test_auc_matches_sklearn).  Like `aucpr`, `auc` is a metric of the container's HPO list that the
+// container does not compute itself (algorithm_mode/train_utils.py:45-76 routes accuracy/f1/rmse/mae... to feval; `auc` and
+// `aucpr` stay native).  This file computes binary `auc` on a one-output model; `aucpr` and one-vs-rest `auc` are curve.cu's.
 // Definition restated from upstream src/metric/auc.cc (BinaryROCAUC): predictions sorted descending, one trapezoid per
 // group of tied predictions, area / (sum_w_pos * sum_w_neg); distributed: sum of local areas / sum of local pos*neg products.
 #include <cub/cub.cuh>

@@ -1374,9 +1374,35 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
       }
       B200_CHECK(mname.rfind("pre@", 0) != 0 && mname != "pre", "metric " + mname + ": the pre / pre@k ranking metric is not implemented on the CUDA hist path (ndcg and map are)");
       check_row_weights(dm);
+      const bool multiclass = (param_.objective == kSoftprob || param_.objective == kSoftmax) && param_.num_class > 1;
+      if (base == "aucpr" || (base == "auc" && multiclass)) {
+        // curve.cu: binary aucpr, and auc / aucpr one-vs-rest over the softmax probabilities (DESIGN.md "AUC family")
+        check_labels(dm);                        // survival:aft skips the check above; its matrices may carry bounds only
+        B200_CHECK(!objective_is_rank(param_.objective) || dm->group_ptr.empty(), mname + " under a rank:* objective on a DMatrix with query groups (ranking " +
+                   (base == "auc" ? "AUC" : "PR-AUC") + ") is not implemented on the CUDA hist path");
+        B200_CHECK(multiclass || param_.num_outputs() <= 1, mname + " reads one output per row or the softmax probabilities of multi:softprob / multi:softmax; a " +
+                   objective_name_ + " model with " + std::to_string(param_.num_outputs()) + " outputs per row is not supported");
+        const int pr = base == "aucpr" ? 1 : 0, K = multiclass ? param_.num_class : 0;
+        const int logistic = (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic) ? 1 : 0;
+        const int len = curve_metric_local(c.margin.p, dm->d_labels.p, ma.weight, dm->n, K, logistic, pr, &curve_scratch_, s);
+        Comm::get().allreduce_sum_f64(curve_scratch_.vec.p, len, s);
+        curve_metric_finish(K, pr, Comm::get().world(), &curve_scratch_, dsum_.p, s);
+        double h[4];
+        CUDA_OK(cudaMemcpyAsync(h, dsum_.p, 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
+        Comm::get().sync_stream(s);
+        if (pr && !K) {
+          B200_CHECK(h[3] == 0.0, "Check failed: label must be in [0, 1] for aucpr (binary PR-AUC reads the label as the positive share of a row)");
+          B200_CHECK(h[1] > 0.0 && h[2] > 0.0, "Check failed: !auc_error AUC: the dataset only contains pos or neg samples");
+        }
+        char buf[64]; snprintf(buf, sizeof buf, "%.17g", h[0]);
+        out += "\t" + names[i] + "-" + mname + ":" + (std::isnan(h[0]) ? std::string("nan") : std::string(buf));
+        continue;
+      }
       if (base == "auc") {
         // validated on hardware against sklearn.metrics.roc_auc_score (tests/test_gpu_parity.py::test_auc_matches_sklearn)
-        B200_CHECK(param_.num_outputs() <= 1, "auc is implemented for binary / regression-style predictions only");
+        check_labels(dm);                        // survival:aft skips the check above; its matrices may carry bounds only
+        B200_CHECK(param_.num_outputs() <= 1, "auc reads one output per row or the softmax probabilities of multi:softprob / multi:softmax; a " +
+                   objective_name_ + " model with " + std::to_string(param_.num_outputs()) + " outputs per row is not supported");
         B200_CHECK(!objective_is_rank(param_.objective) || dm->group_ptr.empty(), "auc under a rank:* objective on a DMatrix with query groups (ranking AUC) is not implemented on the CUDA hist path");
         const int logistic = (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic) ? 1 : 0;
         compute_auc_device(c.margin.p, dm->d_labels.p, dm->weights.empty() ? nullptr : dm->d_weights.p, dm->n, logistic, dsum_.p, s);
@@ -1425,7 +1451,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         else if (base == "poisson-nloglik") ma.metric = kMetricPoissonNll; else if (base == "gamma-nloglik") ma.metric = kMetricGammaNll;
         else if (base == "gamma-deviance") ma.metric = kMetricGammaDeviance;
         else if (base == "tweedie-nloglik") { ma.metric = kMetricTweedieNll; if (ma.aux == 0.0f) throw Error("tweedie-nloglik needs its variance power: tweedie-nloglik@rho"); }
-        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, quantile, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik, ndcg, ndcg@k, map, map@k)");
+        else throw Error("Unknown metric function " + mname + " (the CUDA hist path implements rmse, mse, rmsle, mae, quantile, mape, mphe, logloss, error, error@t, merror, mlogloss, auc, aucpr, poisson-nloglik, gamma-nloglik, gamma-deviance, tweedie-nloglik@rho, aft-nloglik, interval-regression-accuracy, cox-nloglik, ndcg, ndcg@k, map, map@k)");
         if (param_.objective == kLogitRaw && (ma.metric == kMetricLogloss || ma.metric == kMetricError)) ma.is_logistic = 1;
         if ((ma.metric == kMetricMerror || ma.metric == kMetricMlogloss)) B200_CHECK(param_.num_class > 1, "Check failed: preds.size() == info.labels_.size() : label and prediction size not match, hint: use merror or mlogloss for multi-class classification");
         CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));

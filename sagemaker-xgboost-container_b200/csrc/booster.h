@@ -4,6 +4,7 @@
 #include <memory>
 #include <string>
 #include <vector>
+#include "curve.h"
 #include "engine.h"
 #include "grow.h"
 #include "json.h"
@@ -205,6 +206,7 @@ class Booster {
   DevBuf<double> dsum_;                         // device sums of the metrics and of the base-score stump
   CoxScratch cox_scratch_;                      // survival:cox: per-round scratch of the gradient and of cox-nloglik
   RankScratch rank_scratch_;                    // rank:* and the ndcg / map metrics: per-call scratch
+  CurveScratch curve_scratch_;                  // aucpr and multi-class auc: per-call scratch, grown on first use
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1

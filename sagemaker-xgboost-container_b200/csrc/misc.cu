@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <utility>
+#include "curve.h"
 #include "engine.h"
 #include "misc.h"
 #include "rng.h"
@@ -17,6 +18,16 @@ __device__ __forceinline__ float sigmoidf_xgb(float x) {
   x = fminf(-x, 88.7f);
   float denom = expf(x) + 1.0f + kEps;
   return 1.0f / denom;
+}
+// softmax of the margins p[0, K): returns the sum of expf(p[k] - wmax) over k, with wmax the largest margin; class k's
+// probability is expf(p[k] - wmax) / sum (predict() and the multi-class auc / aucpr scores)
+__device__ __forceinline__ float softmax_sum(const float* p, int K, float* wmax_out) {
+  float wmax = p[0];
+  for (int k = 1; k < K; ++k) if (p[k] > wmax) wmax = p[k];
+  float wsum = 0.f;
+  for (int k = 0; k < K; ++k) wsum += expf(p[k] - wmax);
+  *wmax_out = wmax;
+  return wsum;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -327,12 +338,24 @@ __global__ void __launch_bounds__(256) transform_kernel(float* m, int64_t n, int
   else if (objective == kHinge) m[r] = m[r] > 0.0f ? 1.0f : 0.0f;
   else if (objective == kSoftprob || objective == kSoftmax) {
     float* p = m + r * K;
-    float wmax = p[0]; int arg = 0;
-    for (int k = 1; k < K; ++k) if (p[k] > wmax) { wmax = p[k]; arg = k; }
-    if (objective == kSoftmax) { out_class[r] = (float)arg; return; }
-    float wsum = 0.f;
-    for (int k = 0; k < K; ++k) { p[k] = expf(p[k] - wmax); wsum += p[k]; }
-    for (int k = 0; k < K; ++k) p[k] /= wsum;
+    if (objective == kSoftmax) {
+      float wmax = p[0]; int arg = 0;
+      for (int k = 1; k < K; ++k) if (p[k] > wmax) { wmax = p[k]; arg = k; }
+      out_class[r] = (float)arg; return;
+    }
+    float wmax; const float wsum = softmax_sum(p, K, &wmax);
+    for (int k = 0; k < K; ++k) p[k] = expf(p[k] - wmax) / wsum;
+  }
+}
+
+// the scores of the curve metrics (curve.h): computed here, with this file's flags, so they are predict()'s values bit for bit
+__global__ void __launch_bounds__(256) curve_scores_kernel(const float* margin, int64_t n, int K, int c, int logistic, float* key, int* iota) {
+  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (int64_t)gridDim.x * blockDim.x) {
+    float p;
+    if (K) { const float* m = margin + r * K; float wmax; const float wsum = softmax_sum(m, K, &wmax); p = expf(m[c] - wmax) / wsum; }
+    else { p = margin[r]; if (logistic) p = sigmoidf_xgb(p); }
+    key[r] = p == 0.0f ? 0.0f : p;        // -0.0 sorts as +0.0: one tie block
+    iota[r] = (int)r;
   }
 }
 
@@ -470,6 +493,10 @@ void launch_predict(const PredictArgs& a, cudaStream_t s) {
 void launch_transform(float* m, int64_t n, int K, int objective, float* out_class, cudaStream_t s) {
   if (n == 0) return;
   transform_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(m, n, K, objective, out_class); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+void launch_curve_scores(const float* margin, int64_t n, int K, int c, int logistic, float* key, int* iota, cudaStream_t s) {
+  if (n == 0) return;
+  curve_scores_kernel<<<grid_for(n), 256, 0, s>>>(margin, n, K, c, logistic, key, iota); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_fill(float* p, int64_t n, float v, cudaStream_t s) {
   if (n == 0) return;
