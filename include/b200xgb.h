@@ -61,6 +61,29 @@ XGB_DLL int XGDMatrixCreateFromCSREx(const size_t* indptr, const unsigned* indic
  * `data` is a JSON __cuda_array_interface__ {"data":[ptr,ro],"shape":[n,F],"typestr":"<f4"[,"strides":null]},
  * config JSON {"missing": NaN} */
 XGB_DLL int XGDMatrixCreateFromCudaArrayInterface(const char* data, const char* config, DMatrixHandle* out);
+
+/* ---- QuantileDMatrix from a data iterator.  The names follow upstream's c_api.h; the signatures are recalled from its 3.0
+ * release and were not checked against its source.  A proxy DMatrix carries one batch: next(iter) sets its data with one of
+ * the XGProxyDMatrixSetData* calls and its meta information with XGDMatrixSetInfoFromInterface (label, weight, base_margin,
+ * qid, label_lower_bound, label_upper_bound), then returns 1 (a batch), 0 (the end) or -1 (an error).  The batch's buffers must
+ * stay valid until the next call of next or reset.  The proxy serves no other DMatrix call. */
+typedef void* DataIterHandle;
+typedef int XGDMatrixCallbackNext(DataIterHandle iter);
+typedef void DataIterResetCallback(DataIterHandle iter);
+XGB_DLL int XGProxyDMatrixCreate(DMatrixHandle* out);
+/* host array interface JSON, 2-D, C-contiguous, any numeric typestr (other than <f4 converted to float32) */
+XGB_DLL int XGProxyDMatrixSetDataDense(DMatrixHandle handle, const char* data);
+/* __cuda_array_interface__ JSON, float32, C-contiguous: read in place (after a device synchronise) unless `missing` is not NaN */
+XGB_DLL int XGProxyDMatrixSetDataCudaArrayInterface(DMatrixHandle handle, const char* data);
+/* host CSR as three array interfaces: indptr (<u8 / <i8), indices (<u4 / <i4), data (<f4); ncol 0 = from the indices.  Absent
+ * entries are missing; `missing` does not apply to the stored values (as XGDMatrixCreateFromCSREx) */
+XGB_DLL int XGProxyDMatrixSetDataCSR(DMatrixHandle handle, const char* indptr, const char* indices, const char* data, bst_ulong ncol);
+/* reset / next iterate the batches twice (once when there is only one batch).  config JSON: {"missing": float, "max_bin": int}
+ * (defaults NaN and 256).  ref (a DMatrixHandle, or NULL): take its cuts and max_bin.  One process only: raises under a
+ * communicator with world_size > 1. */
+XGB_DLL int XGQuantileDMatrixCreateFromCallback(DataIterHandle iter, DMatrixHandle proxy, DataIterHandle ref, DataIterResetCallback* reset,
+                                                XGDMatrixCallbackNext* next, const char* config, DMatrixHandle* out);
+
 XGB_DLL int XGDMatrixFree(DMatrixHandle handle);
 XGB_DLL int XGDMatrixNumRow(DMatrixHandle handle, bst_ulong* out);                                   /* train.py:339-342 */
 XGB_DLL int XGDMatrixNumCol(DMatrixHandle handle, bst_ulong* out);
@@ -172,6 +195,9 @@ XGB_DLL int XGB200DMatrixCreateFromColumns(const void* const* cols, const int* c
                                    int weight_column, DMatrixHandle* out);
 /* the float32 feature matrix as the engine holds it (row-major n x F, NaN = missing), for bit-exact checks of the input paths */
 XGB_DLL int XGB200DMatrixGetRaw(DMatrixHandle handle, float* out_row_major);
+/* device bytes the engine holds in its buffers now (*live) and at most since the last reset (*peak); reset_peak != 0 first
+ * sets the peak to the live bytes.  Allocations outside the engine's buffer type (a 4 KB peer-exchange word) are not counted. */
+XGB_DLL int XGB200DeviceMemory(bst_ulong* live, bst_ulong* peak, int reset_peak);
 /* binned feature blocks back on the host in plain row-major n x F order (for bit-exact checks of the binning kernel) */
 XGB_DLL int XGB200DMatrixGetBins(DMatrixHandle handle, int max_bin, uint8_t* out_row_major);
 /* the two other binned copies the kernels read: the 128 B line-aligned row copy (built when the main block is 96 B wide;

@@ -9,7 +9,7 @@ import sys
 
 from . import callback, collective, core, dask, sklearn, tracker, training  # noqa: F401
 from .backend import XGBoostError, get_backend  # noqa: F401
-from .core import Booster, DMatrix  # noqa: F401
+from .core import Booster, DataIter, DMatrix, QuantileDMatrix  # noqa: F401
 from .training import cv, train  # noqa: F401
 from .sklearn import XGBClassifier, XGBModel, XGBRanker, XGBRegressor, XGBRFClassifier, XGBRFRegressor  # noqa: F401
 

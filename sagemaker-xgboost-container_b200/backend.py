@@ -97,6 +97,53 @@ class CudaBackend:
         self._check(self.lib.XGDMatrixCreateFromCudaArrayInterface(_cstr(json.dumps(iface)), _cstr(json.dumps(cfg)), C.byref(h)))
         return h
 
+    # ------------------------------------------------------------------ QuantileDMatrix (proxy batches + callbacks)
+    _RESET_CB = C.CFUNCTYPE(None, C.c_void_p)
+    _NEXT_CB = C.CFUNCTYPE(C.c_int, C.c_void_p)
+
+    def proxy_create(self):
+        h = C.c_void_p()
+        self._check(self.lib.XGProxyDMatrixCreate(C.byref(h)))
+        return h
+
+    @staticmethod
+    def _host_iface(arr):
+        return json.dumps({"data": [int(arr.ctypes.data), True], "shape": list(arr.shape), "typestr": arr.dtype.str, "version": 3})
+
+    def proxy_set_dense(self, h, arr):
+        """arr: 2-D C-contiguous numpy array of a numeric dtype (kept alive by the caller until the next batch)."""
+        self._check(self.lib.XGProxyDMatrixSetDataDense(h, _cstr(self._host_iface(arr))))
+
+    def proxy_set_cuda(self, h, obj):
+        """obj exposes __cuda_array_interface__: float32, 2-D, C-contiguous (read in place)."""
+        iface = dict(obj.__cuda_array_interface__)
+        n, F = iface["shape"]
+        if iface["typestr"] != "<f4" or (iface.get("strides") is not None and list(iface["strides"]) != [4 * F, 4]):
+            raise ValueError("device batch must be float32 and C-contiguous")
+        out = {"data": [int(iface["data"][0]), bool(iface["data"][1])], "shape": [int(n), int(F)], "typestr": "<f4", "strides": None, "version": 3}
+        self._check(self.lib.XGProxyDMatrixSetDataCudaArrayInterface(h, _cstr(json.dumps(out))))
+
+    def proxy_set_csr(self, h, indptr, indices, data, ncol):
+        self._check(self.lib.XGProxyDMatrixSetDataCSR(h, _cstr(self._host_iface(indptr)), _cstr(self._host_iface(indices)),
+                                                      _cstr(self._host_iface(data)), c_bst_ulong(ncol)))
+
+    def quantile_dmatrix_from_callback(self, proxy, ref, reset, next_, missing, max_bin):
+        """reset() / next_() -> bool are Python callables; next_ sets the batch on `proxy` before it returns True."""
+        reset_cb = self._RESET_CB(lambda _: reset())
+        next_cb = self._NEXT_CB(lambda _: 1 if next_() else 0)
+        cfg = {"max_bin": int(max_bin)}
+        if missing is not None and missing == missing:
+            cfg["missing"] = float(missing)
+        h = C.c_void_p()
+        self._check(self.lib.XGQuantileDMatrixCreateFromCallback(None, proxy, ref, reset_cb, next_cb, _cstr(json.dumps(cfg)), C.byref(h)))
+        return h
+
+    def device_memory(self, reset_peak=False):
+        """(live, peak) bytes the engine holds in its device buffers (XGB200DeviceMemory)."""
+        live, peak = c_bst_ulong(), c_bst_ulong()
+        self._check(self.lib.XGB200DeviceMemory(C.byref(live), C.byref(peak), C.c_int(1 if reset_peak else 0)))
+        return int(live.value), int(peak.value)
+
     def dmatrix_get_raw(self, h):
         n, F = self.dmatrix_num_row(h), self.dmatrix_num_col(h)
         out = np.empty(n * F, np.float32)

@@ -34,6 +34,9 @@ class DMatrix:
                  feature_types=None, nthread=None, group=None, qid=None, label_lower_bound=None, label_upper_bound=None,
                  feature_weights=None, enable_categorical=False, data_split_mode=None):
         self.handle = None
+        if isinstance(data, DataIter):
+            raise XGBoostError("DMatrix(DataIter) (external memory) is not supported by the CUDA hist path; build a QuantileDMatrix from the "
+                               "iterator instead")
         if group is not None or qid is not None:
             _check_ranking_backend()
         if enable_categorical:
@@ -243,6 +246,201 @@ class DMatrix:
     @feature_types.setter
     def feature_types(self, types):
         get_backend().dmatrix_set_str_info(self.handle, "feature_type", list(types) if types else [])
+
+
+class DataIter:
+    """Batches of a QuantileDMatrix (upstream xgboost.DataIter).  Subclasses implement reset() and next(input_data): next passes
+    one batch to input_data(data=..., label=..., ...) and returns True, or returns False at the end.  The QuantileDMatrix reads
+    the batches twice (once when there is only one), calling reset() before each pass.  A batch is released when next() is
+    called again.  cache_prefix, release_data and on_host are accepted for compatibility; the batches are never cached."""
+
+    def __init__(self, cache_prefix=None, release_data=True, *, on_host=True, min_cache_page_bytes=None):
+        self.cache_prefix = cache_prefix
+        self.release_data = release_data
+        self.on_host = on_host
+        self.min_cache_page_bytes = min_cache_page_bytes
+
+    def reset(self):
+        raise NotImplementedError()
+
+    def next(self, input_data):
+        raise NotImplementedError()
+
+
+_BATCH_FIELDS = ("label", "weight", "base_margin", "qid", "label_lower_bound", "label_upper_bound")
+
+
+def _set_proxy_batch(be, proxy, data, keep):
+    """Hands one batch's features to the proxy; `keep` collects the arrays that must outlive the call."""
+    if hasattr(data, "__cuda_array_interface__"):
+        iface = data.__cuda_array_interface__
+        shape = tuple(iface["shape"])
+        if len(shape) != 2:
+            raise ValueError("Expecting a 2-dimensional device array, got shape %s" % (shape,))
+        contiguous = iface.get("strides") is None or list(iface["strides"]) == [4 * shape[1], 4]
+        if iface["typestr"] != "<f4" or not contiguous:           # other layouts are staged as a float32 C-contiguous copy
+            if hasattr(data, "contiguous") and hasattr(data, "float"):
+                data = data.float().contiguous()
+            elif hasattr(data, "astype"):
+                data = data.astype("float32", order="C")
+            else:
+                raise ValueError("device batch must be float32 and C-contiguous")
+        keep.append(data)
+        be.proxy_set_cuda(proxy, data)
+    elif _is_scipy_sparse(data):
+        csr = data.tocsr()
+        arrs = (np.ascontiguousarray(csr.indptr, dtype=np.uint64), np.ascontiguousarray(csr.indices, dtype=np.uint32),
+                np.ascontiguousarray(csr.data, dtype=np.float32))
+        keep.extend(arrs)
+        be.proxy_set_csr(proxy, *arrs, csr.shape[1])
+    else:
+        if _is_pandas_df(data):
+            arr = data.to_numpy(dtype=np.float32, na_value=np.nan)
+        else:
+            arr = np.asarray(data)
+            if arr.dtype == object or arr.dtype.kind not in "fiub":
+                arr = arr.astype(np.float32)
+        if arr.ndim == 1:
+            arr = arr.reshape(-1, 1)
+        if arr.ndim != 2:
+            raise ValueError("Expecting 2 dimensional numpy.ndarray, got: %s" % (arr.shape,))
+        if arr.dtype == np.float16 or arr.dtype.byteorder == ">":
+            arr = arr.astype(np.float32)
+        arr = np.ascontiguousarray(arr)
+        keep.append(arr)
+        be.proxy_set_dense(proxy, arr)
+
+
+class _SingleBatch(DataIter):
+    """In-memory data as an iterator of one batch."""
+
+    def __init__(self, **kwargs):
+        super().__init__()
+        self._kwargs = kwargs
+        self._done = False
+
+    def reset(self):
+        self._done = False
+
+    def next(self, input_data):
+        if self._done:
+            return False
+        self._done = True
+        input_data(**self._kwargs)
+        return True
+
+
+class QuantileDMatrix(DMatrix):
+    """A DMatrix that holds only the binned features (upstream xgboost.QuantileDMatrix): the batches of a DataIter, or in-memory
+    data, are binned as they arrive and no float copy of the matrix stays on the device.  max_bin is fixed here (default 256);
+    training with another max_bin raises.  ref=: bin with the cuts of that matrix (for evaluation sets).  Prediction reads the
+    bins (each value at the lower edge of its bin).  As with DMatrix, a scipy CSR input marks missing values by absence and
+    `missing` does not apply to its stored values.  SHAP contributions, booster=dart, process_type=update, slice and xgb.cv
+    need the raw features and raise on a QuantileDMatrix."""
+
+    def __init__(self, data, label=None, *, weight=None, base_margin=None, missing=None, silent=False, feature_names=None,
+                 feature_types=None, nthread=None, max_bin=None, ref=None, group=None, qid=None, label_lower_bound=None,
+                 label_upper_bound=None, feature_weights=None, enable_categorical=False, max_quantile_batches=None,
+                 data_split_mode=None):
+        self.handle = None
+        if enable_categorical:
+            raise XGBoostError("categorical features are not supported on the CUDA hist path")
+        if feature_weights is not None:
+            raise XGBoostError("QuantileDMatrix: feature_weights are not supported on the CUDA hist path")
+        if max_bin is None:
+            max_bin = 256
+        else:
+            max_bin = _check_unapplied("max_bin", max_bin)
+        if ref is not None and not isinstance(ref, DMatrix):
+            raise TypeError("ref must be a DMatrix or a QuantileDMatrix")
+        be = get_backend()
+        if isinstance(data, DataIter):
+            given = dict(label=label, weight=weight, base_margin=base_margin, group=group, qid=qid, label_lower_bound=label_lower_bound,
+                         label_upper_bound=label_upper_bound)
+            named = [k for k, v in given.items() if v is not None]
+            if named:
+                raise XGBoostError("QuantileDMatrix(DataIter): pass %s per batch through input_data" % ", ".join(named))
+            it = data
+        else:
+            if group is not None:
+                if qid is not None:
+                    raise XGBoostError("QuantileDMatrix: give either group or qid")
+                sizes = np.asarray(group, dtype=np.int64).reshape(-1)
+                qid = np.repeat(np.arange(len(sizes), dtype=np.int64), sizes)
+            if feature_names is None and _is_pandas_df(data):
+                feature_names = [str(c) for c in data.columns]
+            it = _SingleBatch(data=data, label=label, weight=weight, base_margin=base_margin, qid=qid, label_lower_bound=label_lower_bound,
+                              label_upper_bound=label_upper_bound)
+        if qid is not None:
+            _check_ranking_backend()
+        proxy = be.proxy_create()
+        state = {"keep": [], "error": None, "names": None, "types": None}
+
+        def input_data(data, *, label=None, weight=None, base_margin=None, qid=None, label_lower_bound=None, label_upper_bound=None,
+                       feature_names=None, feature_types=None, group=None, **kwargs):
+            unknown = [k for k, v in kwargs.items() if v is not None]
+            if group is not None or unknown:
+                raise XGBoostError("QuantileDMatrix: input_data does not take %s (query groups go per batch as qid)" %
+                                   ", ".join((["group"] if group is not None else []) + unknown))
+            _set_proxy_batch(be, proxy, data, state["keep"])
+            meta = dict(label=label, weight=weight, base_margin=base_margin, qid=qid, label_lower_bound=label_lower_bound,
+                        label_upper_bound=label_upper_bound)
+            for field in _BATCH_FIELDS:
+                v = meta[field]
+                if v is None:
+                    continue
+                if hasattr(v, "__cuda_array_interface__") and hasattr(v, "cpu"):
+                    v = v.cpu()
+                a = np.asarray(v)
+                if field == "qid":
+                    a = a if a.dtype.kind in "iu" else a.astype(np.float64)
+                else:
+                    a = a.astype(np.float32)
+                a = np.ascontiguousarray(a).reshape(-1)
+                state["keep"].append(a)
+                be.dmatrix_set_info_interface(proxy, field, a)
+            if state["names"] is None:
+                state["names"] = feature_names if feature_names is not None else ([str(c) for c in data.columns] if _is_pandas_df(data) else None)
+                state["types"] = feature_types
+
+        def reset():
+            state["keep"] = []
+            if state["error"] is None:
+                try:
+                    it.reset()
+                except BaseException as e:  # re-raised once the engine returns
+                    state["error"] = e
+
+        def next_():
+            state["keep"] = []            # the engine is done with the previous batch
+            if state["error"] is not None:
+                return False
+            try:
+                return bool(it.next(input_data))
+            except BaseException as e:  # re-raised once the engine returns
+                state["error"] = e
+                return False
+
+        try:
+            h = be.quantile_dmatrix_from_callback(proxy, None if ref is None else ref.handle, reset, next_, missing, max_bin)
+        except XGBoostError:
+            if state["error"] is not None:        # the iterator's own exception explains the engine's
+                raise state["error"]
+            raise
+        finally:
+            state["keep"] = []
+            be.dmatrix_free(proxy)
+        if state["error"] is not None:
+            be.dmatrix_free(h)
+            raise state["error"]
+        self.handle = h
+        self.max_bin = max_bin if ref is None else getattr(ref, "max_bin", max_bin)
+        names = feature_names if feature_names is not None else state["names"]
+        types = feature_types if feature_types is not None else state["types"]
+        if names is not None:
+            self.feature_names = names
+        if types is not None:
+            self.feature_types = types
 
 
 def _check_ranking_backend():

@@ -41,10 +41,28 @@ std::atomic<uint64_t> g_uid{1};
 cudaStream_t engine_stream() { return ctx().stream; }
 int engine_num_sms() { return ctx().num_sms; }
 
+namespace {
+std::atomic<int64_t> g_devmem_live{0}, g_devmem_peak{0};
+}  // namespace
+void devmem_note(int64_t delta) {
+  const int64_t now = g_devmem_live.fetch_add(delta) + delta;
+  int64_t peak = g_devmem_peak.load();
+  while (now > peak && !g_devmem_peak.compare_exchange_weak(peak, now)) {}
+}
+void devmem_query(uint64_t* live, uint64_t* peak, bool reset_peak) {
+  if (reset_peak) g_devmem_peak.store(g_devmem_live.load());
+  if (live) *live = (uint64_t)g_devmem_live.load();
+  if (peak) *peak = (uint64_t)g_devmem_peak.load();
+}
+
 // ---------------------------------------------------------------------------------------------
 // DMatrix
 // ---------------------------------------------------------------------------------------------
 DMatrix::DMatrix() : uid(g_uid++) {}
+
+void DMatrix::require_raw(const char* what) const {
+  B200_CHECK(!quantile, std::string(what) + " is not supported on a QuantileDMatrix: it keeps only the binned features; build a DMatrix for it");
+}
 
 void DMatrix::finish_upload(float missing) {
   cudaStream_t s = engine_stream();
@@ -96,6 +114,7 @@ __global__ void gather_rows_kernel(const float* X, int F, const int* idx, int64_
 }
 
 std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len, bool allow_groups) const {
+  require_raw("DMatrix.slice (and xgb.cv, which slices its folds)");
   for (int64_t i = 0; i < len; ++i) B200_CHECK(idx[i] >= 0 && idx[i] < n, "DMatrix.slice: row index out of range");
   // with query groups: idx must list whole groups, each one's rows in order; the slice keeps those groups (and their weights)
   std::vector<unsigned> ptr; std::vector<int> groups;
@@ -151,8 +170,9 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
   else if (field == "label_upper_bound") put(label_upper, d_label_upper);
   else if (field == "weight") {
     for (size_t i = 0; i < len; ++i) B200_CHECK(v[i] >= 0 && !std::isnan(v[i]), "Weights must be positive values.");
+    B200_CHECK(!quantile || group_ptr.empty(), "weights together with query groups are not supported on a QuantileDMatrix");
     put(weights, d_weights);
-    binned = false;      // weighted quantiles depend on the weights
+    binned = binned && quantile;      // weighted quantiles depend on the weights; a QuantileDMatrix keeps the cuts it was built with
     rank_groups.valid = false;
   }
   else if (field == "base_margin") put(base_margin, d_base_margin);
@@ -164,9 +184,10 @@ void DMatrix::set_group_ptr(std::vector<unsigned> ptr) {
   for (size_t g = 1; g < ptr.size(); ++g) B200_CHECK(ptr[g] >= ptr[g - 1], "group_ptr must not decrease");
   B200_CHECK((int64_t)ptr.back() == n, "the query groups cover " + std::to_string(ptr.back()) + " rows but the DMatrix has " + std::to_string(n) +
              " (group sizes must add up to num_row)");
+  B200_CHECK(!quantile || weights.empty() || ptr.size() <= 1, "weights together with query groups are not supported on a QuantileDMatrix");
   group_ptr = ptr.size() > 1 ? std::move(ptr) : std::vector<unsigned>{};
   rank_groups.valid = false;
-  binned = binned && weights.empty();       // the sketch reads per-group weights row by row
+  binned = binned && (quantile || weights.empty());       // the sketch reads per-group weights row by row
 }
 
 void DMatrix::set_group_sizes(const unsigned* sizes, size_t len) {
@@ -198,6 +219,12 @@ const std::vector<float>& DMatrix::get_float_info(const std::string& field) cons
 }
 
 void DMatrix::bin_with_cuts() {
+  alloc_bins();
+  launch_bin(X.p, n, F, ngroups, tw, d_cut_ptrs.p, d_cut_vals.p, bins.p, bins_tail.p, engine_stream());
+  finish_bins();
+}
+
+void DMatrix::alloc_bins() {
   cudaStream_t s = engine_stream();
   feature_layout(F, &ngroups, &tw, &ntail);
   ++binned_version;
@@ -210,7 +237,10 @@ void DMatrix::bin_with_cuts() {
   bins.alloc(n_alloc * ngroups * kSlots); bins_tail.alloc(tw ? n_alloc * tw : 0);
   CUDA_OK(cudaMemsetAsync(bins.p + (size_t)n * ngroups * kSlots, 0, (size_t)512 * ngroups * kSlots, s));
   if (tw) CUDA_OK(cudaMemsetAsync(bins_tail.p + (size_t)n * tw, 0, (size_t)512 * tw, s));
-  launch_bin(X.p, n, F, ngroups, tw, d_cut_ptrs.p, d_cut_vals.p, bins.p, bins_tail.p, s);
+}
+
+void DMatrix::finish_bins() {
+  cudaStream_t s = engine_stream();
   gather_stride = ngroups * kSlots;
   bins_gather.release();
   static const bool no_aligned = getenv("B200XGB_NO_ALIGNED_ROWS") != nullptr;
@@ -229,6 +259,7 @@ void DMatrix::bin_with_cuts() {
 }
 
 void DMatrix::set_cuts(const HostCuts& c) {
+  require_raw("XGB200DMatrixSetCuts (re-binning)");
   B200_CHECK((int)c.ptrs.size() == F + 1 && (int)c.mins.size() == F, "SetCuts: cut_ptrs/min_vals do not match the number of features");
   for (int f = 0; f < F; ++f) B200_CHECK(c.ptrs[f + 1] - c.ptrs[f] >= 1 && c.ptrs[f + 1] - c.ptrs[f] <= (has_missing ? 255 : 256), "SetCuts: 1..256 cuts per feature (255 with missing values)");
   cuts = c; binned_max_bin = -1;
@@ -237,6 +268,8 @@ void DMatrix::set_cuts(const HostCuts& c) {
 
 void DMatrix::ensure_binned(int max_bin) {
   if (binned && (binned_max_bin == max_bin || binned_max_bin == -1)) return;
+  B200_CHECK(!quantile, "max_bin=" + std::to_string(max_bin) + " differs from the max_bin=" + std::to_string(quantile_max_bin) +
+             " this QuantileDMatrix was built with; pass the training max_bin to QuantileDMatrix(max_bin=...)");
   B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
   cudaStream_t s = engine_stream();
   Comm& comm = Comm::get();
@@ -302,6 +335,182 @@ void DMatrix::ensure_binned(int max_bin) {
   }
   binned_max_bin = max_bin;
   bin_with_cuts();
+}
+
+// ---------------------------------------------------------------------------------------------
+// QuantileDMatrix: binned from batches, no float copy of the whole matrix (DESIGN.md "QuantileDMatrix")
+// ---------------------------------------------------------------------------------------------
+void ProxyBatch::set_float_info(const std::string& field, const float* v, size_t len) {
+  if (field == "label") labels.assign(v, v + len);
+  else if (field == "weight") {
+    for (size_t i = 0; i < len; ++i) B200_CHECK(v[i] >= 0 && !std::isnan(v[i]), "Weights must be positive values.");
+    weights.assign(v, v + len);
+  }
+  else if (field == "base_margin") base_margin.assign(v, v + len);
+  else if (field == "label_lower_bound") label_lower.assign(v, v + len);
+  else if (field == "label_upper_bound") label_upper.assign(v, v + len);
+  else throw Error("Unknown float field name: " + field);
+}
+
+namespace {
+// The proxy's batch as a row-major float matrix on the device with NaN for missing.  A float32 device batch is read in place
+// unless it must be copied (copy, or a `missing` other than NaN: the producer's buffer is never written); everything else is
+// staged in `scratch`, which grows to the largest batch.  A CSR batch marks missing values by absence and keeps its stored
+// values, as DMatrix::from_csr does.  *nmiss: the missing entries.
+const float* stage_batch(const ProxyBatch& p, float missing, bool copy, DevBuf<float>& scratch, int64_t* nmiss, cudaStream_t s) {
+  B200_CHECK(p.kind != ProxyBatch::kNone, "QuantileDMatrix: the iterator's next() returned true without setting data on the proxy");
+  B200_CHECK(p.n >= 0 && p.n < (int64_t)0x7fffffff && p.F >= 0, "QuantileDMatrix: bad batch shape");
+  const size_t count = (size_t)p.n * p.F;
+  const bool use_missing = !std::isnan(missing) && p.kind != ProxyBatch::kCSR;
+  const float* dX = nullptr;
+  if (p.kind == ProxyBatch::kDevice) {
+    CUDA_OK(cudaDeviceSynchronize());       // the producer (e.g. a torch stream) must be done before we read its buffer
+    if (!copy && !use_missing) dX = p.data;
+    else { scratch.ensure(std::max<size_t>(count, 1)); if (count) CUDA_OK(cudaMemcpyAsync(scratch.p, p.data, sizeof(float) * count, cudaMemcpyDeviceToDevice, s)); }
+  } else if (p.kind == ProxyBatch::kHostDense) {
+    scratch.ensure(std::max<size_t>(count, 1));
+    const float* src = p.converted.empty() ? p.data : p.converted.data();
+    if (count) CUDA_OK(cudaMemcpyAsync(scratch.p, src, sizeof(float) * count, cudaMemcpyHostToDevice, s));
+  } else {
+    scratch.ensure(std::max<size_t>(count, 1));
+    if (count) {
+      DevBuf<unsigned long long> d_ptr; DevBuf<unsigned> d_idx; DevBuf<float> d_val;
+      d_ptr.alloc((size_t)p.n + 1); d_idx.alloc(std::max<size_t>(p.nelem, 1)); d_val.alloc(std::max<size_t>(p.nelem, 1));
+      CUDA_OK(cudaMemcpyAsync(d_ptr.p, p.indptr, sizeof(size_t) * ((size_t)p.n + 1), cudaMemcpyHostToDevice, s));
+      if (p.nelem) { CUDA_OK(cudaMemcpyAsync(d_idx.p, p.indices, sizeof(unsigned) * p.nelem, cudaMemcpyHostToDevice, s));
+                     CUDA_OK(cudaMemcpyAsync(d_val.p, p.values, sizeof(float) * p.nelem, cudaMemcpyHostToDevice, s)); }
+      csr_to_dense_device(d_ptr.p, d_idx.p, d_val.p, p.n, p.F, scratch.p, s);
+      Comm::get().sync_stream(s);                 // the staging buffers above die with this scope
+    }
+  }
+  if (!dX) dX = scratch.p;
+  DevBuf<unsigned long long> cnt; cnt.alloc(1); cnt.zero(s);
+  launch_count_nan(dX, (int64_t)count, missing, use_missing ? 1 : 0, cnt.p, s);
+  if (use_missing) launch_replace_missing(scratch.p, (int64_t)count, missing, s);   // dX == scratch.p here
+  unsigned long long c = 0;
+  CUDA_OK(cudaMemcpyAsync(&c, cnt.p, 8, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaStreamSynchronize(s));
+  *nmiss = (int64_t)c;
+  return dX;
+}
+}  // namespace
+
+std::unique_ptr<DMatrix> DMatrix::from_batches(ProxyBatch* proxy, const std::function<void()>& reset, const std::function<bool()>& next,
+                                               DMatrix* ref, float missing, int max_bin) {
+  B200_CHECK(!Comm::get().distributed(), "QuantileDMatrix is not supported with more than one GPU (world_size > 1); build a DMatrix on each worker");
+  B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
+  if (ref) {
+    if (!ref->quantile) ref->ensure_binned(max_bin);
+    B200_CHECK(ref->binned, "QuantileDMatrix: ref has no cuts");
+  }
+  cudaStream_t s = engine_stream();
+  auto dm = std::make_unique<DMatrix>();
+  dm->quantile = true;
+  DevBuf<float> scratch, wbuf;
+  std::vector<int64_t> rows;
+  std::vector<std::vector<FeatureSummary>> per_batch;
+  std::vector<float> labels, weights, base_margin, lower, upper, w0;
+  std::vector<int64_t> qid;
+  int64_t nmiss_total = 0;
+  auto summarise = [&](const float* dX, int64_t nr, const std::vector<float>& w) {
+    if (!w.empty()) { wbuf.ensure(w.size()); CUDA_OK(cudaMemcpyAsync(wbuf.p, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice, s)); }
+    per_batch.emplace_back();
+    compute_summaries_device(dX, nr, dm->F, w.empty() ? nullptr : wbuf.p, kRankSummaryCap, &per_batch.back(), s);
+  };
+  auto append = [](std::vector<float>& dst, const std::vector<float>& src, int64_t nr, int b, const char* what) {
+    B200_CHECK(src.empty() || (int64_t)src.size() == nr || std::string(what) == "base_margin",
+               std::string("QuantileDMatrix: batch ") + std::to_string(b) + " has " + std::to_string(src.size()) + " " + what + " for " + std::to_string(nr) + " rows");
+    dst.insert(dst.end(), src.begin(), src.end());
+  };
+  // pass 1: shapes, missing values, meta information, and (without ref) one summary per batch.  Batch 0 is always copied to
+  // the scratch buffer: if it is the only batch, it is binned from there with the exact single-rank cuts.
+  reset();
+  bool more = next();
+  int b = 0;
+  while (more) {
+    const ProxyBatch& p = *proxy;
+    if (b == 0) dm->F = p.F;
+    B200_CHECK(p.F == dm->F, "QuantileDMatrix: batch " + std::to_string(b) + " has " + std::to_string(p.F) + " columns, the first batch has " + std::to_string(dm->F));
+    int64_t nm = 0;
+    const float* dX = stage_batch(p, missing, b == 0, scratch, &nm, s);
+    nmiss_total += nm; rows.push_back(p.n);
+    append(labels, p.labels, p.n, b, "labels"); append(weights, p.weights, p.n, b, "weights"); append(base_margin, p.base_margin, p.n, b, "base_margin");
+    append(lower, p.label_lower, p.n, b, "label_lower_bound"); append(upper, p.label_upper, p.n, b, "label_upper_bound");
+    B200_CHECK(p.qid.empty() || (int64_t)p.qid.size() == p.n, "QuantileDMatrix: batch " + std::to_string(b) + " has " + std::to_string(p.qid.size()) + " qid for " + std::to_string(p.n) + " rows");
+    qid.insert(qid.end(), p.qid.begin(), p.qid.end());
+    if (b == 0) w0 = p.weights;
+    else if (!ref) summarise(dX, p.n, p.weights);          // before next(): the producer may release the batch
+    more = next();
+    if (b == 0 && more && !ref) summarise(scratch.p, rows[0], w0);
+    ++b;
+  }
+  const int nb = b;
+  int64_t n = 0;
+  for (int64_t r : rows) n += r;
+  B200_CHECK(n < (int64_t)0x7fffffff, "QuantileDMatrix: more than 2^31-1 rows per GPU are not supported");
+  dm->n = n;
+  dm->has_missing = nmiss_total > 0;
+  int F = dm->F;
+  if (ref) {
+    B200_CHECK(ref->F == F || nb == 0, "QuantileDMatrix: the data has " + std::to_string(F) + " columns, ref has " + std::to_string(ref->F));
+    dm->F = F = ref->F;
+    dm->cuts = ref->cuts;
+    if (dm->has_missing)
+      for (int f = 0; f < F; ++f)
+        B200_CHECK(ref->cuts.ptrs[f + 1] - ref->cuts.ptrs[f] <= kMissingBin,
+                   "QuantileDMatrix: the data has missing values, but the cuts of ref use all 256 bin codes for feature " + std::to_string(f) +
+                   " (ref has no missing values), so code 255 cannot mark them; build ref with a missing value, or use a DMatrix");
+    dm->binned_max_bin = ref->quantile ? ref->quantile_max_bin : ref->binned_max_bin;
+  } else {
+    if (nb == 1) {
+      if (!w0.empty()) { wbuf.ensure(w0.size()); CUDA_OK(cudaMemcpyAsync(wbuf.p, w0.data(), sizeof(float) * w0.size(), cudaMemcpyHostToDevice, s)); }
+      compute_cuts_device(scratch.p, n, F, w0.empty() ? nullptr : wbuf.p, max_bin, dm->has_missing, &dm->cuts, s);
+    } else {
+      std::vector<FeatureSummary> merged;
+      merge_summaries(per_batch, F, &merged);
+      cuts_from_summaries(merged, max_bin, dm->has_missing, &dm->cuts);
+    }
+    dm->binned_max_bin = max_bin;
+  }
+  per_batch.clear(); wbuf.release();
+  dm->quantile_max_bin = dm->binned_max_bin;
+  dm->alloc_bins();
+  if (nb == 1) {
+    if (n) launch_bin(scratch.p, n, F, dm->ngroups, dm->tw, dm->d_cut_ptrs.p, dm->d_cut_vals.p, dm->bins.p, dm->bins_tail.p, s);
+  } else if (nb > 1) {
+    // pass 2: every batch binned into the final bins at its row offset
+    reset();
+    int64_t off = 0; int bi = 0;
+    while (next()) {
+      const ProxyBatch& p = *proxy;
+      B200_CHECK(bi < nb, "QuantileDMatrix: the iterator yielded more than the " + std::to_string(nb) + " batches of its first pass");
+      B200_CHECK(p.n == rows[bi] && p.F == F, "QuantileDMatrix: batch " + std::to_string(bi) + " is " + std::to_string(p.n) + " x " + std::to_string(p.F) +
+                 " in the second pass but was " + std::to_string(rows[bi]) + " x " + std::to_string(F) + " in the first; the iterator must yield the same batches after reset()");
+      int64_t nm = 0;
+      const float* dX = stage_batch(p, missing, false, scratch, &nm, s);
+      if (p.n) launch_bin(dX, p.n, F, dm->ngroups, dm->tw, dm->d_cut_ptrs.p, dm->d_cut_vals.p, dm->bins.p + (size_t)off * dm->ngroups * kSlots,
+                          dm->tw ? dm->bins_tail.p + (size_t)off * dm->tw : nullptr, s);
+      CUDA_OK(cudaStreamSynchronize(s));      // before next(): the producer may release the batch
+      off += p.n; ++bi;
+    }
+    B200_CHECK(bi == nb, "QuantileDMatrix: the iterator yielded " + std::to_string(bi) + " batches in its second pass and " + std::to_string(nb) + " in its first");
+  }
+  scratch.release();
+  dm->finish_bins();
+  B200_CHECK(qid.empty() || weights.empty(), "weights together with query groups are not supported on a QuantileDMatrix");
+  auto need_all = [&](const std::vector<float>& v, const char* what) {
+    B200_CHECK(v.empty() || (int64_t)v.size() == n, std::string("QuantileDMatrix: ") + what + " must be given for every batch or for none (" +
+               std::to_string(v.size()) + " for " + std::to_string(n) + " rows)");
+  };
+  need_all(labels, "labels"); need_all(weights, "weights"); need_all(lower, "label_lower_bound"); need_all(upper, "label_upper_bound");
+  B200_CHECK(qid.empty() || (int64_t)qid.size() == n, "QuantileDMatrix: qid must be given for every batch or for none");
+  if (!labels.empty()) dm->set_float_info("label", labels.data(), labels.size());
+  if (!weights.empty()) dm->set_float_info("weight", weights.data(), weights.size());
+  if (!base_margin.empty()) dm->set_float_info("base_margin", base_margin.data(), base_margin.size());
+  if (!lower.empty()) dm->set_float_info("label_lower_bound", lower.data(), lower.size());
+  if (!upper.empty()) dm->set_float_info("label_upper_bound", upper.data(), upper.size());
+  if (!qid.empty()) dm->set_qid(qid.data(), qid.size());
+  return dm;
 }
 
 // Column sampling (upstream src/common/random.h ColumnSampler: bytree, then bylevel inside it, then bynode inside that; a
@@ -734,6 +943,7 @@ void Booster::bring_cache_up_to_date(DMatrix* dm, PredCache& c) {
   if (dart_.on) {
     // booster=dart: first fl(w_now - w_applied) * leaf for the trees whose weight changed since, then the new trees with their
     // weights, in one pass of the weighted tree-list kernel
+    dm->require_raw("booster=dart");
     std::vector<int> ids; std::vector<float> coef;
     for (int t = 0; t < c.trees_applied; ++t)
       if (c.weights[t] != weight_drop_[t]) { ids.push_back(t); coef.push_back(weight_drop_[t] - c.weights[t]); }
@@ -743,7 +953,7 @@ void Booster::bring_cache_up_to_date(DMatrix* dm, PredCache& c) {
     upload_model();
     PredictArgs pa = predict_args(dm, c.trees_applied, nt);
     pa.margin = c.margin.p;
-    launch_predict(pa, s);
+    run_predict(dm, pa, s);
   }
   c.trees_applied = nt;
   c.weights.assign(weight_drop_.begin(), weight_drop_.begin() + nt);
@@ -884,7 +1094,8 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
   if (objective_is_rank(param_.objective)) rank_groups(dtrain, objective_name_.c_str());
   else check_row_weights(dtrain);
-  if (update_mode_) { refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
+  if (update_mode_) { dtrain->require_raw("process_type=update"); refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
+  if (dart_.on) dtrain->require_raw("booster=dart");
   check_train_width(dtrain);
   dtrain->ensure_binned(param_.max_bin);
   const int K = param_.num_outputs();
@@ -1496,7 +1707,7 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     const int nt = te - tb;
     DevBuf<int>& leaf = pred_leaf_; leaf.ensure((size_t)n * std::max(nt, 1));
     pa.margin = nullptr; pa.leaf = leaf.p;
-    launch_predict(pa, s);
+    run_predict(dm, pa, s);
     std::vector<int> h((size_t)n * nt);
     if (!h.empty()) CUDA_OK(cudaMemcpyAsync(h.data(), leaf.p, sizeof(int) * h.size(), cudaMemcpyDeviceToHost, s));
     Comm::get().sync_stream(s);
@@ -1511,12 +1722,13 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     CUDA_OK(cudaMemcpyAsync(margin.p, dm->d_base_margin.p, sizeof(float) * n * K, cudaMemcpyDeviceToDevice, s));
   } else launch_fill(margin.p, n * K, base_margin(), s);
   if (dart_.on) {            // booster=dart: base + sum_t fl(w_t * leaf_t) in tree order (training=True predicts the same)
+    dm->require_raw("booster=dart");
     std::vector<int> ids; std::vector<float> coef;
     for (int t = tb; t < te; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
     if (!ids.empty()) dart_margin(dm, ids, coef, {}, margin.p, nullptr);
   } else {
     pa.margin = margin.p; pa.leaf = nullptr;
-    launch_predict(pa, s);
+    run_predict(dm, pa, s);
   }
   int out_cols = K;
   DevBuf<float>& cls = pred_cls_;
@@ -1549,6 +1761,7 @@ std::string Booster::debug_eval_root(DMatrix* dm, const long long* hist_fm, long
 
 // pred_contribs: path-dependent Tree SHAP on the device (shap.cu); output [n][F + 1], or [n][K][F + 1] for multi-class models
 void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* out, std::vector<uint64_t>* shape) {
+  dm->require_raw("pred_contribs (SHAP)");
   cudaStream_t s = engine_stream();
   sync_model();
   const int K = param_.num_outputs();
@@ -1610,6 +1823,18 @@ PredictArgs Booster::predict_args(DMatrix* dm, int tree_begin, int tree_end) {
   return pa;
 }
 
+void Booster::run_predict(DMatrix* dm, PredictArgs pa, cudaStream_t s) {
+  if (!dm->quantile) { launch_predict(pa, s); return; }
+  if (pa.tree_end <= pa.tree_begin) return;
+  // only the node slots of trees [tree_begin, tree_end) are mapped: an eval set maps each round's new trees once
+  int64_t lo = h_tree_offset[pa.tree_begin], hi = h_tree_offset[pa.tree_begin + 1];
+  for (int t = pa.tree_begin + 1; t < pa.tree_end; ++t) { lo = std::min(lo, h_tree_offset[t]); hi = std::max(hi, h_tree_offset[t + 1]); }
+  bin_nodes_.ensure(std::max<size_t>(d_nodes.n, 1));     // indexed like d_nodes; grows (and is rewritten) with it
+  launch_bin_thresholds(d_nodes.p + lo, (size_t)(hi - lo), dm->d_cut_ptrs.p, dm->d_cut_vals.p, dm->d_min_vals.p, dm->F, bin_nodes_.p + lo, s);
+  pa.nodes = bin_nodes_.p;
+  launch_predict_bins(pa, dm->binned_view(), s);
+}
+
 // the plan predict(dm, iteration_range = [iter_begin, iter_end)) executes (iter_end == 0: every round)
 std::string Booster::debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end) {
   configure();
@@ -1617,7 +1842,7 @@ std::string Booster::debug_predict_plan(DMatrix* dm, int iter_begin, int iter_en
   if (iter_end == 0) iter_end = layers();
   B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end <= layers(), "debug_predict_plan: invalid iteration range");
   const PredictArgs pa = predict_args(dm, iteration_indptr_[iter_begin], iteration_indptr_[iter_end]);
-  return predict_plan_json(plan_for(pa), pa.tree_begin, pa.tree_end, pa.has_nan != 0);
+  return predict_plan_json(dm->quantile ? plan_for_bins(pa, dm->binned_view()) : plan_for(pa), pa.tree_begin, pa.tree_end, pa.has_nan != 0);
 }
 
 // device time of the predictor kernel alone (margins of all trees into the scratch buffer), for the roofline line of bench.py
@@ -1634,7 +1859,7 @@ float Booster::debug_predict_kernel_ms(DMatrix* dm, int repeats) {
   for (int r = 0; r < std::max(1, repeats); ++r) {
     launch_fill(pred_margin_.p, dm->n * K, base_margin(), s);
     CUDA_OK(cudaEventRecord(e0, s));
-    launch_predict(pa, s);
+    run_predict(dm, pa, s);
     CUDA_OK(cudaEventRecord(e1, s));
     CUDA_OK(cudaEventSynchronize(e1));
     float ms = 0; CUDA_OK(cudaEventElapsedTime(&ms, e0, e1)); total += ms;

@@ -1,5 +1,6 @@
 // booster.h -- host-side objects behind the C-ABI handles (DMatrixHandle / BoosterHandle).
 #pragma once
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -17,6 +18,20 @@
 
 namespace b200 {
 
+// One batch of a QuantileDMatrix as its producer hands it over (upstream's proxy DMatrix): the features stay where the
+// producer keeps them until the next batch is requested; the meta information is copied.
+struct ProxyBatch {
+  enum Kind { kNone, kHostDense, kDevice, kCSR } kind = kNone;
+  int64_t n = 0; int F = 0;
+  const float* data = nullptr;                        // kHostDense (float32, row-major) / kDevice (float32, C-contiguous)
+  std::vector<float> converted;                       // kHostDense of another dtype, converted to float32
+  const size_t* indptr = nullptr; const unsigned* indices = nullptr; const float* values = nullptr; size_t nelem = 0;   // kCSR
+  std::vector<float> labels, weights, base_margin, label_lower, label_upper;
+  std::vector<int64_t> qid;
+  void clear_meta() { labels.clear(); weights.clear(); base_margin.clear(); label_lower.clear(); label_upper.clear(); qid.clear(); }
+  void set_float_info(const std::string& field, const float* v, size_t len);
+};
+
 // ---------------------------------------------------------------------------------------------
 // DMatrix: features resident on the device (raw float row-major + lazily the binned feature blocks)
 // ---------------------------------------------------------------------------------------------
@@ -24,7 +39,9 @@ class DMatrix {
  public:
   int64_t n = 0; int F = 0;
   bool has_missing = false;
-  DevBuf<float> X;                                    // n x F, NaN = missing
+  // a QuantileDMatrix: binned once from batches at construction, X never allocated, the bins fixed at quantile_max_bin
+  bool quantile = false; int quantile_max_bin = 0;
+  DevBuf<float> X;                                    // n x F, NaN = missing (empty on a quantile matrix)
   std::vector<float> labels, weights, base_margin;    // host copies (returned by GetFloatInfo)
   DevBuf<float> d_labels, d_weights, d_base_margin;
   std::vector<float> label_lower, label_upper;         // survival:aft interval bounds (label_lower_bound / label_upper_bound)
@@ -58,6 +75,12 @@ class DMatrix {
   static std::unique_ptr<DMatrix> from_csr(const size_t* indptr, const unsigned* indices, const float* data, size_t nindptr, size_t nelem, size_t ncol);
   // recordio-protobuf body (recordio.cu): status 0 decoded, 1 the body is invalid (*message names the rule), 2 needs the host route
   static std::unique_ptr<DMatrix> from_recordio(const char* buf, int64_t len, int* status, std::string* message);
+  // QuantileDMatrix (DESIGN.md "QuantileDMatrix"): reset() then next() until false, twice; next() leaves the batch in *proxy.
+  // Cuts: ref's when given, the exact single-rank cuts for one batch, else the multi-rank recipe over the batches in order.
+  static std::unique_ptr<DMatrix> from_batches(ProxyBatch* proxy, const std::function<void()>& reset, const std::function<bool()>& next,
+                                               DMatrix* ref, float missing, int max_bin);
+  // names the reader of the raw features that a quantile matrix cannot serve
+  void require_raw(const char* what) const;
   // allow_groups: a matrix with groups may be sliced by whole groups, which the slice carries
   std::unique_ptr<DMatrix> slice(const int* idx, int64_t len, bool allow_groups = false) const;
   void set_float_info(const std::string& field, const float* v, size_t len);
@@ -74,6 +97,8 @@ class DMatrix {
   void finish_upload(float missing);
  private:
   void bin_with_cuts();
+  void alloc_bins();                                  // uploads the cuts, allocates the main / tail bins with their pad rows
+  void finish_bins();                                 // the aligned and column-major copies of the binned main / tail
 };
 
 // device half of DMatrix::from_csr (ingest.cu): X (nrow x F) filled with NaN, then row r's entries [d_ptr[r], d_ptr[r + 1]) stored
@@ -175,6 +200,10 @@ class Booster {
 
  private:
   PredictArgs predict_args(DMatrix* dm, int tree_begin, int tree_end);   // the device model on dm (outputs left unset)
+  // margins / leaves of trees [pa.tree_begin, pa.tree_end) into pa's outputs: the float predictor, or on a quantile matrix the
+  // bin predictor with the model's thresholds mapped to dm's bins first
+  void run_predict(DMatrix* dm, PredictArgs pa, cudaStream_t s);
+  DevBuf<DevNode> bin_nodes_;                   // d_nodes with each split's cond replaced by its bin threshold (run_predict)
   std::map<std::string, std::string> raw_params_;
   std::vector<std::string> eval_metrics_;
   std::vector<int> monotone_;              // parsed monotone_constraints (empty = none)

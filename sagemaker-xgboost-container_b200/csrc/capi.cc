@@ -22,6 +22,7 @@ namespace {
 thread_local std::string g_last_error;
 struct DMatrixBox {
   std::unique_ptr<DMatrix> dm;
+  std::unique_ptr<ProxyBatch> proxy;              // a proxy DMatrix (XGProxyDMatrixCreate): one batch of a QuantileDMatrix
   std::vector<const char*> str_ptrs; std::vector<std::string> strs;
   std::vector<uint8_t> scratch_u8;
 };
@@ -33,7 +34,10 @@ struct BoosterBox {
 thread_local std::string g_ret_str;
 
 int fail(const std::exception& e) { g_last_error = e.what(); return -1; }
-DMatrix* DM(DMatrixHandle h) { if (!h) throw Error("DMatrix handle is NULL"); return static_cast<DMatrixBox*>(h)->dm.get(); }
+DMatrix* DM(DMatrixHandle h) { if (!h) throw Error("DMatrix handle is NULL"); DMatrixBox* b = static_cast<DMatrixBox*>(h);
+  if (!b->dm) throw Error("a proxy DMatrix only carries one batch of a QuantileDMatrix"); return b->dm.get(); }
+ProxyBatch* PROXY(DMatrixHandle h) { if (!h) throw Error("DMatrix handle is NULL"); DMatrixBox* b = static_cast<DMatrixBox*>(h);
+  if (!b->proxy) throw Error("not a proxy DMatrix (XGProxyDMatrixCreate)"); return b->proxy.get(); }
 Booster* BST(BoosterHandle h) { if (!h) throw Error("Booster handle is NULL"); return static_cast<BoosterBox*>(h)->bst.get(); }
 #define API_BEGIN() try {
 #define API_END() } catch (const std::exception& e) { return fail(e); } return 0;
@@ -152,9 +156,99 @@ int XGDMatrixSetInfoFromInterface(DMatrixHandle handle, const char* field, const
   API_BEGIN();
   HostArray h = parse_array_interface(data);
   const std::string f(field);
+  if (handle && static_cast<DMatrixBox*>(handle)->proxy) {            // the current batch's meta information
+    ProxyBatch* p = PROXY(handle);
+    B200_CHECK(f != "group", "QuantileDMatrix: give query groups per batch as qid, not group");
+    if (f == "qid") p->qid = to_int64(h, field);
+    else { std::vector<float> v = to_float32(h); p->set_float_info(f, v.data(), v.size()); }
+    return 0;
+  }
   if (f == "qid") { std::vector<int64_t> q = to_int64(h, field); DM(handle)->set_qid(q.data(), q.size()); }
   else if (f == "group") { std::vector<unsigned> g = to_group_sizes(to_int64(h, field)); DM(handle)->set_group_sizes(g.data(), g.size()); }
   else { std::vector<float> v = to_float32(h); DM(handle)->set_float_info(field, v.data(), v.size()); }
+  API_END();
+}
+
+// ---- proxy DMatrix and QuantileDMatrix (upstream c_api.h names; see include/b200xgb.h)
+int XGProxyDMatrixCreate(DMatrixHandle* out) {
+  API_BEGIN();
+  auto box = new DMatrixBox(); box->proxy = std::make_unique<ProxyBatch>();
+  *out = box;
+  API_END();
+}
+namespace {
+ProxyBatch* fresh_batch(DMatrixHandle handle) {
+  ProxyBatch* p = PROXY(handle);
+  p->kind = ProxyBatch::kNone; p->converted.clear(); p->clear_meta();
+  return p;
+}
+}  // namespace
+int XGProxyDMatrixSetDataDense(DMatrixHandle handle, const char* data) {
+  API_BEGIN();
+  ProxyBatch* p = fresh_batch(handle);
+  HostArray h = parse_array_interface(data);
+  p->n = h.n; p->F = (int)h.m;
+  if (h.typestr == "<f4") p->data = static_cast<const float*>(h.ptr);
+  else { p->converted = to_float32(h); p->data = nullptr; }
+  p->kind = ProxyBatch::kHostDense;
+  API_END();
+}
+int XGProxyDMatrixSetDataCudaArrayInterface(DMatrixHandle handle, const char* data) {
+  API_BEGIN();
+  ProxyBatch* p = fresh_batch(handle);
+  JPtr a = parse_json(data);
+  const JValue& shape = a->at("shape");
+  if (shape.length() != 2) throw Error("cuda array interface: expecting a 2-dimensional array");
+  if (a->at("typestr").s != "<f4") throw Error("cuda array interface: only float32 (<f4) is supported, got " + a->at("typestr").s);
+  if (a->has("strides") && a->at("strides").type != JValue::kNull) throw Error("cuda array interface: only C-contiguous arrays are supported");
+  p->data = reinterpret_cast<const float*>((uintptr_t)a->at("data").arr[0]->as_int());
+  p->n = (int64_t)shape.num_at(0); p->F = (int)shape.num_at(1);
+  p->kind = ProxyBatch::kDevice;
+  API_END();
+}
+int XGProxyDMatrixSetDataCSR(DMatrixHandle handle, const char* indptr, const char* indices, const char* data, bst_ulong ncol) {
+  API_BEGIN();
+  ProxyBatch* p = fresh_batch(handle);
+  HostArray ip = parse_array_interface(indptr), ix = parse_array_interface(indices), dv = parse_array_interface(data);
+  B200_CHECK(ip.typestr == "<u8" || ip.typestr == "<i8", "CSR indptr must be 64-bit integers");
+  B200_CHECK(ix.typestr == "<u4" || ix.typestr == "<i4", "CSR indices must be 32-bit integers");
+  B200_CHECK(dv.typestr == "<f4", "CSR data must be float32");
+  B200_CHECK(ip.n >= 1 && ix.n == dv.n, "CSR: indptr must not be empty and indices / data must have the same length");
+  p->indptr = static_cast<const size_t*>(ip.ptr); p->indices = static_cast<const unsigned*>(ix.ptr); p->values = static_cast<const float*>(dv.ptr);
+  p->nelem = (size_t)dv.n; p->n = ip.n - 1;
+  B200_CHECK(p->indptr[0] == 0 && p->indptr[p->n] <= p->nelem, "CSR: indptr must start at 0 and end within the index / value arrays");
+  for (int64_t r = 0; r < p->n; ++r) B200_CHECK(p->indptr[r] <= p->indptr[r + 1], "CSR: indptr is not non-decreasing");
+  size_t F = (size_t)ncol;
+  for (size_t i = 0; i < p->nelem; ++i) F = std::max<size_t>(F, (size_t)p->indices[i] + 1);
+  p->F = (int)F;
+  p->kind = ProxyBatch::kCSR;
+  API_END();
+}
+int XGQuantileDMatrixCreateFromCallback(DataIterHandle iter, DMatrixHandle proxy, DataIterHandle ref, DataIterResetCallback* reset,
+                                        XGDMatrixCallbackNext* next, const char* config, DMatrixHandle* out) {
+  API_BEGIN();
+  ProxyBatch* p = PROXY(proxy);
+  JPtr cfg = parse_json(config ? config : "{}");
+  const float missing = cfg->has("missing") && cfg->at("missing").type != JValue::kNull ? (float)cfg->at("missing").as_double() : std::nanf("");
+  const int max_bin = cfg->has("max_bin") && cfg->at("max_bin").type != JValue::kNull ? (int)cfg->at("max_bin").as_int() : 256;
+  auto do_reset = [&]() { p->kind = ProxyBatch::kNone; p->clear_meta(); reset(iter); };
+  auto do_next = [&]() -> bool {
+    p->kind = ProxyBatch::kNone; p->clear_meta();
+    const int r = next(iter);
+    B200_CHECK(r >= 0, "QuantileDMatrix: the iterator's next() failed");
+    return r != 0;
+  };
+  auto box = new DMatrixBox(); std::unique_ptr<DMatrixBox> guard(box);
+  box->dm = DMatrix::from_batches(p, do_reset, do_next, ref ? DM(ref) : nullptr, missing, max_bin);
+  *out = guard.release();
+  API_END();
+}
+int XGB200DeviceMemory(bst_ulong* live, bst_ulong* peak, int reset_peak) {
+  API_BEGIN();
+  uint64_t l = 0, pk = 0;
+  devmem_query(&l, &pk, reset_peak != 0);
+  if (live) *live = l;
+  if (peak) *peak = pk;
   API_END();
 }
 
@@ -495,6 +589,7 @@ int XGB200DMatrixRankCuts(DMatrixHandle handle, int max_bin, const int64_t* row_
   API_BEGIN();
   DMatrix* dm = DM(handle);
   B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
+  dm->require_raw("XGB200DMatrixRankCuts");
   B200_CHECK(n_ranges >= 1 && row_bounds[0] == 0 && row_bounds[n_ranges] == dm->n, "XGB200DMatrixRankCuts: the ranges must cover the rows");
   B200_CHECK(dm->weights.empty() || (int64_t)dm->weights.size() == dm->n, "XGB200DMatrixRankCuts: the weights must be one per row");
   for (int r = 0; r < n_ranges; ++r) B200_CHECK(row_bounds[r] <= row_bounds[r + 1], "XGB200DMatrixRankCuts: row_bounds must not decrease");
@@ -580,6 +675,7 @@ static void hist_to_feature_major(const DMatrix* dm, const std::vector<long long
 int XGB200DMatrixGetRaw(DMatrixHandle handle, float* out_row_major) {
   API_BEGIN();
   DMatrix* dm = DM(handle);
+  dm->require_raw("XGB200DMatrixGetRaw");
   if (dm->n * dm->F > 0) CUDA_OK(cudaMemcpy(out_row_major, dm->X.p, sizeof(float) * (size_t)dm->n * dm->F, cudaMemcpyDeviceToHost));
   API_END();
 }

@@ -26,13 +26,18 @@ extern long long g_kernel_launches;
 cudaStream_t engine_stream();
 int engine_num_sms();
 
+// bytes held through DevBuf, now and at most since the last reset (include/b200xgb.h XGB200DeviceMemory)
+void devmem_note(int64_t delta);
+void devmem_query(uint64_t* live, uint64_t* peak, bool reset_peak);
+
 template <typename T> struct DevBuf {
   T* p = nullptr; size_t n = 0;
   DevBuf() = default;
   DevBuf(const DevBuf&) = delete; DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { release(); }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-  void alloc(size_t count) { if (count == n && p) return; release(); if (count) { CUDA_OK(cudaMalloc(&p, count * sizeof(T))); } n = count; }
+  void release() { if (p) { cudaFree(p); devmem_note(-(int64_t)(n * sizeof(T))); } p = nullptr; n = 0; }
+  void alloc(size_t count) { if (count == n && p) return; release();
+    if (count) { CUDA_OK(cudaMalloc(&p, count * sizeof(T))); devmem_note((int64_t)(count * sizeof(T))); } n = count; }
   void ensure(size_t count) { if (count > n) alloc(count); }
   void zero(cudaStream_t s) { if (n) CUDA_OK(cudaMemsetAsync(p, 0, n * sizeof(T), s)); }
 };

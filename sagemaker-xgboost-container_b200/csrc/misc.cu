@@ -8,6 +8,7 @@
 #include "curve.h"
 #include "engine.h"
 #include "misc.h"
+#include "predict_tile.h"
 #include "rng.h"
 #include "traverse.h"
 
@@ -249,36 +250,12 @@ __global__ void __launch_bounds__(256) predict_kernel(PredictArgs a) {
 // (the thread-per-row kernel above gathers 4 B at a time from a 4*F-byte row: 1 % of HBM peak in round 1) and keeps the
 // trees there too, 8 B per node, so a traversal step is two LDS.  With T trees of depth D a row costs ~8*T*D instructions
 // against 4*F bytes: beyond T*D ~ 100 the kernel is issue-bound, not HBM-bound (DESIGN.md "predictor").
-struct PNode { float cond; unsigned w; };            // w = left child (16 bit, 0xffff = leaf) | feature << 16 | default_left << 31
-
-// PNode::w keeps 15 bits of feature id: the plan tiles only matrices of at most kPredictMaxPitch features
-static_assert(kPredictMaxPitch <= 0x7fff + 1, "the tiled predictor's feature field has 15 bits");
-
 template <bool HAS_NAN, bool LEAF_OUT>
 __global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, int tree_lo, int tree_hi, int pitch, int rows_per_tile, int64_t num_tiles) {
   extern __shared__ __align__(16) unsigned char psm[];
-  const int nt_chunk = tree_hi - tree_lo;
-  int* s_toff = reinterpret_cast<int*>(psm);                                   // [nt_chunk + 1] node offsets inside s_nodes
-  PNode* s_nodes = reinterpret_cast<PNode*>(psm + (((size_t)(nt_chunk + 1) * 4 + 15) & ~(size_t)15));
-  __shared__ int s_total;
-  if (threadIdx.x == 0) {
-    int off = 0;
-    for (int t = 0; t < nt_chunk; ++t) { s_toff[t] = off; off += (int)(a.tree_offset[tree_lo + t + 1] - a.tree_offset[tree_lo + t]); }
-    s_toff[nt_chunk] = off; s_total = off;
-  }
-  __syncthreads();
-  for (int t = 0; t < nt_chunk; ++t) {
-    const DevNode* src = a.nodes + a.tree_offset[tree_lo + t];
-    const int cnt = s_toff[t + 1] - s_toff[t];
-    for (int i = threadIdx.x; i < cnt; i += blockDim.x) {
-      const DevNode d = src[i];
-      PNode p; p.cond = d.cond;
-      p.w = (d.left < 0 ? 0xffffu : (unsigned)d.left) | ((d.fidx_dl & 0x7fffu) << 16) | (d.fidx_dl & 0x80000000u);
-      s_nodes[s_toff[t] + i] = p;
-    }
-  }
-  float* s_x = reinterpret_cast<float*>(s_nodes + s_total);
-  const int F = a.F, K = a.K, nt_all = a.tree_end - a.tree_begin;
+  int* s_toff; PNode* s_nodes;
+  float* s_x = reinterpret_cast<float*>(stage_tree_chunk(a, tree_lo, tree_hi, psm, &s_toff, &s_nodes));
+  const int F = a.F, nt_chunk = tree_hi - tree_lo;
   for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int64_t r0 = tile * rows_per_tile;
     const int rows = (int)((a.n - r0 < rows_per_tile) ? a.n - r0 : rows_per_tile);
@@ -289,42 +266,12 @@ __global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, int 
     __syncthreads();
     for (int rl = threadIdx.x; rl < rows; rl += blockDim.x) {
       const float* x = s_x + rl * pitch;
-      const int64_t r = r0 + rl;
-      float acc = (!LEAF_OUT && K == 1) ? a.margin[r] : 0.f;
-      auto step = [&](const PNode* tn, int& nid, PNode& nd) {
+      predict_staged_row<LEAF_OUT>(a, s_nodes, s_toff, nt_chunk, tree_lo, r0 + rl, [&](const PNode& nd) {
         const float v = x[(nd.w >> 16) & 0x7fffu];
-        const int left = (int)(nd.w & 0xffffu);
         bool go_left = v < nd.cond;
         if (HAS_NAN) { if (isnan(v)) go_left = (nd.w >> 31) != 0; }
-        nid = go_left ? left : left + 1;                                        // children are allocated as adjacent pairs
-        nd = tn[nid];
-      };
-      auto emit = [&](int t, int nid, const PNode& nd) {
-        if (LEAF_OUT) a.leaf[r * nt_all + (tree_lo - a.tree_begin) + t] = nid;
-        else if (K == 1) acc += nd.cond;                                        // fp32, in tree order (== the reference's sequential sum)
-        else a.margin[r * K + a.tree_info[tree_lo + t]] += nd.cond;
-      };
-      int t = 0;
-      for (; t + 4 <= nt_chunk; t += 4) {                                       // four independent traversals in flight hide the LDS latency
-        const PNode* tn[4]; int nid[4]; PNode nd[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { tn[j] = s_nodes + s_toff[t + j]; nid[j] = 0; nd[j] = tn[j][0]; }
-        bool any = true;
-        while (any) {
-          any = false;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) if ((nd[j].w & 0xffffu) != 0xffffu) { step(tn[j], nid[j], nd[j]); any = true; }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) emit(t + j, nid[j], nd[j]);
-      }
-      for (; t < nt_chunk; ++t) {
-        const PNode* tn = s_nodes + s_toff[t];
-        int nid = 0; PNode nd = tn[0];
-        while ((nd.w & 0xffffu) != 0xffffu) step(tn, nid, nd);
-        emit(t, nid, nd);
-      }
-      if (!LEAF_OUT && K == 1) a.margin[r] = acc;
+        return go_left;
+      });
     }
   }
 }

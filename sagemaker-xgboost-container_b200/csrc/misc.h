@@ -91,6 +91,15 @@ void launch_count_nan(const float* X, int64_t count, float missing, int use_miss
 void launch_replace_missing(float* X, int64_t count, float missing, cudaStream_t s);
 PredictPlan plan_for(const PredictArgs& a);             // what launch_predict(a) runs
 void launch_predict(const PredictArgs& a, cudaStream_t s);
+// Prediction from the bins (predict_bins.cu).  Each value stands at the lower edge of its bin (min_vals[f] for bin 0, else
+// cut_vals[ptr + b - 1]), so `x < cond` becomes `b < t` with t the number of the feature's lower edges below cond.
+// launch_bin_thresholds copies nodes[0, count) to out with each split's cond replaced by t (as int bits); a split on a feature
+// f >= F reads feature 0 with t fixed to its default direction (0: right, 512: left).
+void launch_bin_thresholds(const DevNode* nodes, size_t count, const int* cut_ptrs, const float* cut_vals, const float* min_vals, int F,
+                           DevNode* out, cudaStream_t s);
+PredictPlan plan_for_bins(const PredictArgs& a, const BinnedMatrix& m);   // what launch_predict_bins(a, m) runs
+// launch_predict on m's bins: a.nodes are launch_bin_thresholds' nodes; a.X and a.has_nan are not read (m.has_missing is)
+void launch_predict_bins(const PredictArgs& a, const BinnedMatrix& m, cudaStream_t s);
 void launch_transform(float* m, int64_t n, int K, int objective, float* out_class, cudaStream_t s);
 void launch_fill(float* p, int64_t n, float v, cudaStream_t s);
 void launch_metric(const MetricArgs& a, cudaStream_t s);
