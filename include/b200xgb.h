@@ -258,6 +258,14 @@ XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dma
  * {"kernel": "predict_tiled_kernel" | "predict_kernel", "reason" (why thread-per-row), "has_nan", "tree_begin", "tree_end",
  * "pitch", "chunks": [{"begin","end","node_bytes","rows","threads","smem"}]} (see csrc/predict_plan.h) */
 XGB_DLL int XGB200BoosterPredictPlan(BoosterHandle handle, DMatrixHandle dmat, int iter_begin, int iter_end, const char** out_json);
+/* the container's own metrics (sagemaker_xgboost_container custom_metrics: accuracy, balanced_accuracy, f1, f1_binary,
+ * f1_macro, precision[_macro|_micro], recall[_macro|_micro], mse, rmse, mae, r2) on `dmat`, from the prediction cache: the
+ * raw results out[8 + 64 * 64] (csrc/container_metrics.h): out[0] bits decided (1 confusion counts, 2 regression sums, 4 the
+ * label sums of r2), out[1] rows, out[2] predicted classes P, out[3] label bound L = 64, out[4..8) float32 bits of
+ * sum (y-p)^2, sum |y-p|, sum y, sum (y-mean)^2 in numpy's pairwise order, out[8..] counts [L][P].  output_margin: the
+ * metric reads the margins (feval=) rather than predict()'s values */
+XGB_DLL int XGB200BoosterEvalContainerMetrics(BoosterHandle handle, DMatrixHandle dmat, const char** names, bst_ulong len, int output_margin,
+                                              long long* out);
 /* raw margins of the prediction cache the trainer keeps for `dmat` (n x outputs per row), brought up to date first */
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */

@@ -556,6 +556,15 @@ class CudaBackend:
         self._check(self.lib.XGB200BoosterPredictPlan(bh, dh, C.c_int(iteration_range[0]), C.c_int(iteration_range[1]), C.byref(out)))
         return json.loads(out.value.decode())
 
+    def booster_eval_container_metrics(self, bh, dh, names, output_margin):
+        """Raw results of the container's own metrics on this matrix, int64[8 + 64 * 64]
+        (include/b200xgb.h XGB200BoosterEvalContainerMetrics)."""
+        arr = (C.c_char_p * len(names))(*[n.encode("utf-8") for n in names])
+        out = np.zeros(8 + 64 * 64, np.int64)
+        self._check(self.lib.XGB200BoosterEvalContainerMetrics(bh, dh, arr, c_bst_ulong(len(names)), C.c_int(1 if output_margin else 0),
+                                                               out.ctypes.data_as(C.POINTER(C.c_longlong))))
+        return out
+
     def booster_cached_margin(self, bh, dh, K):
         n = self.dmatrix_num_row(dh)
         out = np.zeros((n, K), np.float32)

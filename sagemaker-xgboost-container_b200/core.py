@@ -743,8 +743,13 @@ class Booster:
             self._validate_features(d)
         msg = get_backend().booster_eval(self.handle, int(iteration), [d.handle for d, _ in evals], [n for _, n in evals])
         if feval is not None:
+            from . import container_metrics
+            names = container_metrics.recognise(feval) if container_metrics.device_route_available() else None
             for dmat, evname in evals:
-                feval_ret = feval(self.predict(dmat, training=False, output_margin=output_margin), dmat)
+                if names is not None:         # the container's own metrics: finished from the engine's exact raw results
+                    feval_ret = container_metrics.evaluate(self, dmat, names, output_margin)
+                else:
+                    feval_ret = feval(self.predict(dmat, training=False, output_margin=output_margin), dmat)
                 if isinstance(feval_ret, list):
                     for name, val in feval_ret:
                         msg += "\t%s-%s:%f" % (evname, name, val)

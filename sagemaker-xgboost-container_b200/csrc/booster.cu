@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cctype>
+#include <climits>
 #include <cmath>
 #include <cstring>
 #include "comm.h"
@@ -165,7 +166,7 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
     h.assign(v, v + len); d.alloc(len);
     if (len) { CUDA_OK(cudaMemcpyAsync(d.p, h.data(), sizeof(float) * len, cudaMemcpyHostToDevice, s)); Comm::get().sync_stream(s); }
   };
-  if (field == "label") { put(labels, d_labels); cox_order.valid = false; rank_groups.valid = false; }
+  if (field == "label") { put(labels, d_labels); cox_order.valid = false; rank_groups.valid = false; container_sums.labels_valid = false; }
   else if (field == "label_lower_bound") put(label_lower, d_label_lower);      // survival:aft; the bins do not depend on them
   else if (field == "label_upper_bound") put(label_upper, d_label_upper);
   else if (field == "weight") {
@@ -1682,10 +1683,81 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
   return out;
 }
 
+// The container's custom_metrics (DESIGN.md "Container metrics"): what the device pass decides exactly, in the raw form the
+// Python finisher turns into scikit-learn's values; anything left undecided is evaluated by the container's own function.
+void Booster::eval_container_metrics(DMatrix* dm, const std::vector<std::string>& names, bool output_margin, long long* out) {
+  configure();
+  static const char* kClass[] = {"accuracy", "balanced_accuracy", "f1", "f1_binary", "f1_macro", "precision", "precision_macro",
+                                 "precision_micro", "recall", "recall_macro", "recall_micro"};
+  bool want_class = false, want_reg = false, want_r2 = false;
+  for (const std::string& name : names) {
+    if (std::find(std::begin(kClass), std::end(kClass), name) != std::end(kClass)) want_class = true;
+    else if (name == "mse" || name == "rmse" || name == "mae") want_reg = true;
+    else if (name == "r2") want_reg = want_r2 = true;
+    else throw Error("unknown container metric " + name);
+  }
+  const int K = param_.num_outputs();
+  const int cols = (!output_margin && param_.objective == kSoftmax) ? 1 : K;
+  const int P = cols == 1 ? 2 : cols;
+  const int64_t n = dm->n;
+  std::fill(out, out + kContainerOutLen, 0LL);
+  out[1] = n; out[2] = P; out[3] = kContainerLabels;
+  if (n == 0 || dm->labels.size() != (size_t)n) return;
+  want_class = want_class && P <= kContainerLabels;
+  want_reg = want_reg && cols == 1 && n <= INT_MAX;
+  want_r2 = want_r2 && want_reg;
+  if (!want_class && !want_reg) return;
+  cudaStream_t s = engine_stream();
+  const float* margin;
+  if (dart_.on) {
+    // the dart cache carries each round's weight changes as fl(w_now - w_applied) * leaf, while predict() sums
+    // fl(w_t * leaf_t) afresh: the two differ in the last bits, so the metrics read predict()'s own margins
+    predict_margin(dm, 0, (int)trees_.size());
+    margin = pred_margin_.p;
+  } else {
+    PredCache& c = cache_for(dm);
+    bring_cache_up_to_date(dm, c);
+    margin = c.margin.p;
+  }
+  ContainerArgs a{}; a.margin = margin; a.label = dm->d_labels.p; a.n = n; a.K = K;
+  a.objective = param_.objective; a.output_margin = output_margin ? 1 : 0;
+  a.want_class = want_class; a.want_reg = want_reg; a.want_r2 = want_r2;
+  container_metrics_device(a, &dm->container_sums, &container_scratch_, s);
+  const size_t len = kContainerOutHead + (size_t)kContainerLabels * P;
+  CUDA_OK(cudaMemcpyAsync(out + 4, container_scratch_.out.p + 4, sizeof(long long) * (len - 4), cudaMemcpyDeviceToHost, s));
+  long long bad = 0;
+  CUDA_OK(cudaMemcpyAsync(&bad, container_scratch_.out.p, sizeof(long long), cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
+  out[0] = (want_class && !(bad & 1) ? kDecidedClass : 0) | (want_reg && !(bad & 2) ? kDecidedReg : 0) |
+           (want_r2 && !(bad & 2) ? kDecidedLabelSums : 0);
+}
+
 // ---------------------------------------------------------------------------------------------
 // prediction (upstream Booster.predict -> XGBoosterPredictFromDMatrix; cpu_predictor.cc semantics)
 // type: 0 value, 1 margin, 6 leaf
 // ---------------------------------------------------------------------------------------------
+void Booster::predict_margin(DMatrix* dm, int tb, int te) {
+  cudaStream_t s = engine_stream();
+  const int K = param_.num_outputs();
+  const int64_t n = dm->n;
+  upload_model();
+  DevBuf<float>& margin = pred_margin_; margin.ensure((size_t)n * K);          // scratch kept across calls: no cudaMalloc / cudaFree per request
+  if (!dm->base_margin.empty()) {
+    B200_CHECK(dm->base_margin.size() == (size_t)n * K, "base_margin size does not match rows x groups");
+    CUDA_OK(cudaMemcpyAsync(margin.p, dm->d_base_margin.p, sizeof(float) * n * K, cudaMemcpyDeviceToDevice, s));
+  } else launch_fill(margin.p, n * K, base_margin(), s);
+  if (dart_.on) {            // booster=dart: base + sum_t fl(w_t * leaf_t) in tree order (training=True predicts the same)
+    dm->require_raw("booster=dart");
+    std::vector<int> ids; std::vector<float> coef;
+    for (int t = tb; t < te; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
+    if (!ids.empty()) dart_margin(dm, ids, coef, {}, margin.p, nullptr);
+  } else {
+    PredictArgs pa = predict_args(dm, tb, te);
+    pa.margin = margin.p; pa.leaf = nullptr;
+    run_predict(dm, pa, s);
+  }
+}
+
 void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int iter_end, bool strict_shape,
                       std::vector<float>* out, std::vector<uint64_t>* shape) {
   configure();
@@ -1716,20 +1788,8 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     shape->assign({(uint64_t)n, (uint64_t)nt});
     return;
   }
-  DevBuf<float>& margin = pred_margin_; margin.ensure((size_t)n * K);          // scratch kept across calls: no cudaMalloc / cudaFree per request
-  if (!dm->base_margin.empty()) {
-    B200_CHECK(dm->base_margin.size() == (size_t)n * K, "base_margin size does not match rows x groups");
-    CUDA_OK(cudaMemcpyAsync(margin.p, dm->d_base_margin.p, sizeof(float) * n * K, cudaMemcpyDeviceToDevice, s));
-  } else launch_fill(margin.p, n * K, base_margin(), s);
-  if (dart_.on) {            // booster=dart: base + sum_t fl(w_t * leaf_t) in tree order (training=True predicts the same)
-    dm->require_raw("booster=dart");
-    std::vector<int> ids; std::vector<float> coef;
-    for (int t = tb; t < te; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
-    if (!ids.empty()) dart_margin(dm, ids, coef, {}, margin.p, nullptr);
-  } else {
-    pa.margin = margin.p; pa.leaf = nullptr;
-    run_predict(dm, pa, s);
-  }
+  DevBuf<float>& margin = pred_margin_;
+  predict_margin(dm, tb, te);
   int out_cols = K;
   DevBuf<float>& cls = pred_cls_;
   if (type == 0) {

@@ -5,6 +5,7 @@
 #include <memory>
 #include <string>
 #include <vector>
+#include "container_metrics.h"
 #include "curve.h"
 #include "engine.h"
 #include "grow.h"
@@ -50,6 +51,7 @@ class DMatrix {
   // query groups: group g is rows [group_ptr[g], group_ptr[g + 1]) (empty: no groups); under groups a weight is one per group
   std::vector<unsigned> group_ptr;
   RankGroups rank_groups;                             // their device layout, built on first use, reset with the labels, groups or weights
+  ContainerSums container_sums;                       // the container metrics' summation plan and label sums (r2), reset with the labels
   std::vector<std::string> feature_names, feature_types;
   // binned representation (built on first use as a training matrix)
   bool binned = false; int binned_max_bin = 0;
@@ -155,6 +157,9 @@ class Booster {
   void update_one_iter(int iter, DMatrix* dtrain);
   void boost_one_iter(DMatrix* dtrain, const float* grad, const float* hess, size_t len);
   std::string eval_one_iter(int iter, const std::vector<DMatrix*>& dms, const std::vector<std::string>& names);
+  // the raw results of the container's own metrics `names` on dm from the prediction cache (container_metrics.h layout, out
+  // holds kContainerOutLen entries); output_margin: the metric reads margins (feval=) instead of predict()'s values
+  void eval_container_metrics(DMatrix* dm, const std::vector<std::string>& names, bool output_margin, long long* out);
   // inference; returns host buffer + shape
   void predict(DMatrix* dm, int type, bool training, int iter_begin, int iter_end, bool strict_shape,
                std::vector<float>* out, std::vector<uint64_t>* shape);
@@ -203,6 +208,8 @@ class Booster {
   // margins / leaves of trees [pa.tree_begin, pa.tree_end) into pa's outputs: the float predictor, or on a quantile matrix the
   // bin predictor with the model's thresholds mapped to dm's bins first
   void run_predict(DMatrix* dm, PredictArgs pa, cudaStream_t s);
+  // predict()'s margins of trees [tb, te) on dm into pred_margin_ (base margin, then the trees; booster=dart: fl(w_t * leaf_t))
+  void predict_margin(DMatrix* dm, int tb, int te);
   DevBuf<DevNode> bin_nodes_;                   // d_nodes with each split's cond replaced by its bin threshold (run_predict)
   std::map<std::string, std::string> raw_params_;
   std::vector<std::string> eval_metrics_;
@@ -236,6 +243,7 @@ class Booster {
   CoxScratch cox_scratch_;                      // survival:cox: per-round scratch of the gradient and of cox-nloglik
   RankScratch rank_scratch_;                    // rank:* and the ndcg / map metrics: per-call scratch
   CurveScratch curve_scratch_;                  // aucpr and multi-class auc: per-call scratch, grown on first use
+  ContainerScratch container_scratch_;          // the container metrics: per-call scratch, grown on first use
   bool labels_checked_ = false;
   DevBuf<float> pred_margin_, pred_cls_; DevBuf<int> pred_leaf_;      // predict() scratch, grown on demand
   bool children_adjacent_ = true;               // every tree on the device has right child == left child + 1

@@ -772,6 +772,14 @@ int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const
   BST(handle)->debug_gradient(DM(dmat), margin, round, out_gpair);
   API_END();
 }
+int XGB200BoosterEvalContainerMetrics(BoosterHandle handle, DMatrixHandle dmat, const char** names, bst_ulong len, int output_margin,
+                                      long long* out) {
+  API_BEGIN();
+  std::vector<std::string> v;
+  for (bst_ulong i = 0; i < len; ++i) v.emplace_back(names[i]);
+  BST(handle)->eval_container_metrics(DM(dmat), v, output_margin != 0, out);
+  API_END();
+}
 int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out) {
   API_BEGIN();
   std::vector<float> v;

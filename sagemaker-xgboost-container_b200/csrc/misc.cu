@@ -10,26 +10,10 @@
 #include "misc.h"
 #include "predict_tile.h"
 #include "rng.h"
+#include "transform.h"
 #include "traverse.h"
 
 namespace b200 {
-
-__device__ __forceinline__ float sigmoidf_xgb(float x) {
-  const float kEps = 1e-16f;
-  x = fminf(-x, 88.7f);
-  float denom = expf(x) + 1.0f + kEps;
-  return 1.0f / denom;
-}
-// softmax of the margins p[0, K): returns the sum of expf(p[k] - wmax) over k, with wmax the largest margin; class k's
-// probability is expf(p[k] - wmax) / sum (predict() and the multi-class auc / aucpr scores)
-__device__ __forceinline__ float softmax_sum(const float* p, int K, float* wmax_out) {
-  float wmax = p[0];
-  for (int k = 1; k < K; ++k) if (p[k] > wmax) wmax = p[k];
-  float wsum = 0.f;
-  for (int k = 0; k < K; ++k) wsum += expf(p[k] - wmax);
-  *wmax_out = wmax;
-  return wsum;
-}
 
 // ---------------------------------------------------------------------------------------------
 // gradient pairs: one thread per row, all K classes; also the running max|g|, max h of the round.  With dense_g only g is
@@ -280,19 +264,12 @@ __global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, int 
 __global__ void __launch_bounds__(256) transform_kernel(float* m, int64_t n, int K, int objective, float* out_class) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  if (objective == kBinaryLogistic || objective == kRegLogistic) m[r] = sigmoidf_xgb(m[r]);
-  else if (objective == kPoisson || objective == kGamma || objective == kTweedie || objective == kAft || objective == kCox) m[r] = expf(m[r]);
-  else if (objective == kHinge) m[r] = m[r] > 0.0f ? 1.0f : 0.0f;
-  else if (objective == kSoftprob || objective == kSoftmax) {
+  if (objective == kSoftprob || objective == kSoftmax) {
     float* p = m + r * K;
-    if (objective == kSoftmax) {
-      float wmax = p[0]; int arg = 0;
-      for (int k = 1; k < K; ++k) if (p[k] > wmax) { wmax = p[k]; arg = k; }
-      out_class[r] = (float)arg; return;
-    }
+    if (objective == kSoftmax) { out_class[r] = (float)softmax_class(p, K); return; }
     float wmax; const float wsum = softmax_sum(p, K, &wmax);
     for (int k = 0; k < K; ++k) p[k] = expf(p[k] - wmax) / wsum;
-  }
+  } else m[r] = transform_one(m[r], objective);
 }
 
 // the scores of the curve metrics (curve.h): computed here, with this file's flags, so they are predict()'s values bit for bit
