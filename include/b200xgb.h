@@ -47,7 +47,8 @@ XGB_DLL int XGBuildInfo(const char** out);
  * config {"missing": NaN, "nthread": 0}; data_utils.py:384 (Parquet -> numpy), encoder.py:52 (CSV payload) reach it */
 XGB_DLL int XGDMatrixCreateFromDense(const char* data, const char* config, DMatrixHandle* out);
 /* labels / weights / base_margin from an array interface (DMatrix(label=...), data_utils.py:384); "group" (query group sizes) and
- * "qid" (one query id per row, non-decreasing; groups are its runs) from DMatrix(group=...) / DMatrix(qid=...) / set_info */
+ * "qid" (one query id per row, non-decreasing; groups are its runs) from DMatrix(group=...) / DMatrix(qid=...) / set_info.  A 2-D
+ * (n, T) "label" with T > 1 is a multi-target label (its rows must be the matrix's rows); GetFloatInfo returns it flat, row-major */
 XGB_DLL int XGDMatrixSetInfoFromInterface(DMatrixHandle handle, const char* field, const char* data);
 /* {"uri": "<path>?format=csv&label_column=0[&weight_column=1][&delimiter=,]" | "<path>?format=libsvm"}: data_utils.py:309-313,361;
  * a directory means every regular file in it (data_utils.py:520-545); CSV text is parsed on the device; libsvm qid:<id> tokens

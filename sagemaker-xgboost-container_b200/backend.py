@@ -255,9 +255,11 @@ class CudaBackend:
         return out
 
     def dmatrix_set_info_interface(self, h, field, arr):
-        """XGDMatrixSetInfoFromInterface with a 1-D host array (upstream's route for "group" and "qid")."""
-        arr = np.ascontiguousarray(arr).reshape(-1)
-        iface = {"data": [int(arr.ctypes.data), True], "shape": [int(arr.size)], "typestr": arr.dtype.str, "version": 3}
+        """XGDMatrixSetInfoFromInterface with a host array (upstream's route for "group" and "qid"): 1-D, or a 2-D (n, T) label."""
+        arr = np.ascontiguousarray(arr)
+        if arr.ndim != 2:
+            arr = arr.reshape(-1)
+        iface = {"data": [int(arr.ctypes.data), True], "shape": [int(d) for d in arr.shape], "typestr": arr.dtype.str, "version": 3}
         self._check(self.lib.XGDMatrixSetInfoFromInterface(h, _cstr(field), _cstr(json.dumps(iface))))
 
     def dmatrix_set_uint_info(self, h, field, arr):

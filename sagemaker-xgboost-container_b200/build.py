@@ -14,13 +14,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "lib", "libb200xgb.so")
-SOURCES = ["hist.cu", "tree.cu", "misc.cu", "predict_bins.cu", "quantile.cu", "auc.cu", "curve.cu", "container_metrics.cu", "shap.cu", "dart.cu", "survival.cu", "rank.cu", "adaptive.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
+SOURCES = ["hist.cu", "tree.cu", "misc.cu", "predict_bins.cu", "quantile.cu", "auc.cu", "curve.cu", "container_metrics.cu", "shap.cu", "dart.cu", "survival.cu", "rank.cu", "adaptive.cu", "multi_target.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
          "-diag-suppress", "177", "-I", os.path.join(HERE, "..", "include")]
 # survival.cu and rank.cu compute their objectives, curve.cu its aucpr / auc terms, in double: no fused multiply-adds, so they
-# round like a host restatement of the formulas.  container_metrics.cu keeps the default flags of misc.cu: both inline
-# predict()'s transform (csrc/transform.h), and --fmad=false would split the multiply-add inside expf
+# round like a host restatement of the formulas.  container_metrics.cu and multi_target.cu keep the default flags of misc.cu:
+# they inline predict()'s transform (csrc/transform.h) or the per-element formulas (csrc/elementwise.h), and --fmad=false
+# would split the multiply-add inside expf
 EXTRA_FLAGS = {"survival.cu": ["--fmad=false"], "rank.cu": ["--fmad=false"], "curve.cu": ["--fmad=false"]}
 
 

@@ -157,7 +157,13 @@ class DMatrix:
         return get_backend().dmatrix_get_float_info(self.handle, field)
 
     def set_label(self, label):
-        self.set_float_info("label", label)
+        """A 1-D label, or an (n, T) numpy / pandas one for multi-target regression (T label columns); an (n, 1) label is the 1-D
+        label.  get_label() returns the labels flat, row-major."""
+        a = label.to_numpy(dtype=np.float32, na_value=np.nan) if _is_pandas_df(label) else np.asarray(label, dtype=np.float32)
+        if a.ndim == 2 and a.shape[1] > 1:
+            get_backend().dmatrix_set_info_interface(self.handle, "label", np.ascontiguousarray(a))
+        else:
+            self.set_float_info("label", a)
 
     def set_weight(self, weight):
         self.set_float_info("weight", weight)
@@ -396,7 +402,8 @@ class QuantileDMatrix(DMatrix):
                     a = a if a.dtype.kind in "iu" else a.astype(np.float64)
                 else:
                     a = a.astype(np.float32)
-                a = np.ascontiguousarray(a).reshape(-1)
+                # an (n, T) label with T > 1 keeps its shape: a multi-target label, T the same in every batch
+                a = np.ascontiguousarray(a) if field == "label" and a.ndim == 2 and a.shape[1] > 1 else np.ascontiguousarray(a).reshape(-1)
                 state["keep"].append(a)
                 be.dmatrix_set_info_interface(proxy, field, a)
             if state["names"] is None:
@@ -481,7 +488,7 @@ _IGNORED_PARAMS = {
     "validate_parameters", "max_cat_to_onehot", "max_cat_threshold",
     "lambda_bias", "feature_selector", "top_k",
     "disable_default_eval_metric",
-    "multi_strategy", "max_cached_hist_node", "random_state",
+    "max_cached_hist_node", "random_state",
 }
 
 

@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstring>
 #include "comm.h"
+#include "multi_target.h"
 #include "rng.h"
 
 namespace b200 {
@@ -145,7 +146,7 @@ std::unique_ptr<DMatrix> DMatrix::slice(const int* idx, int64_t len, bool allow_
   }
   auto take = [&](const std::vector<float>& src, size_t per_row) { std::vector<float> o; if (src.empty()) return o; o.resize(len * per_row);
     for (int64_t i = 0; i < len; ++i) for (size_t k = 0; k < per_row; ++k) o[i * per_row + k] = src[(size_t)idx[i] * per_row + k]; return o; };
-  if (!labels.empty()) { auto v = take(labels, 1); dm->set_float_info("label", v.data(), v.size()); }
+  if (!labels.empty()) { auto v = take(labels, (size_t)label_cols); dm->set_label_matrix(v.data(), len, label_cols); }      // whole label rows
   if (!group_ptr.empty()) {
     dm->set_group_ptr(ptr);
     if (!weights.empty()) {
@@ -166,7 +167,7 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
     h.assign(v, v + len); d.alloc(len);
     if (len) { CUDA_OK(cudaMemcpyAsync(d.p, h.data(), sizeof(float) * len, cudaMemcpyHostToDevice, s)); Comm::get().sync_stream(s); }
   };
-  if (field == "label") { put(labels, d_labels); cox_order.valid = false; rank_groups.valid = false; container_sums.labels_valid = false; }
+  if (field == "label") { put(labels, d_labels); label_cols = 1; cox_order.valid = false; rank_groups.valid = false; container_sums.labels_valid = false; }
   else if (field == "label_lower_bound") put(label_lower, d_label_lower);      // survival:aft; the bins do not depend on them
   else if (field == "label_upper_bound") put(label_upper, d_label_upper);
   else if (field == "weight") {
@@ -178,6 +179,13 @@ void DMatrix::set_float_info(const std::string& field, const float* v, size_t le
   }
   else if (field == "base_margin") put(base_margin, d_base_margin);
   else throw Error("Unknown float field name: " + field);
+}
+
+void DMatrix::set_label_matrix(const float* v, int64_t rows, int64_t cols) {
+  B200_CHECK(cols >= 1 && cols <= INT_MAX, "label: a 2-D label needs at least one column");
+  B200_CHECK(rows == n, "label: the label has " + std::to_string(rows) + " rows but the DMatrix has " + std::to_string(n));
+  set_float_info("label", v, (size_t)(rows * cols));
+  label_cols = (int)cols;
 }
 
 void DMatrix::set_group_ptr(std::vector<unsigned> ptr) {
@@ -342,7 +350,7 @@ void DMatrix::ensure_binned(int max_bin) {
 // QuantileDMatrix: binned from batches, no float copy of the whole matrix (DESIGN.md "QuantileDMatrix")
 // ---------------------------------------------------------------------------------------------
 void ProxyBatch::set_float_info(const std::string& field, const float* v, size_t len) {
-  if (field == "label") labels.assign(v, v + len);
+  if (field == "label") { labels.assign(v, v + len); label_cols = 1; }
   else if (field == "weight") {
     for (size_t i = 0; i < len; ++i) B200_CHECK(v[i] >= 0 && !std::isnan(v[i]), "Weights must be positive values.");
     weights.assign(v, v + len);
@@ -412,6 +420,7 @@ std::unique_ptr<DMatrix> DMatrix::from_batches(ProxyBatch* proxy, const std::fun
   std::vector<std::vector<FeatureSummary>> per_batch;
   std::vector<float> labels, weights, base_margin, lower, upper, w0;
   std::vector<int64_t> qid;
+  int label_cols = 0;                                 // T of the batches' labels (0: no batch had labels yet)
   int64_t nmiss_total = 0;
   auto summarise = [&](const float* dX, int64_t nr, const std::vector<float>& w) {
     if (!w.empty()) { wbuf.ensure(w.size()); CUDA_OK(cudaMemcpyAsync(wbuf.p, w.data(), sizeof(float) * w.size(), cudaMemcpyHostToDevice, s)); }
@@ -435,7 +444,15 @@ std::unique_ptr<DMatrix> DMatrix::from_batches(ProxyBatch* proxy, const std::fun
     int64_t nm = 0;
     const float* dX = stage_batch(p, missing, b == 0, scratch, &nm, s);
     nmiss_total += nm; rows.push_back(p.n);
-    append(labels, p.labels, p.n, b, "labels"); append(weights, p.weights, p.n, b, "weights"); append(base_margin, p.base_margin, p.n, b, "base_margin");
+    if (!p.labels.empty()) {
+      B200_CHECK(label_cols == 0 || p.label_cols == label_cols, "QuantileDMatrix: batch " + std::to_string(b) + " has a label of " + std::to_string(p.label_cols) +
+                 " columns, an earlier batch one of " + std::to_string(label_cols) + "; every batch's label must have the same number of columns");
+      label_cols = p.label_cols;
+      B200_CHECK((int64_t)p.labels.size() == p.n * p.label_cols, "QuantileDMatrix: batch " + std::to_string(b) + " has " + std::to_string(p.labels.size()) +
+                 " labels for " + std::to_string(p.n) + " rows");
+      labels.insert(labels.end(), p.labels.begin(), p.labels.end());
+    }
+    append(weights, p.weights, p.n, b, "weights"); append(base_margin, p.base_margin, p.n, b, "base_margin");
     append(lower, p.label_lower, p.n, b, "label_lower_bound"); append(upper, p.label_upper, p.n, b, "label_upper_bound");
     B200_CHECK(p.qid.empty() || (int64_t)p.qid.size() == p.n, "QuantileDMatrix: batch " + std::to_string(b) + " has " + std::to_string(p.qid.size()) + " qid for " + std::to_string(p.n) + " rows");
     qid.insert(qid.end(), p.qid.begin(), p.qid.end());
@@ -503,9 +520,11 @@ std::unique_ptr<DMatrix> DMatrix::from_batches(ProxyBatch* proxy, const std::fun
     B200_CHECK(v.empty() || (int64_t)v.size() == n, std::string("QuantileDMatrix: ") + what + " must be given for every batch or for none (" +
                std::to_string(v.size()) + " for " + std::to_string(n) + " rows)");
   };
-  need_all(labels, "labels"); need_all(weights, "weights"); need_all(lower, "label_lower_bound"); need_all(upper, "label_upper_bound");
+  B200_CHECK(labels.empty() || (int64_t)labels.size() == n * label_cols, "QuantileDMatrix: labels must be given for every batch or for none (" +
+             std::to_string(labels.size() / std::max(label_cols, 1)) + " label rows for " + std::to_string(n) + " rows)");
+  need_all(weights, "weights"); need_all(lower, "label_lower_bound"); need_all(upper, "label_upper_bound");
   B200_CHECK(qid.empty() || (int64_t)qid.size() == n, "QuantileDMatrix: qid must be given for every batch or for none");
-  if (!labels.empty()) dm->set_float_info("label", labels.data(), labels.size());
+  if (!labels.empty()) dm->set_label_matrix(labels.data(), n, label_cols);
   if (!weights.empty()) dm->set_float_info("weight", weights.data(), weights.size());
   if (!base_margin.empty()) dm->set_float_info("base_margin", base_margin.data(), base_margin.size());
   if (!lower.empty()) dm->set_float_info("label_lower_bound", lower.data(), lower.size());
@@ -557,7 +576,7 @@ Booster::~Booster() {
   for (auto& p : pending_) if (p.ready) cudaEventDestroy(p.ready);
 }
 
-static const std::map<std::string, int>& objective_table() {
+const std::map<std::string, int>& objective_table() {
   static const std::map<std::string, int> t = {{"reg:squarederror", kSquaredError}, {"reg:linear", kSquaredError}, {"binary:logistic", kBinaryLogistic},
     {"reg:logistic", kRegLogistic}, {"binary:logitraw", kLogitRaw}, {"multi:softprob", kSoftprob}, {"multi:softmax", kSoftmax},
     {"reg:squaredlogerror", kSquaredLogError}, {"reg:pseudohubererror", kPseudoHuber}, {"count:poisson", kPoisson}, {"reg:gamma", kGamma},
@@ -744,10 +763,16 @@ void Booster::configure() {
   }
   auto bs = raw_params_.find("base_score");
   if (bs != raw_params_.end() && !bs->second.empty()) {
+    B200_CHECK(bs->second.find_first_of("[,") == std::string::npos, "base_score: a vector base_score (one value per target) is not supported; give one number (got " +
+               bs->second + ")");
     base_score_ = std::stof(bs->second); base_score_set_ = true;
     if (p.objective == kBinaryLogistic || p.objective == kRegLogistic || p.objective == kLogitRaw)
       B200_CHECK(base_score_ > 0.0f && base_score_ < 1.0f, "Check failed: base_score > 0.0f && base_score < 1.0f base_score must be in (0,1) for logistic loss");
   }
+  if (auto ms = raw_params_.find("multi_strategy"); ms != raw_params_.end())
+    B200_CHECK(ms->second == "one_output_per_tree" || ms->second == "multi_output_tree", "Invalid value for parameter multi_strategy: " + ms->second +
+               " (one_output_per_tree, multi_output_tree)");
+  p.num_target = num_target_;
   if (!p.lossguide) B200_CHECK(p.max_depth >= 1, "max_depth=" + std::to_string(p.max_depth) + " (no depth limit) needs grow_policy=lossguide with max_leaves; the depth-wise builder takes max_depth in [1, 16]");
   if (p.max_bin > 256) p.max_bin = 256;            // uint8 bin codes (the Python layer warns)
   // process_type=update (upstream GBTree): updater is a list of refresh / prune, "refresh,prune" or the "(refresh,prune)" of a
@@ -801,15 +826,23 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
   if (objective_is_log_link(param_.objective) || param_.objective == kHinge || objective_is_survival(param_.objective) || objective_is_rank(param_.objective)) { base_score_ = 0.5f; return; }
   cudaStream_t s = engine_stream();
   TreeBuilder& b = *builder_;
+  const int T = param_.num_target;
   if (param_.objective == kAbsoluteError) {
     // the median of the labels over every rank's rows, weighted when there are weights (on the fixed-point grid of the
     // weights, adaptive.h); upstream averages each worker's median [UPSTREAM-RECALL: MeanAbsoluteError::InitEstimation]
-    // sizing the refresh's buffers first (and dropping any captured tree if they move) leaves none for the select to move
-    b.ensure_adaptive();
-    float med = 0.0f;
-    segmented_quantile(dtrain->d_labels.p, nullptr, dtrain->weights.empty() ? nullptr : dtrain->d_weights.p, dtrain->n, b.global_n, 1, 0.5,
-                       &med, &b.adapt, s);
-    base_score_ = std::isnan(med) ? 0.0f : med;
+    // sizing the refresh's buffers first (and dropping any captured tree if they move) leaves none for the select to move.
+    // Multi-target: the mean of the T columns' medians, in double, in target order (DESIGN.md "Multi-target regression")
+    b.ensure_adaptive(param_.num_outputs());
+    DevBuf<float> col; if (T > 1) col.alloc((size_t)std::max<int64_t>(dtrain->n, 1));
+    double sum = 0.0;
+    for (int j = 0; j < T; ++j) {
+      if (T > 1) launch_label_column(dtrain->d_labels.p, dtrain->n, T, j, col.p, s);
+      float med = 0.0f;
+      segmented_quantile(T > 1 ? col.p : dtrain->d_labels.p, nullptr, dtrain->weights.empty() ? nullptr : dtrain->d_weights.p, dtrain->n, b.global_n, 1, 0.5,
+                         &med, &b.adapt, s);
+      sum += std::isnan(med) ? 0.0 : (double)med;
+    }
+    base_score_ = (float)(sum / (double)T);
     return;
   }
   if (param_.objective == kQuantileError) {
@@ -840,18 +873,31 @@ void Booster::estimate_base_score(DMatrix* dtrain) {
     base_score_ = (float)(meanq * sw / (sw + 1e-6));
     return;
   }
-  GradArgs ga{}; ga.margin = nullptr; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
-  ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = nullptr; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = 1; ga.objective = param_.objective;
-  ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = 1.0f; ga.seed = 0; ga.iter = 0; ga.aux = objective_aux(param_);
-  dsum_.ensure(4);
-  CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 4 * sizeof(double), s));
-  launch_gradient(ga, s);
-  launch_sum_gpair(b.gpair.p, dtrain->n, dsum_.p, s);
-  Comm::get().allreduce_sum_f64(dsum_.p, 2, s);
-  double h[2];
-  CUDA_OK(cudaMemcpyAsync(h, dsum_.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  // Multi-target: each target's stump as the single-target one, then their mean in margin space, in double, in target order
+  // [UPSTREAM-RECALL: FitIntercept::InitEstimation fits the stump of every target, takes their mean, then PredTransform]
+  const size_t nsum = std::max<size_t>(4, 2 * (size_t)T);
+  dsum_.ensure(nsum);
+  CUDA_OK(cudaMemsetAsync(dsum_.p, 0, nsum * sizeof(double), s));
+  if (T == 1) {
+    GradArgs ga{}; ga.margin = nullptr; ga.label = dtrain->d_labels.p; ga.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
+    ga.gpair = b.gpair.p; ga.gp_stride = b.gp_stride; ga.absmax = nullptr; ga.err = b.err.p; ga.n = dtrain->n; ga.row_offset = 0; ga.K = 1; ga.objective = param_.objective;
+    ga.scale_pos_weight = param_.scale_pos_weight; ga.subsample = 1.0f; ga.seed = 0; ga.iter = 0; ga.aux = objective_aux(param_);
+    launch_gradient(ga, s);
+  } else {
+    MultiGradArgs ma{}; ma.margin = nullptr; ma.label = dtrain->d_labels.p; ma.weight = dtrain->weights.empty() ? nullptr : dtrain->d_weights.p;
+    ma.gpair = b.gpair.p; ma.resid = nullptr; ma.absmax = nullptr; ma.err = b.err.p; ma.n = dtrain->n; ma.row_offset = 0; ma.gp_stride = b.gp_stride;
+    ma.T = T; ma.objective = param_.objective; ma.per_target = 0; ma.scale_pos_weight = param_.scale_pos_weight; ma.subsample = 1.0f;
+    ma.aux = objective_aux(param_); ma.seed = 0; ma.iter = 0;
+    launch_multi_target_gradient(ma, s);
+  }
+  for (int j = 0; j < T; ++j) launch_sum_gpair(b.gpair.p + (size_t)j * b.gp_stride, dtrain->n, dsum_.p + 2 * j, s);
+  Comm::get().allreduce_sum_f64(dsum_.p, 2 * (size_t)T, s);
+  std::vector<double> h(2 * (size_t)T);
+  CUDA_OK(cudaMemcpyAsync(h.data(), dsum_.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
   Comm::get().sync_stream(s);
-  float w = h[1] <= 0.0 ? 0.0f : (float)(-h[0] / h[1]);
+  double wsum = 0.0;
+  for (int j = 0; j < T; ++j) wsum += (double)(h[2 * j + 1] <= 0.0 ? 0.0f : (float)(-h[2 * j] / h[2 * j + 1]));
+  float w = (float)(wsum / (double)T);
   // binary:logitraw keeps base_score in probability space like the other logistic objectives (the estimated stump weight
   // w is a margin; storing it raw and taking its logit again gives NaN whenever w <= 0, i.e. whenever mean(y) < 0.5)
   if (param_.objective == kBinaryLogistic || param_.objective == kRegLogistic || param_.objective == kLogitRaw) {
@@ -1033,7 +1079,7 @@ void Booster::dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::v
 }
 
 static void check_labels(const DMatrix* dm) {
-  B200_CHECK(dm->labels.size() == (size_t)dm->n, "Check failed: preds.size() == info.labels_.size() (" + std::to_string(dm->n) + " vs. " +
+  B200_CHECK(dm->labels.size() == (size_t)dm->n * dm->label_cols, "Check failed: preds.size() == info.labels_.size() (" + std::to_string(dm->n) + " vs. " +
              std::to_string(dm->labels.size()) + ") : labels are not correctly provided");
 }
 // survival:aft reads the interval bounds instead of the label
@@ -1050,6 +1096,23 @@ static void check_row_weights(const DMatrix* dm) {
 static void check_train_width(const DMatrix* dm) {
   B200_CHECK(dm->F <= kMaxTrainFeatures, "the CUDA hist builder trains on at most " + std::to_string(kMaxTrainFeatures) + " features (the data has " +
              std::to_string(dm->F) + ")");
+}
+
+void Booster::check_targets(const DMatrix* dm, bool training) {
+  configure();
+  const int T = dm->label_cols;
+  if (T > 1) {
+    // [UPSTREAM-RECALL: ObjFunction::Targets defaults to "multioutput is not supported by the current objective function"]
+    B200_CHECK(objective_is_multi_target(param_.objective), "multi-target: the label has " + std::to_string(T) + " columns, but objective " + objective_name_ +
+               " does not support a label with more than one column (multioutput is not supported by the current objective function); the multi-target "
+               "objectives are reg:squarederror, reg:squaredlogerror, reg:pseudohubererror, reg:logistic, binary:logistic, binary:logitraw and reg:absoluteerror");
+    auto ms = raw_params_.find("multi_strategy");
+    B200_CHECK(ms == raw_params_.end() || ms->second != "multi_output_tree", "multi-target: multi_strategy=multi_output_tree (one tree with a vector leaf for all "
+               "targets) is not implemented on the CUDA hist path; use multi_strategy=one_output_per_tree");
+    B200_CHECK(!update_mode_, "multi-target: process_type=update is not implemented for a label with more than one column");
+  }
+  if (training && T != num_target_ && layers() == 0 && !update_mode_) { num_target_ = T; configured_ = false; configure(); }
+  B200_CHECK(T == num_target_, "multi-target: the label has " + std::to_string(T) + " column(s) but the model has num_target = " + std::to_string(num_target_));
 }
 
 // label-range errors must surface from update() (the container maps them to UserError, train.py:461-467)
@@ -1087,7 +1150,7 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   configure();
   (void)iter;
   cudaStream_t s = engine_stream();
-  if (param_.objective == kAft) check_aft_bounds(dtrain); else check_labels(dtrain);
+  if (param_.objective == kAft) check_aft_bounds(dtrain); else { check_targets(dtrain, true); check_labels(dtrain); }
   B200_CHECK(param_.objective != kCox || !Comm::get().distributed(), "survival:cox is not supported with more than one GPU (world_size > 1): its risk sets span the rows of every rank");
   if (num_feature_ == 0) num_feature_ = dtrain->F;
   B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
@@ -1126,9 +1189,10 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   // likewise constant-hessian growth never meets a gradient-based sample, whose kept rows have h / p != 1
   B200_CHECK(!(dense_g && gbs), "gradient-based sampling of a constant-hessian round");
   CUDA_OK(cudaMemsetAsync(b.gs.absmax, 0, 8, s));
-  // reg:quantileerror without a per-tree or gradient-based sample: each target's trees grow on the grid of its own gradients
-  // (upstream quantises each tree's gradients by themselves), so a target's trees do not depend on the other targets
-  const bool per_target_grid = param_.objective == kQuantileError && !per_tree_sample && !gbs;
+  // reg:quantileerror and multi-target models without a per-tree or gradient-based sample: each target's trees grow on the grid
+  // of its own gradients (upstream quantises each tree's gradients by themselves), so a target's trees do not depend on the
+  // other targets
+  const bool per_target_grid = (param_.objective == kQuantileError || param_.num_target > 1) && !per_tree_sample && !gbs;
   // reg:absoluteerror / reg:quantileerror: the round's residuals of every output, read by the leaf refresh of every tree of the round
   float* resid = objective_is_adaptive(param_.objective) ? b.ensure_adaptive(K) : nullptr;
   if (per_tree_sample) {
@@ -1201,6 +1265,15 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
                                bool dense_g, float* resid, bool per_target_absmax) {
   cudaStream_t s = engine_stream();
   const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
+  if (param_.num_target > 1) {               // multi-target: one pair per label element (multi_target.cu)
+    B200_CHECK(!dense_g, "multi-target gradients are (g,h) pairs");
+    MultiGradArgs ma{}; ma.margin = margin; ma.label = dm->d_labels.p; ma.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
+    ma.gpair = gpair; ma.resid = resid; ma.absmax = absmax; ma.err = builder_->err.p; ma.n = dm->n; ma.row_offset = row_offset; ma.gp_stride = gp_stride;
+    ma.T = param_.num_target; ma.objective = param_.objective; ma.per_target = per_target_absmax ? 1 : 0; ma.scale_pos_weight = param_.scale_pos_weight;
+    ma.subsample = subsample; ma.aux = objective_aux(param_); ma.seed = param_.seed; ma.iter = (unsigned long long)round;
+    launch_multi_target_gradient(ma, s);
+    return;
+  }
   if (param_.objective == kAbsoluteError) {
     AbsErrGradArgs aa{}; aa.margin = margin; aa.label = dm->d_labels.p; aa.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
     aa.gpair = gpair; aa.resid = resid; aa.absmax = absmax; aa.n = dm->n; aa.row_offset = row_offset; aa.subsample = subsample; aa.seed = param_.seed;
@@ -1271,7 +1344,7 @@ const RankGroups& Booster::rank_groups(DMatrix* dm, const char* what) {
 void Booster::debug_gradient(DMatrix* dm, const float* margin, int round, float* out) {
   configure();
   cudaStream_t s = engine_stream();
-  if (param_.objective == kAft) check_aft_bounds(dm); else check_labels(dm);
+  if (param_.objective == kAft) check_aft_bounds(dm); else { check_targets(dm, true); check_labels(dm); }
   dm->ensure_binned(param_.max_bin); builder_for(dm);        // the builder owns the label-error flag gradient_kernel writes
   const int K = param_.num_outputs();
   const int64_t n = dm->n;
@@ -1431,6 +1504,7 @@ void Booster::begin_update() {
 void Booster::refresh_one_iter(DMatrix* dtrain) {
   cudaStream_t s = engine_stream();
   B200_CHECK(!dart_.on, "process_type=update is not implemented for booster=dart");
+  B200_CHECK(num_target_ == 1, "multi-target: process_type=update is not implemented for a model with num_target = " + std::to_string(num_target_));
   check_label_ranges(dtrain);
   if (!update_->started) begin_update();
   UpdateState& u = *update_;
@@ -1561,7 +1635,7 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
   std::string out = "[" + std::to_string(iter) + "]";
   for (size_t i = 0; i < dms.size(); ++i) {
     DMatrix* dm = dms[i];
-    if (param_.objective != kAft) check_labels(dm);
+    if (param_.objective != kAft) { check_targets(dm, false); check_labels(dm); }
     PredCache& c = cache_for(dm);
     bring_cache_up_to_date(dm, c);
     for (const std::string& mname : metrics) {
@@ -1572,6 +1646,13 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
       std::string base = mname;
       if (mname.rfind("tweedie-nloglik@", 0) == 0) { base = "tweedie-nloglik"; ma.aux = std::stof(mname.substr(16)); B200_CHECK(ma.aux >= 1.0f && ma.aux < 2.0f, "tweedie variance power must be in interval [1, 2)"); }
       if (mname.rfind("error@", 0) == 0) { base = "error"; ma.threshold = std::stof(mname.substr(6)); }
+      // multi-target: the element-wise metrics over the n x T elements; auc / aucpr raise below as for any model with several outputs
+      static const std::map<std::string, int> kElementwise = {{"rmse", kMetricRmse}, {"rmsle", kMetricRmsle}, {"mae", kMetricMae}, {"mape", kMetricMape},
+                                                             {"mphe", kMetricMphe}, {"logloss", kMetricLogloss}, {"error", kMetricError}};
+      const auto ew = kElementwise.find(base);
+      if (param_.num_target > 1)
+        B200_CHECK(ew != kElementwise.end() || base == "auc" || base == "aucpr", "multi-target: metric " + mname + " is not implemented for a model with " +
+                   std::to_string(param_.num_target) + " targets (rmse, rmsle, mae, mape, mphe, logloss, error and error@t are)");
       int rank_map = 0, rank_k = 0, rank_minus = 0;
       if (parse_rank_metric(mname, &rank_map, &rank_k, &rank_minus)) {     // ndcg / map over the query groups (rank.cu)
         const RankGroups& rg = rank_groups(dm, mname.c_str());
@@ -1633,7 +1714,13 @@ std::string Booster::eval_one_iter(int iter, const std::vector<DMatrix*>& dms, c
         out += "\t" + names[i] + "-" + mname + ":" + buf;
         continue;
       }
-      if (mname == "aft-nloglik" || mname == "interval-regression-accuracy") {     // at the margin, in double (survival.cu)
+      if (param_.num_target > 1) {               // sum_i sum_j w_i loss(y_ij, p_ij) / (T sum_i w_i) (multi_target.cu)
+        MultiMetricArgs mt{}; mt.margin = c.margin.p; mt.label = dm->d_labels.p; mt.weight = ma.weight; mt.out = dsum_.p; mt.n = dm->n; mt.T = param_.num_target;
+        mt.metric = ew->second; mt.is_logistic = ma.is_logistic || (param_.objective == kLogitRaw && (ew->second == kMetricLogloss || ew->second == kMetricError));
+        mt.transform = ma.transform; mt.threshold = ma.threshold; mt.aux = ew->second == kMetricMphe ? param_.huber_slope : 0.0f;
+        CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
+        launch_multi_target_metric(mt, s);
+      } else if (mname == "aft-nloglik" || mname == "interval-regression-accuracy") {     // at the margin, in double (survival.cu)
         check_aft_bounds(dm);
         CUDA_OK(cudaMemsetAsync(dsum_.p, 0, 2 * sizeof(double), s));
         launch_aft_metric(c.margin.p, dm->d_label_lower.p, dm->d_label_upper.p, ma.weight, dm->n, param_.aft_dist, param_.aft_sigma,
@@ -1702,7 +1789,7 @@ void Booster::eval_container_metrics(DMatrix* dm, const std::vector<std::string>
   const int64_t n = dm->n;
   std::fill(out, out + kContainerOutLen, 0LL);
   out[1] = n; out[2] = P; out[3] = kContainerLabels;
-  if (n == 0 || dm->labels.size() != (size_t)n) return;
+  if (n == 0 || dm->labels.size() != (size_t)n || param_.num_target > 1) return;      // a multi-target model: the container's own function
   want_class = want_class && P <= kContainerLabels;
   want_reg = want_reg && cols == 1 && n <= INT_MAX;
   want_r2 = want_r2 && want_reg;
@@ -1794,7 +1881,8 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
   DevBuf<float>& cls = pred_cls_;
   if (type == 0) {
     if (param_.objective == kSoftmax) { cls.ensure(n); launch_transform(margin.p, n, K, param_.objective, cls.p, s); out_cols = 1; }
-    else launch_transform(margin.p, n, K, param_.objective, nullptr, s);
+    else if (param_.objective == kSoftprob) launch_transform(margin.p, n, K, param_.objective, nullptr, s);
+    else launch_transform(margin.p, n * K, 1, param_.objective, nullptr, s);       // element-wise over the n x K outputs
   }
   out->resize((size_t)n * out_cols);
   if (!out->empty()) CUDA_OK(cudaMemcpyAsync(out->data(), (type == 0 && param_.objective == kSoftmax) ? cls.p : margin.p, sizeof(float) * out->size(), cudaMemcpyDeviceToHost, s));

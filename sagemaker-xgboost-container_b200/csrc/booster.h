@@ -28,8 +28,9 @@ struct ProxyBatch {
   std::vector<float> converted;                       // kHostDense of another dtype, converted to float32
   const size_t* indptr = nullptr; const unsigned* indices = nullptr; const float* values = nullptr; size_t nelem = 0;   // kCSR
   std::vector<float> labels, weights, base_margin, label_lower, label_upper;
+  int label_cols = 1;                                 // labels is [n][label_cols] row-major
   std::vector<int64_t> qid;
-  void clear_meta() { labels.clear(); weights.clear(); base_margin.clear(); label_lower.clear(); label_upper.clear(); qid.clear(); }
+  void clear_meta() { labels.clear(); label_cols = 1; weights.clear(); base_margin.clear(); label_lower.clear(); label_upper.clear(); qid.clear(); }
   void set_float_info(const std::string& field, const float* v, size_t len);
 };
 
@@ -44,6 +45,7 @@ class DMatrix {
   bool quantile = false; int quantile_max_bin = 0;
   DevBuf<float> X;                                    // n x F, NaN = missing (empty on a quantile matrix)
   std::vector<float> labels, weights, base_margin;    // host copies (returned by GetFloatInfo)
+  int label_cols = 1;                                 // T: labels is [n][T] row-major (a multi-target label; 1 from set_float_info)
   DevBuf<float> d_labels, d_weights, d_base_margin;
   std::vector<float> label_lower, label_upper;         // survival:aft interval bounds (label_lower_bound / label_upper_bound)
   DevBuf<float> d_label_lower, d_label_upper;
@@ -86,6 +88,8 @@ class DMatrix {
   // allow_groups: a matrix with groups may be sliced by whole groups, which the slice carries
   std::unique_ptr<DMatrix> slice(const int* idx, int64_t len, bool allow_groups = false) const;
   void set_float_info(const std::string& field, const float* v, size_t len);
+  // a (rows, cols) label, row-major: rows must be the matrix's row count; cols == 1 is the 1-D label
+  void set_label_matrix(const float* v, int64_t rows, int64_t cols);
   void set_group_ptr(std::vector<unsigned> ptr);      // validated: starts at 0, non-decreasing, ends at n
   void set_group_sizes(const unsigned* sizes, size_t len);
   void set_qid(const int64_t* qid, size_t len);       // groups are the runs of equal consecutive qid; qid must not decrease
@@ -220,6 +224,7 @@ class Booster {
   std::string objective_name_ = "reg:squarederror";
   bool base_score_set_ = false; float base_score_ = 0.5f; bool base_score_estimated_ = false;
   int num_feature_ = 0;
+  int num_target_ = 1;                          // label columns of the model (multi-target regression), fixed by its first round
   std::vector<HostTree> trees_; std::vector<int> tree_info_;
   // boosting round (layer) r holds trees [iteration_indptr_[r], iteration_indptr_[r + 1]): K * num_parallel_tree of them,
   // class-major.  The only round <-> tree map; always starts with 0 and ends with trees_.size()
@@ -255,6 +260,8 @@ class Booster {
 
   void configure();
   void check_label_ranges(const DMatrix* dtrain);
+  // a matrix's label width against the model: the first round of an empty model takes T from dtrain; the rejections of T > 1
+  void check_targets(const DMatrix* dm, bool training);
   const RankGroups& rank_groups(DMatrix* dm, const char* what);   // dm's groups on the device; checks one weight per group
   void begin_update();                               // the model's layers become the trees to update; the model is emptied
   void refresh_one_iter(DMatrix* dtrain);            // one update round: the next layer refreshed / pruned into the model
@@ -290,6 +297,8 @@ class Booster {
   void reset_model();
 };
 
+// objective name -> engine.h Objective (booster.cu)
+const std::map<std::string, int>& objective_table();
 // quantile_alpha in any of its accepted forms (booster.cu); raises on a malformed, empty or out-of-range value
 std::vector<float> parse_quantile_alpha(const std::string& v);
 std::string colsample_mask(unsigned seed, int tree_index, int F, float frac);   // bytes, 1 = feature usable

@@ -160,11 +160,12 @@ int XGDMatrixSetInfoFromInterface(DMatrixHandle handle, const char* field, const
     ProxyBatch* p = PROXY(handle);
     B200_CHECK(f != "group", "QuantileDMatrix: give query groups per batch as qid, not group");
     if (f == "qid") p->qid = to_int64(h, field);
-    else { std::vector<float> v = to_float32(h); p->set_float_info(f, v.data(), v.size()); }
+    else { std::vector<float> v = to_float32(h); p->set_float_info(f, v.data(), v.size()); if (f == "label") p->label_cols = (int)std::max<int64_t>(h.m, 1); }
     return 0;
   }
   if (f == "qid") { std::vector<int64_t> q = to_int64(h, field); DM(handle)->set_qid(q.data(), q.size()); }
   else if (f == "group") { std::vector<unsigned> g = to_group_sizes(to_int64(h, field)); DM(handle)->set_group_sizes(g.data(), g.size()); }
+  else if (f == "label" && h.m > 1) { std::vector<float> v = to_float32(h); DM(handle)->set_label_matrix(v.data(), h.n, h.m); }   // (n, T): multi-target
   else { std::vector<float> v = to_float32(h); DM(handle)->set_float_info(field, v.data(), v.size()); }
   API_END();
 }

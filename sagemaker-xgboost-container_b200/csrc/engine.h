@@ -135,9 +135,10 @@ struct TrainParam {
   // lambdarank_normalization, lambdarank_score_normalization, lambdarank_bias_norm (inert: lambdarank_unbiased is rejected)
   // lambdarank_unbiased=true is read and written, and a model with it predicts, but it does not train
   int rank_mean = 0, rank_unbiased = 0, rank_k = 32, rank_exp_gain = 1, rank_normalization = 1, rank_score_normalization = 1; float rank_bias_norm = 2.0f;
+  int num_target = 1;            // label columns of a multi-target model (multi_target.h; the model's learner_model_param.num_target)
   // Outputs per row: margin columns, trees per round and layer (times num_parallel_tree), prediction columns.  num_class
   // itself is the class count of multi:* (softmax, merror / mlogloss) and 1 otherwise.
-  int num_outputs() const { return objective == kQuantileError ? (int)quantile_alpha.size() : num_class; }
+  int num_outputs() const { return objective == kQuantileError ? (int)quantile_alpha.size() : num_target > 1 ? num_target : num_class; }
 };
 
 // ---------------------------------------------------------------------------------------------

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <utility>
 #include "curve.h"
+#include "elementwise.h"
 #include "engine.h"
 #include "misc.h"
 #include "predict_tile.h"
@@ -44,45 +45,9 @@ __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
         mg = fmaxf(mg, fabsf(g)); mh = fmaxf(mh, h);
       }
     } else {
-      const bool reg_loss = a.objective <= kLogitRaw || a.objective == kSquaredLogError || a.objective == kPseudoHuber;     // RegLossObj family
-      if (reg_loss && y == 1.0f) w *= a.scale_pos_weight;
-      float p = a.margin ? a.margin[r] : 0.f, g, h;
-      // upstream src/objective/regression_loss.h (RegLossObj family), regression_obj.cu (Poisson / Gamma / Tweedie), hinge.cu
-      switch (a.objective) {
-        case kSquaredError: g = p - y; h = 1.0f; break;
-        case kSquaredLogError: {
-          if (!(y > -1.0f)) *a.err = 3;
-          p = fmaxf(p, -1.0f + 1e-6f);
-          g = (log1pf(p) - log1pf(y)) / (p + 1.0f);
-          h = fmaxf((-log1pf(p) + log1pf(y) + 1.0f) / ((p + 1.0f) * (p + 1.0f)), 1e-6f);
-          break; }
-        case kPseudoHuber: {
-          const float z = p - y, s2 = a.aux * a.aux, scale_sqrt = sqrtf(1.0f + z * z / s2);
-          g = z / scale_sqrt; h = s2 / ((s2 + z * z) * scale_sqrt);
-          break; }
-        case kPoisson: {
-          if (y < 0.0f) *a.err = 4;
-          g = expf(p) - y; h = expf(p + a.aux);
-          break; }
-        case kGamma: {
-          if (!(y > 0.0f)) *a.err = 5;
-          const float ep = expf(p);
-          g = 1.0f - y / ep; h = y / ep;
-          break; }
-        case kTweedie: {
-          if (y < 0.0f) *a.err = 6;
-          const float rho = a.aux, e1 = expf((1.0f - rho) * p), e2 = expf((2.0f - rho) * p);
-          g = -y * e1 + e2; h = -y * (1.0f - rho) * e1 + (2.0f - rho) * e2;
-          break; }
-        case kHinge: {
-          const float yy = y * 2.0f - 1.0f;
-          if (p * yy < 1.0f) { g = -yy; h = 1.0f; } else { g = 0.0f; h = 1.17549435e-38f; }      // upstream: numeric_limits<float>::min()
-          break; }
-        default: {
-          if (y < 0.0f || y > 1.0f) *a.err = 1;
-          p = sigmoidf_xgb(p); g = p - y; h = fmaxf(p * (1.0f - p), 1e-16f);
-          break; }
-      }
+      if (objective_is_reg_loss(a.objective) && y == 1.0f) w *= a.scale_pos_weight;
+      float g, h;
+      elementwise_gradient(a.objective, y, a.margin ? a.margin[r] : 0.f, a.aux, a.err, &g, &h);
       g *= w; h *= w;
       if (dropped) { g = 0.f; h = 0.f; }
       if (a.dense_g) reinterpret_cast<float*>(a.gpair)[r] = g; else a.gpair[r] = make_float2(g, h);
@@ -313,30 +278,7 @@ __global__ void __launch_bounds__(256) metric_kernel(MetricArgs a) {
         loss = p > eps ? -logf(p) : -logf(eps);
       }
     } else {
-      float p = a.margin[r];
-      if (a.is_logistic || a.transform == kTransformSigmoid) p = sigmoidf_xgb(p);
-      else if (a.transform == kTransformExp) p = expf(p);
-      else if (a.transform == kTransformHinge) p = p > 0.0f ? 1.0f : 0.0f;
-      switch (a.metric) {          // upstream src/metric/elementwise_metric.cu
-        case kMetricRmsle: { float d = log1pf(y) - log1pf(p); loss = d * d; break; }
-        case kMetricMape: loss = fabsf((y - p) / y); break;
-        case kMetricMphe: { const float z = (y - p) / a.aux; loss = a.aux * a.aux * (sqrtf(1.0f + z * z) - 1.0f); break; }
-        case kMetricPoissonNll: { const float py = fmaxf(p, 1e-16f); loss = lgammaf(y + 1.0f) + py - logf(py) * y; break; }
-        case kMetricGammaNll: { const float py = fmaxf(p, 1e-6f); loss = y / py + logf(py); break; }       // psi = 1: -((y * theta - b) / a + c), theta = -1 / py, b = -log(-theta)
-        case kMetricGammaDeviance: { const float py = p + 1e-6f, yy = y + 1e-6f; loss = logf(py / yy) + yy / py - 1.0f; break; }      // x 2 on the host
-        case kMetricTweedieNll: { const float rho = a.aux, lp = logf(p); loss = -y * expf((1.0f - rho) * lp) / (1.0f - rho) + expf((2.0f - rho) * lp) / (2.0f - rho); break; }
-        case kMetricRmse: { float d = p - y; loss = d * d; break; }
-        case kMetricMae: loss = fabsf(p - y); break;
-        case kMetricLogloss: {
-          const float eps = 1e-16f;
-          float pneg = 1.0f - p;
-          if (p < eps) loss = -y * logf(eps) - (1.0f - y) * logf(1.0f - eps);
-          else if (pneg < eps) loss = -y * logf(1.0f - eps) - (1.0f - y) * logf(eps);
-          else loss = -y * logf(p) - (1.0f - y) * logf(pneg);
-          break; }
-        case kMetricError: loss = (p > a.threshold) ? (1.0f - y) : y; break;
-        default: break;
-      }
+      loss = elementwise_loss(a.metric, y, metric_prediction(a.margin[r], a.is_logistic, a.transform), a.threshold, a.aux);
     }
     s += (double)(loss * w); ws += (double)w;
   }

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdlib>
 #include "booster.h"
+#include "multi_target.h"
 
 namespace b200 {
 
@@ -129,7 +130,7 @@ JPtr Booster::model_to_json() {
   // reader below accepts as well: the reference's own fixture is a [3,2,0] file)
   lmp->set("base_score", S(float_repr(base_score_))); lmp->set("boost_from_average", S("1"));
   lmp->set("num_class", S(std::to_string(K > 1 ? K : 0))); lmp->set("num_feature", S(std::to_string(num_feature_)));
-  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : 1)));
+  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : param_.num_target)));
   learner->set("learner_model_param", lmp);
   JPtr obj = JValue::Object(); obj->set("name", S(objective_name_));
   if (param_.objective == kSoftprob || param_.objective == kSoftmax) { JPtr sp = JValue::Object(); sp->set("num_class", S(std::to_string(K))); obj->set("softmax_multiclass_param", sp); }
@@ -196,6 +197,18 @@ void Booster::model_from_json(const JValue& doc) {
     B200_CHECK(qa != raw_params_.end(), "model: a reg:quantileerror model needs objective.quantile_loss_param.quantile_alpha");
     B200_CHECK((int)parse_quantile_alpha(qa->second).size() == nt, "model: num_target is " + std::to_string(nt) + " but quantile_alpha is " + qa->second);
     K = std::max(1, nt);
+  }
+  // multi-target regression: num_target outputs of one of the multi-target objectives (multi_target.h)
+  num_target_ = 1;
+  if (objective_name_ != "reg:quantileerror" && lmp.has("num_target")) {
+    const int64_t nt = lmp.at("num_target").as_int();
+    B200_CHECK(nt >= 1 && nt <= (1 << 20), "model: num_target must be a positive integer (got " + std::to_string(nt) + ")");
+    auto ot = objective_table().find(objective_name_);
+    B200_CHECK(nt == 1 || (ot != objective_table().end() && objective_is_multi_target(ot->second)), "model: num_target is " + std::to_string(nt) +
+               " but objective " + objective_name_ + " does not support multi-target models (multi-target)");
+    B200_CHECK(nt == 1 || nc <= 1, "model: num_target and num_class cannot both be above 1");
+    num_target_ = (int)nt;
+    if (nt > 1) K = (int)nt;
   }
   for (size_t t = 0; t < trees.arr.size(); ++t) { const double g = tinfo.num_at(t); B200_CHECK(g >= 0 && g < K, "model: tree_info entry out of range"); }
   // the layer layout: iteration_indptr when the document has it (2.x / 3.x), else K * num_parallel_tree trees per round (1.x)
@@ -323,7 +336,7 @@ JPtr Booster::config_to_json() {
   learner->set("gradient_booster", gb);
   JPtr lmp = JValue::Object(); lmp->set("base_score", S(float_repr(base_score_))); lmp->set("boost_from_average", S("1"));
   lmp->set("num_class", S(std::to_string(param_.num_class > 1 ? param_.num_class : 0))); lmp->set("num_feature", S(std::to_string(num_feature_)));
-  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : 1)));
+  lmp->set("num_target", S(std::to_string(param_.objective == kQuantileError ? param_.num_outputs() : param_.num_target)));
   learner->set("learner_model_param", lmp);
   JPtr ltp = JValue::Object(); ltp->set("booster", S(dart_.on ? "dart" : "gbtree")); ltp->set("disable_default_eval_metric", S("0")); ltp->set("multi_strategy", S("one_output_per_tree")); ltp->set("objective", S(objective_name_));
   learner->set("learner_train_param", ltp);
@@ -363,6 +376,14 @@ void Booster::config_from_json(const JValue& doc) {
     aft_params_from_json(*o, &raw_params_);
     quantile_params_from_json(*o, &raw_params_);
     rank_params_from_json(*o, &raw_params_);
+    // a multi-target model's num_target (the model document carries it too; a fresh Booster takes it from the config)
+    if (auto lmp = learner.get("learner_model_param")) if (auto nt = lmp->get("num_target")) if (nt->type == JValue::kString && o->at("name").s != "reg:quantileerror") {
+      auto ot = objective_table().find(o->at("name").s);
+      const int v = std::atoi(nt->s.c_str());
+      if (v > 1) B200_CHECK(ot != objective_table().end() && objective_is_multi_target(ot->second), "config: num_target is " + nt->s + " but objective " +
+                            o->at("name").s + " does not support multi-target models (multi-target)");
+      if (v >= 1) num_target_ = v;
+    }
   }
   if (auto m = learner.get("metrics")) { eval_metrics_.clear(); for (auto& x : m->arr) eval_metrics_.push_back(x->at("name").s); }
   configured_ = false;
@@ -386,6 +407,7 @@ std::unique_ptr<Booster> Booster::slice(int begin, int end, int step) {
   auto b = std::make_unique<Booster>();
   b->raw_params_ = raw_params_; b->eval_metrics_ = eval_metrics_; b->attrs = attrs; b->feature_names = feature_names; b->feature_types = feature_types;
   b->objective_name_ = objective_name_; b->base_score_ = base_score_; b->base_score_set_ = base_score_set_; b->base_score_estimated_ = true; b->num_feature_ = num_feature_;
+  b->num_target_ = num_target_;
   b->raw_params_.erase("base_score"); b->base_score_set_ = true;
   for (int r = begin; r < end; r += step) {
     for (int t = iteration_indptr_[r]; t < iteration_indptr_[r + 1]; ++t) {

@@ -135,6 +135,10 @@ class XGBClassifier(XGBModel):
 
     def fit(self, X, y, *, sample_weight=None, base_margin=None, eval_set=None, verbose=True, xgb_model=None, sample_weight_eval_set=None):
         y = np.asarray(y)
+        if y.ndim == 2 and y.shape[1] > 1:
+            # multi-label classification is not implemented: the label reaches the engine flat, which refuses its n * T entries
+            # ("labels are not correctly provided") rather than training T binary:logistic targets
+            y = y.reshape(-1)
         self.classes_ = np.unique(y)
         self.n_classes_ = len(self.classes_)
         if not np.array_equal(self.classes_, np.arange(self.n_classes_)):
