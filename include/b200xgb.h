@@ -110,7 +110,13 @@ XGB_DLL int XGBoosterFree(BoosterHandle handle);
 XGB_DLL int XGBoosterSetParam(BoosterHandle handle, const char* name, const char* value);
 /* one boosting round of the configured objective on dtrain (the hot path) */
 XGB_DLL int XGBoosterUpdateOneIter(BoosterHandle handle, int iter, DMatrixHandle dtrain);
-/* custom objective: not implemented on the device path, returns -1 */
+/* one boosting round on the caller's gradients (a custom objective): grad and hess are array-interface JSON documents of
+ * shape (rows, outputs) or, with one output, (rows,); float32 or float64; host memory or CUDA memory on the booster's device,
+ * read in place, with optional "strides" (bytes) and "stream" (__cuda_array_interface__ v3: the engine waits for that stream's
+ * work first; null: no wait; no "stream" key: a device synchronise before CUDA memory is read).  Labels are not read; the base score is base_score, else 0.5.  A non-finite value or a negative hessian fails
+ * the call, naming the row, and leaves the model as it was.  iter is unused.  [UPSTREAM-RECALL: 2.x/3.0 c_api.h signature] */
+XGB_DLL int XGBoosterTrainOneIter(BoosterHandle handle, DMatrixHandle dtrain, int iter, const char* grad, const char* hess);
+/* the same round from float32 host arrays of len = rows x outputs each, row-major */
 XGB_DLL int XGBoosterBoostOneIter(BoosterHandle handle, DMatrixHandle dtrain, float* grad, float* hess, bst_ulong len);
 /* "[iter]\t<name>-<metric>:<value>..." -- callback.py:85 EvaluationMonitor parses this */
 XGB_DLL int XGBoosterEvalOneIter(BoosterHandle handle, int iter, DMatrixHandle dmats[], const char* evnames[], bst_ulong len,
@@ -269,6 +275,9 @@ XGB_DLL int XGB200BoosterEvalContainerMetrics(BoosterHandle handle, DMatrixHandl
                                               long long* out);
 /* raw margins of the prediction cache the trainer keeps for `dmat` (n x outputs per row), brought up to date first */
 XGB_DLL int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out);
+/* the margins a custom objective sees before the next round on dtrain: the prediction cache (rows x cols, row-major, valid until
+ * the next call on the handle), with the outputs a first round takes from dtrain's label columns */
+XGB_DLL int XGB200BoosterGetTrainingMargin(BoosterHandle handle, DMatrixHandle dtrain, bst_ulong* out_rows, bst_ulong* out_cols, const float** out);
 /* the weight of every tree in model order (booster=dart: weight_drop; 1 for gbtree); out may be NULL to query the length */
 XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, float* out);
 /* process_type=update: the exact fixed-point (G_q, H_q) sums of every node of every tree being updated, in the node order of the

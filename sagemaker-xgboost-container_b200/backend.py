@@ -567,6 +567,30 @@ class CudaBackend:
                                                                out.ctypes.data_as(C.POINTER(C.c_longlong))))
         return out
 
+    @staticmethod
+    def _gradient_iface(a):
+        if isinstance(a, np.ndarray):     # C-contiguous (n, K), core._gradient_array
+            return {"data": [int(a.ctypes.data), True], "shape": [int(d) for d in a.shape], "typestr": a.dtype.str, "strides": None, "version": 3}
+        iface = a.__cuda_array_interface__
+        out = {"data": [int(iface["data"][0]), False], "shape": [int(d) for d in iface["shape"]], "typestr": iface["typestr"],
+               "strides": [int(d) for d in iface["strides"]], "version": 3}
+        if "stream" in iface:                # absent: the engine synchronises the device before reading the array
+            out["stream"] = None if iface["stream"] is None else int(iface["stream"])
+        return out
+
+    def booster_boost(self, bh, dh, it, grad, hess):
+        """XGBoosterTrainOneIter: one round on (n, K) gradients, numpy arrays or CUDA array views (core._gradient_array)."""
+        self._check(self.lib.XGBoosterTrainOneIter(bh, dh, C.c_int(it), _cstr(json.dumps(self._gradient_iface(grad))),
+                                                   _cstr(json.dumps(self._gradient_iface(hess)))))
+
+    def booster_training_margin(self, bh, dh):
+        """The margins a custom objective sees before the next round on dh: float32 (n, K), a copy."""
+        rows, cols, ptr = c_bst_ulong(), c_bst_ulong(), C.POINTER(C.c_float)()
+        self._check(self.lib.XGB200BoosterGetTrainingMargin(bh, dh, C.byref(rows), C.byref(cols), C.byref(ptr)))
+        if rows.value * cols.value == 0:
+            return np.zeros((rows.value, cols.value), np.float32)
+        return np.ctypeslib.as_array(ptr, shape=(rows.value, cols.value)).copy()
+
     def booster_cached_margin(self, bh, dh, K):
         n = self.dmatrix_num_row(dh)
         out = np.zeros((n, K), np.float32)

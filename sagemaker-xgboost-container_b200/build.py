@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "lib", "libb200xgb.so")
-SOURCES = ["hist.cu", "tree.cu", "misc.cu", "predict_bins.cu", "quantile.cu", "auc.cu", "curve.cu", "container_metrics.cu", "shap.cu", "dart.cu", "survival.cu", "rank.cu", "adaptive.cu", "multi_target.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
+SOURCES = ["hist.cu", "tree.cu", "misc.cu", "predict_bins.cu", "quantile.cu", "auc.cu", "curve.cu", "container_metrics.cu", "shap.cu", "dart.cu", "survival.cu", "rank.cu", "adaptive.cu", "multi_target.cu", "custom_grad.cu", "sampling.cu", "refresh.cu", "csv.cu", "recordio.cu", "ingest.cu", "nvlink.cu", "grow.cu", "booster.cu", "model_io.cc", "legacy_io.cc", "comm.cc", "capi.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-fvisibility=hidden",
          "-diag-suppress", "177", "-I", os.path.join(HERE, "..", "include")]

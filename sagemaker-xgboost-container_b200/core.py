@@ -537,6 +537,51 @@ def _check_unapplied(k, v):
     return v
 
 
+class _DeviceGradient:
+    """A CUDA array viewed as (rows, outputs): its __cuda_array_interface__ with the shape and strides of that view."""
+
+    def __init__(self, obj, iface, shape, strides):
+        self._obj = obj                      # keeps the memory alive
+        self.shape = tuple(shape)
+        self.__cuda_array_interface__ = dict(iface, shape=self.shape, strides=tuple(strides))
+
+
+def _gradient_array(a, n, what):
+    """grad or hess as a (n, K) numpy float32 / float64 array, or a (n, K) view of a CUDA array (read in place)."""
+    if hasattr(a, "__cuda_array_interface__"):
+        iface = dict(a.__cuda_array_interface__)
+        if "stream" not in iface and type(a).__module__.startswith("torch"):
+            # torch exports interface v2 without a stream: its producer is the tensor's current stream (0 is the legacy
+            # default stream, 1 in the v3 convention)
+            import torch
+            iface["stream"] = torch.cuda.current_stream(a.device).cuda_stream or 1
+        shape = tuple(int(d) for d in iface["shape"])
+        if iface["typestr"] not in ("<f4", "<f8"):
+            raise ValueError("%s: CUDA arrays must be float32 or float64, got typestr %s" % (what, iface["typestr"]))
+        isz = int(iface["typestr"][2:])
+        strides = iface.get("strides")
+        if strides is None:                  # C-contiguous
+            strides = (isz,) if len(shape) == 1 else (shape[1] * isz, isz)
+        if len(shape) == 1:
+            if n == 0 or shape[0] % n:
+                raise ValueError("%s has %d elements, which is not a multiple of the %d rows" % (what, shape[0], n))
+            K = shape[0] // n
+            shape, strides = (n, K), (K * strides[0], strides[0])
+        elif len(shape) != 2:
+            raise ValueError("%s must be 1- or 2-dimensional, got shape %s" % (what, shape))
+        return _DeviceGradient(a, iface, shape, strides)
+    a = np.asarray(a)
+    if a.dtype not in (np.float32, np.float64):
+        a = a.astype(np.float32)
+    if a.ndim == 1:
+        if (n == 0 and a.size) or (n and a.size % n):
+            raise ValueError("%s has %d elements, which is not a multiple of the %d rows" % (what, a.size, n))
+        a = a.reshape(n, -1) if n else a.reshape(0, 1)
+    elif a.ndim != 2:
+        raise ValueError("%s must be 1- or 2-dimensional, got shape %s" % (what, a.shape))
+    return np.ascontiguousarray(a)
+
+
 class Booster:
     """A gradient-boosted tree model trained / evaluated by the CUDA engine."""
 
@@ -734,12 +779,26 @@ class Booster:
         if not isinstance(dtrain, DMatrix):
             raise TypeError("invalid training matrix: %s" % type(dtrain).__name__)
         self._assign_dmatrix_features(dtrain)
-        if fobj is not None:
-            raise XGBoostError("custom objectives are not supported on the CUDA hist path")
-        get_backend().booster_update(self.handle, int(iteration), dtrain.handle)
+        if fobj is None:
+            get_backend().booster_update(self.handle, int(iteration), dtrain.handle)
+            return
+        # the margins of the training matrix's prediction cache, shaped as predict(output_margin=True) shapes them: no pass
+        # over the ensemble per round
+        margin = get_backend().booster_training_margin(self.handle, dtrain.handle)
+        grad, hess = fobj(margin[:, 0] if margin.shape[1] == 1 else margin, dtrain)
+        self.boost(dtrain, iteration, grad, hess)
 
-    def boost(self, dtrain, iteration=0, grad=None, hess=None):
-        raise XGBoostError("custom objectives (Booster.boost) are not supported on the CUDA hist path")
+    def boost(self, dtrain, iteration, grad, hess):
+        """One boosting round on the given gradients and hessians: numpy arrays, or CUDA arrays (`__cuda_array_interface__`:
+        torch tensors, cupy arrays) read in place, float32 or float64, of shape (rows, outputs) or (rows * outputs,) row-major."""
+        if not isinstance(dtrain, DMatrix):
+            raise TypeError("invalid training matrix: %s" % type(dtrain).__name__)
+        n = dtrain.num_row()
+        grad, hess = _gradient_array(grad, n, "grad"), _gradient_array(hess, n, "hess")
+        if grad.shape != hess.shape:
+            raise ValueError("grad / hess shape mismatch: %s / %s" % (grad.shape, hess.shape))
+        self._assign_dmatrix_features(dtrain)
+        get_backend().booster_boost(self.handle, dtrain.handle, int(iteration), grad, hess)
 
     def eval_set(self, evals, iteration=0, feval=None, output_margin=True):
         for d, name in evals:

@@ -820,6 +820,9 @@ static float objective_aux(const TrainParam& p) {
 void Booster::estimate_base_score(DMatrix* dtrain) {
   if (base_score_set_ || base_score_estimated_ || !trees_.empty()) { base_score_estimated_ = true; return; }
   base_score_estimated_ = true;
+  // a cache filled before the estimate (a custom round's margin, a failed custom round) starts over from the new base margin;
+  // the model has no trees, so this costs one fill
+  for (auto& kv : caches_) kv.second.trees_applied = -1;
   if (param_.objective == kSoftprob || param_.objective == kSoftmax) { base_score_ = 0.5f; return; }
   // 3.0.x fits the intercept for the RegLossObj family only; the log-link objectives and binary:hinge keep the 0.5 default
   // [UPSTREAM-RECALL: src/objective/init_estimation.cc; later releases changed the GLM objectives]
@@ -1149,23 +1152,33 @@ void Booster::check_label_ranges(const DMatrix* dtrain) {
 void Booster::update_one_iter(int iter, DMatrix* dtrain) {
   configure();
   (void)iter;
-  cudaStream_t s = engine_stream();
   if (param_.objective == kAft) check_aft_bounds(dtrain); else { check_targets(dtrain, true); check_labels(dtrain); }
   B200_CHECK(param_.objective != kCox || !Comm::get().distributed(), "survival:cox is not supported with more than one GPU (world_size > 1): its risk sets span the rows of every rank");
+  train_round(dtrain, nullptr);
+}
+
+// One round of the configured objective (custom == nullptr) or of the caller's gradients: they differ only in where
+// launch_objective takes the pairs from.  A custom round reads no labels and estimates no base score.
+void Booster::train_round(DMatrix* dtrain, const CustomGradArgs* custom) {
+  cudaStream_t s = engine_stream();
   if (num_feature_ == 0) num_feature_ = dtrain->F;
   B200_CHECK(num_feature_ == dtrain->F, "Check failed: learner_model_param_.num_feature == p_fmat->Info().num_col_ (" + std::to_string(num_feature_) +
              " vs. " + std::to_string(dtrain->F) + ") : Number of columns does not match number of features in booster.");
   B200_CHECK(dtrain->n > 0 || Comm::get().distributed(), "Empty dataset at worker: 0");
-  if (objective_is_rank(param_.objective)) rank_groups(dtrain, objective_name_.c_str());
-  else check_row_weights(dtrain);
+  if (!custom) {
+    if (objective_is_rank(param_.objective)) rank_groups(dtrain, objective_name_.c_str());
+    else check_row_weights(dtrain);
+  }
   if (update_mode_) { dtrain->require_raw("process_type=update"); refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
   if (dart_.on) dtrain->require_raw("booster=dart");
   check_train_width(dtrain);
   dtrain->ensure_binned(param_.max_bin);
   const int K = param_.num_outputs();
   TreeBuilder& b = builder_for(dtrain);
-  check_label_ranges(dtrain);
-  estimate_base_score(dtrain);
+  if (!custom) { check_label_ranges(dtrain); estimate_base_score(dtrain); }
+  // the caller's arrays are read by launch_objective in this round only
+  struct CustomScope { const CustomGradArgs*& p; ~CustomScope() { p = nullptr; } } scope{custom_};
+  custom_ = custom;
   PredCache& cache = cache_for(dtrain);
   bring_cache_up_to_date(dtrain, cache);
 
@@ -1208,6 +1221,10 @@ void Booster::update_one_iter(int iter, DMatrix* dtrain) {
     CUDA_OK(cudaMemsetAsync(target_absmax_.p, 0, 2 * sizeof(unsigned) * K, s));
     launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, target_absmax_.p, param_.subsample, dense_g, resid, true);
   } else launch_objective(dtrain, grad_margin, round, b.gpair.p, b.gp_stride, b.gs.absmax, param_.subsample, dense_g, resid);
+  // a custom round keeps base_score if given, else 0.5, once its gradients passed the check in launch_objective: a failed
+  // round leaves a later round of the configured objective free to estimate it [UPSTREAM-RECALL: BoostOneIter does not call
+  // InitBaseScore]
+  if (custom) base_score_estimated_ = true;
   // weighted adaptive objectives under gradient-based sampling: the refresh weighs its rows by their instance weight (h is w / p)
   if (gbs && resid && !dtrain->weights.empty()) weight_grid(dtrain->d_weights.p, dtrain->n, b.global_n, &b.adapt, s);
   if (per_target_grid) Comm::get().allreduce_max_u32(target_absmax_.p, 2 * (size_t)K, s);
@@ -1265,6 +1282,11 @@ void Booster::launch_objective(DMatrix* dm, const float* margin, int round, floa
                                bool dense_g, float* resid, bool per_target_absmax) {
   cudaStream_t s = engine_stream();
   const int64_t row_offset = (int64_t)Comm::get().rank() << 40;
+  if (custom_) {                             // the caller's gradients (custom_grad.cu): no labels, no residuals, never dense g
+    B200_CHECK(!dense_g && !resid, "custom gradients are (g,h) pairs of a non-adaptive objective");
+    launch_custom_gradient_checked(round, gpair, gp_stride, absmax, subsample, per_target_absmax);
+    return;
+  }
   if (param_.num_target > 1) {               // multi-target: one pair per label element (multi_target.cu)
     B200_CHECK(!dense_g, "multi-target gradients are (g,h) pairs");
     MultiGradArgs ma{}; ma.margin = margin; ma.label = dm->d_labels.p; ma.weight = dm->weights.empty() ? nullptr : dm->d_weights.p;
@@ -1385,7 +1407,7 @@ TreeBuilder& Booster::builder_for(DMatrix* dm) {
 // (launch_objective) and the tree reads them so (root_mode != 0); this one predicate decides both.  B200XGB_NO_CONSTH turns it off.
 bool Booster::constant_hessian(const DMatrix& dm) const {
   static const bool no_consth = getenv("B200XGB_NO_CONSTH") != nullptr;
-  return !no_consth && (param_.objective == kSquaredError || param_.objective == kAbsoluteError || param_.objective == kQuantileError) &&
+  return !no_consth && !custom_ && (param_.objective == kSquaredError || param_.objective == kAbsoluteError || param_.objective == kQuantileError) &&
          param_.num_outputs() == 1 && dm.weights.empty() &&
          param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
 }
@@ -1581,8 +1603,124 @@ void Booster::debug_refresh_sums(std::vector<long long>* out) {
   Comm::get().sync_stream(s);
 }
 
-void Booster::boost_one_iter(DMatrix*, const float*, const float*, size_t) {
-  throw Error("custom objective (BoostOneIter) is not implemented on the CUDA hist path");
+// ---------------------------------------------------------------------------------------------
+// custom objectives (upstream LearnerImpl::BoostOneIter; DESIGN.md "Custom objectives")
+// ---------------------------------------------------------------------------------------------
+static std::string shape_str(int64_t n, int64_t m) { return "(" + std::to_string(n) + ", " + std::to_string(m) + ")"; }
+
+// whether in's elements are device memory (checked to be on the engine's device); anything else is read as host memory
+static bool custom_on_device(const GradInput& in, const char* what) {
+  if (in.n == 0 || in.m == 0) return false;
+  cudaPointerAttributes attr{};
+  const bool device = cudaPointerGetAttributes(&attr, in.ptr) == cudaSuccess && (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+  (void)cudaGetLastError();                  // an unregistered host pointer may leave an error behind on older drivers
+  if (device) {
+    int dev = 0; CUDA_OK(cudaGetDevice(&dev));
+    B200_CHECK(attr.device == dev, std::string("custom objective: ") + what + " is on CUDA device " + std::to_string(attr.device) + " but the booster trains on device " +
+               std::to_string(dev));
+  }
+  return device;
+}
+
+// the bytes a host array's elements span, wherever the strides point: [lo, hi) from its pointer
+static void host_extent(const GradInput& in, int64_t* lo, int64_t* hi) {
+  const int64_t isz = in.f64 ? 8 : 4;
+  *lo = std::min<int64_t>(0, (in.n - 1) * in.s0) + std::min<int64_t>(0, (in.m - 1) * in.s1);
+  *hi = std::max<int64_t>(0, (in.n - 1) * in.s0) + std::max<int64_t>(0, (in.m - 1) * in.s1) + isz;
+}
+static size_t host_span(const GradInput& in) {
+  int64_t lo, hi; host_extent(in, &lo, &hi);
+  return (size_t)((hi - lo + 255) & ~(int64_t)255);
+}
+
+// in's elements as the kernel reads them.  Device memory is read in place once the engine stream is ordered after the
+// producer: an event on the given stream, or with no stream named at all a device synchronise.  Host memory is copied to
+// the staging buffer at staging_offset bytes, which boost_one_iter has sized for the host arrays only.
+GradArray Booster::custom_array(const GradInput& in, bool device, size_t staging_offset) {
+  const int64_t isz = in.f64 ? 8 : 4;
+  GradArray a{}; a.s0 = in.s0 / isz; a.s1 = in.s1 / isz; a.f64 = in.f64 ? 1 : 0; a.data = in.ptr;
+  if (in.n == 0 || in.m == 0) return a;
+  cudaStream_t s = engine_stream();
+  if (device) {
+    if (in.stream == GradInput::kNoStream) CUDA_OK(cudaDeviceSynchronize());
+    else if (in.stream != 0) {
+      const cudaStream_t ps = in.stream == 1 ? cudaStreamLegacy : in.stream == 2 ? cudaStreamPerThread : reinterpret_cast<cudaStream_t>(in.stream);
+      cudaEvent_t ev; CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      const cudaError_t e1 = cudaEventRecord(ev, ps), e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(s, ev, 0) : e1;
+      cudaEventDestroy(ev);
+      CUDA_OK(e2);
+    }
+    return a;
+  }
+  int64_t lo, hi; host_extent(in, &lo, &hi);
+  unsigned char* dst = custom_staging_.p + staging_offset;
+  CUDA_OK(cudaMemcpyAsync(dst, static_cast<const unsigned char*>(in.ptr) + lo, (size_t)(hi - lo), cudaMemcpyHostToDevice, s));
+  a.data = dst - lo;
+  return a;
+}
+
+void Booster::boost_one_iter(DMatrix* dtrain, const GradInput& grad, const GradInput& hess) {
+  configure();
+  B200_CHECK(!dart_.on, "custom objective: booster=dart is not supported with custom gradients (its drop set is drawn inside the round)");
+  B200_CHECK(!objective_is_adaptive(param_.objective), "custom objective: objective=" + objective_name_ + " is not supported with custom gradients "
+             "(its leaf refresh reads the residuals of its own loss); configure another objective, e.g. reg:squarederror");
+  B200_CHECK(!update_mode_, "custom objective: process_type=update is not supported with custom gradients");
+  check_targets(dtrain, true);                   // a multi-target label sets the model's outputs on its first round
+  const int K = param_.num_outputs();
+  const int64_t n = dtrain->n;
+  for (const GradInput* in : {&grad, &hess}) {
+    const char* what = in == &grad ? "grad" : "hess";
+    const int64_t isz = in->f64 ? 8 : 4;
+    B200_CHECK(in->s0 % isz == 0 && in->s1 % isz == 0, std::string("custom objective: the strides of ") + what + " are not multiples of its element size");
+    if (in->n == n && (in->m == K || n == 0)) continue;
+    std::string msg = std::string("custom objective: ") + what + " has shape " + shape_str(in->n, in->m) + " but the model trains " + shape_str(n, K) +
+                      " outputs on this matrix (rows, outputs)";
+    if (in->n == n && K == 1 && in->m > 1)
+      msg += "; num_class is ignored unless objective is multi:softprob or multi:softmax: set objective=multi:softprob and num_class=" + std::to_string(in->m) +
+             " to train " + std::to_string(in->m) + " outputs";
+    throw Error(msg);
+  }
+  const bool dev_g = custom_on_device(grad, "grad"), dev_h = custom_on_device(hess, "hess");
+  const size_t span_g = dev_g || grad.n == 0 || grad.m == 0 ? 0 : host_span(grad);
+  const size_t span_h = dev_h || hess.n == 0 || hess.m == 0 ? 0 : host_span(hess);
+  if (span_g + span_h) custom_staging_.ensure(span_g + span_h);
+  custom_bad_.ensure(1); custom_bad_flag_.ensure(1);
+  CustomGradArgs a{};
+  a.g = custom_array(grad, dev_g, 0); a.h = custom_array(hess, dev_h, span_g);
+  a.bad = custom_bad_.p; a.bad_flag = custom_bad_flag_.p; a.n = n; a.K = K;
+  train_round(dtrain, &a);
+}
+
+// launch_objective for a custom round: the caller's arrays into the round's pairs, then a host check of the invalid-element
+// report, every rank's taken together, before anything reads the pairs
+void Booster::launch_custom_gradient_checked(int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool per_target_absmax) {
+  cudaStream_t s = engine_stream();
+  CustomGradArgs a = *custom_;
+  a.gpair = gpair; a.gp_stride = gp_stride; a.absmax = absmax; a.per_target = per_target_absmax ? 1 : 0;
+  a.row_offset = (int64_t)Comm::get().rank() << 40; a.subsample = subsample; a.seed = param_.seed; a.iter = (unsigned long long)round;
+  CUDA_OK(cudaMemsetAsync(a.bad, 0xff, sizeof(unsigned long long), s));
+  CUDA_OK(cudaMemsetAsync(a.bad_flag, 0, sizeof(unsigned), s));
+  launch_custom_gradient(a, s);
+  Comm::get().allreduce_max_u32(a.bad_flag, 1, s);
+  unsigned long long bad = 0; unsigned flag = 0;
+  CUDA_OK(cudaMemcpyAsync(&bad, a.bad, sizeof bad, cudaMemcpyDeviceToHost, s));
+  CUDA_OK(cudaMemcpyAsync(&flag, a.bad_flag, sizeof flag, cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
+  if (!flag) return;
+  B200_CHECK(bad != ~0ull, "custom objective: the gradients of another rank are not finite or have a negative hessian");
+  const int64_t r = (int64_t)(bad / (unsigned long long)a.K); const int k = (int)(bad % (unsigned long long)a.K);
+  double v[2];
+  for (int i = 0; i < 2; ++i) {                   // the offending values as the caller gave them
+    const GradArray& ga = i == 0 ? a.g : a.h;
+    const int64_t off = r * ga.s0 + (int64_t)k * ga.s1;
+    if (ga.f64) CUDA_OK(cudaMemcpyAsync(&v[i], static_cast<const double*>(ga.data) + off, 8, cudaMemcpyDeviceToHost, s));
+    else { float f; CUDA_OK(cudaMemcpyAsync(&f, static_cast<const float*>(ga.data) + off, 4, cudaMemcpyDeviceToHost, s)); Comm::get().sync_stream(s); v[i] = f; }
+  }
+  Comm::get().sync_stream(s);
+  char buf[96]; snprintf(buf, sizeof buf, "grad = %.9g, hess = %.9g", v[0], v[1]);
+  throw Error("custom objective: the gradient pair at row " + std::to_string(r) + ", output column " + std::to_string(k) + " is " +
+              (std::isfinite((float)v[0]) && std::isfinite((float)v[1]) ? "invalid (the hessian is negative)" : "not finite") + ": " + buf +
+              "; the CUDA hist path needs finite gradients and hessians >= 0");
 }
 
 int Booster::boosted_rounds() { configure(); return layers(); }
@@ -2014,6 +2152,13 @@ float Booster::debug_predict_kernel_ms(DMatrix* dm, int repeats) {
   }
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   return total / std::max(1, repeats);
+}
+
+int Booster::training_margin(DMatrix* dtrain, std::vector<float>* out) {
+  configure();
+  if (layers() == 0 && !update_mode_) check_targets(dtrain, true);
+  cached_margin(dtrain, out);
+  return param_.num_outputs();
 }
 
 void Booster::cached_margin(DMatrix* dm, std::vector<float>* out) {

@@ -7,6 +7,7 @@
 #include <vector>
 #include "container_metrics.h"
 #include "curve.h"
+#include "custom_grad.h"
 #include "engine.h"
 #include "grow.h"
 #include "json.h"
@@ -149,6 +150,15 @@ bool looks_like_legacy_binary(const char* buf, size_t len);
 JPtr legacy_binary_to_doc(const char* buf, size_t len);
 std::pair<const char*, size_t> legacy_serialized_model_section(const char* buf, size_t len);
 
+// One of the caller's gradient arrays for Booster::boost_one_iter (upstream's array interface): n rows, m columns, element
+// (r, k) at ptr + r * s0 + k * s1 bytes, float32 or float64 (f64), in host or device memory.  stream: the producer's CUDA stream
+// as __cuda_array_interface__ v3 gives it (1 = legacy default, 2 = per-thread default, else a cudaStream_t), 0 = null (no
+// ordering needed), kNoStream = not given (device memory is then read after a device synchronise).
+struct GradInput {
+  static constexpr uint64_t kNoStream = ~0ull;
+  const void* ptr = nullptr; int64_t n = 0, m = 1, s0 = 0, s1 = 0; bool f64 = false; uint64_t stream = kNoStream;
+};
+
 class Booster {
  public:
   Booster();
@@ -159,7 +169,8 @@ class Booster {
   void load_config(const std::string& json);
   // training
   void update_one_iter(int iter, DMatrix* dtrain);
-  void boost_one_iter(DMatrix* dtrain, const float* grad, const float* hess, size_t len);
+  // one boosting round on the caller's gradients (DESIGN.md "Custom objectives"), (dtrain rows, num_outputs) each
+  void boost_one_iter(DMatrix* dtrain, const GradInput& grad, const GradInput& hess);
   std::string eval_one_iter(int iter, const std::vector<DMatrix*>& dms, const std::vector<std::string>& names);
   // the raw results of the container's own metrics `names` on dm from the prediction cache (container_metrics.h layout, out
   // holds kContainerOutLen entries); output_margin: the metric reads margins (feval=) instead of predict()'s values
@@ -182,6 +193,9 @@ class Booster {
   // introspection used by tests/bench (build-specific C-ABI entry points)
   void sync_model();                              // materialise pending trees on the host
   void cached_margin(DMatrix* dm, std::vector<float>* out);   // the trainer's prediction cache for dm
+  // the margin the next round's objective reads on dtrain ([n][K] into out, K returned): the prediction cache, with the output
+  // count a first round on dtrain takes (its label columns)
+  int training_margin(DMatrix* dtrain, std::vector<float>* out);
   float debug_predict_kernel_ms(DMatrix* dm, int repeats);
   std::string debug_predict_plan(DMatrix* dm, int iter_begin, int iter_end);   // JSON of the plan predict() would run
   const std::vector<HostTree>& trees() { sync_model(); return trees_; }
@@ -257,6 +271,13 @@ class Booster {
   std::unique_ptr<UpdateState> update_ = std::make_unique<UpdateState>();
   DevBuf<float> quantile_alpha_dev_; std::vector<float> quantile_alpha_host_;   // reg:quantileerror / the quantile metric: alpha on the device
   DevBuf<unsigned> target_absmax_;              // reg:quantileerror: each target's max|g| and max h ([2 Q]), for a grid per target
+  // custom objectives: the round's caller arrays on the device (nullptr in a round of the configured objective), the staging
+  // buffer of host arrays (grown, reused across rounds) and the kernel's invalid-element report
+  const CustomGradArgs* custom_ = nullptr;
+  DevBuf<unsigned char> custom_staging_; DevBuf<unsigned long long> custom_bad_; DevBuf<unsigned> custom_bad_flag_;
+  void train_round(DMatrix* dtrain, const CustomGradArgs* custom);   // update_one_iter / boost_one_iter
+  GradArray custom_array(const GradInput& in, bool device, size_t staging_offset);
+  void launch_custom_gradient_checked(int round, float2* gpair, int64_t gp_stride, unsigned* absmax, float subsample, bool per_target_absmax);
 
   void configure();
   void check_label_ranges(const DMatrix* dtrain);

@@ -90,15 +90,27 @@ int XGDMatrixCreateFromCudaArrayInterface(const char* data, const char* config, 
 }
 // ---- host array interface (numpy `__array_interface__` as JSON): what upstream's Python package passes for ndarray inputs
 namespace {
-struct HostArray { const void* ptr; int64_t n, m; std::string typestr; };
-HostArray parse_array_interface(const char* json) {
+// s0 / s1: the byte strides of rows and columns; stream: __cuda_array_interface__ v3's "stream", 0 when null and
+// GradInput::kNoStream when the document names none.
+// Strides other than C-contiguous are accepted only where the caller reads them (allow_strides).
+struct HostArray { const void* ptr; int64_t n, m; std::string typestr; int64_t s0, s1; uint64_t stream; };
+HostArray parse_array_interface(const char* json, bool allow_strides = false) {
   JPtr a = parse_json(json);
   HostArray h{};
   const JValue& shape = a->at("shape");
   if (shape.length() < 1 || shape.length() > 2) throw Error("array interface: expecting a 1- or 2-dimensional array");
   h.n = (int64_t)shape.num_at(0); h.m = shape.length() == 2 ? (int64_t)shape.num_at(1) : 1;
-  if (a->has("strides") && a->at("strides").type != JValue::kNull) throw Error("array interface: only C-contiguous arrays are supported");
   h.typestr = a->at("typestr").s;
+  const int64_t isz = h.typestr.size() >= 3 ? std::atoi(h.typestr.c_str() + 2) : 0;
+  h.s1 = isz; h.s0 = isz * h.m;
+  if (a->has("strides") && a->at("strides").type != JValue::kNull) {
+    if (!allow_strides) throw Error("array interface: only C-contiguous arrays are supported");
+    const JValue& st = a->at("strides");
+    if (st.length() != shape.length()) throw Error("array interface: strides and shape differ in length");
+    h.s0 = (int64_t)st.num_at(0); if (shape.length() == 2) h.s1 = (int64_t)st.num_at(1);
+    if (shape.length() == 1) { h.s1 = h.s0; h.s0 = h.s1 * h.m; }
+  }
+  h.stream = !a->has("stream") ? GradInput::kNoStream : a->at("stream").type == JValue::kNull ? 0 : (uint64_t)a->at("stream").as_int();
   h.ptr = reinterpret_cast<const void*>((uintptr_t)a->at("data").arr[0]->as_int());
   return h;
 }
@@ -411,8 +423,30 @@ int XGBoosterCreate(const DMatrixHandle dmats[], bst_ulong len, BoosterHandle* o
 int XGBoosterFree(BoosterHandle handle) { API_BEGIN(); delete static_cast<BoosterBox*>(handle); API_END(); }
 int XGBoosterSetParam(BoosterHandle handle, const char* name, const char* value) { API_BEGIN(); BST(handle)->set_param(name, value ? value : ""); API_END(); }
 int XGBoosterUpdateOneIter(BoosterHandle handle, int iter, DMatrixHandle dtrain) { API_BEGIN(); BST(handle)->update_one_iter(iter, DM(dtrain)); API_END(); }
+namespace {
+GradInput grad_input(const char* json, const char* what) {
+  const HostArray h = parse_array_interface(json, true);
+  B200_CHECK(h.typestr == "<f4" || h.typestr == "<f8", std::string("custom objective: ") + what + " must be float32 or float64 (typestr <f4 or <f8), got " + h.typestr);
+  GradInput g; g.ptr = h.ptr; g.n = h.n; g.m = h.m; g.s0 = h.s0; g.s1 = h.s1; g.f64 = h.typestr == "<f8"; g.stream = h.stream;
+  return g;
+}
+}  // namespace
+int XGBoosterTrainOneIter(BoosterHandle handle, DMatrixHandle dtrain, int iter, const char* grad, const char* hess) {
+  API_BEGIN();
+  (void)iter;
+  BST(handle)->boost_one_iter(DM(dtrain), grad_input(grad, "grad"), grad_input(hess, "hess"));
+  API_END();
+}
 int XGBoosterBoostOneIter(BoosterHandle handle, DMatrixHandle dtrain, float* grad, float* hess, bst_ulong len) {
-  API_BEGIN(); BST(handle)->boost_one_iter(DM(dtrain), grad, hess, (size_t)len); API_END();
+  API_BEGIN();
+  DMatrix* dm = DM(dtrain);
+  const int64_t n = dm->n;
+  B200_CHECK(n > 0 ? len % (bst_ulong)n == 0 : len == 0, "custom objective: " + std::to_string(len) + " gradients are not a multiple of the " +
+             std::to_string(n) + " rows");
+  GradInput g; g.n = n; g.m = n > 0 ? (int64_t)(len / (bst_ulong)n) : 1; g.s1 = 4; g.s0 = 4 * g.m;
+  GradInput h = g; g.ptr = grad; h.ptr = hess;
+  BST(handle)->boost_one_iter(dm, g, h);
+  API_END();
 }
 int XGBoosterEvalOneIter(BoosterHandle handle, int iter, DMatrixHandle dmats[], const char* evnames[], bst_ulong len, const char** out_result) {
   API_BEGIN();
@@ -779,6 +813,13 @@ int XGB200BoosterEvalContainerMetrics(BoosterHandle handle, DMatrixHandle dmat, 
   std::vector<std::string> v;
   for (bst_ulong i = 0; i < len; ++i) v.emplace_back(names[i]);
   BST(handle)->eval_container_metrics(DM(dmat), v, output_margin != 0, out);
+  API_END();
+}
+int XGB200BoosterGetTrainingMargin(BoosterHandle handle, DMatrixHandle dtrain, bst_ulong* out_rows, bst_ulong* out_cols, const float** out) {
+  API_BEGIN();
+  BoosterBox* box = static_cast<BoosterBox*>(handle);
+  const int K = BST(handle)->training_margin(DM(dtrain), &box->ret_vec);
+  *out_rows = (bst_ulong)DM(dtrain)->n; *out_cols = (bst_ulong)K; *out = box->ret_vec.data();
   API_END();
 }
 int XGB200BoosterGetCachedMargin(BoosterHandle handle, DMatrixHandle dmat, float* out) {

@@ -25,8 +25,7 @@ __global__ void __launch_bounds__(256) gradient_kernel(GradArgs a) {
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < a.n; r += (int64_t)gridDim.x * blockDim.x) {
     const float y = a.label[r];
     float w = a.weight ? a.weight[r] : 1.0f;
-    bool dropped = false;
-    if (a.subsample < 1.0f) dropped = !(rng_uniform(a.seed, 0x2000ull + a.iter, (unsigned long long)(r + a.row_offset)) < a.subsample);
+    const bool dropped = !row_sampled(a.seed, a.iter, (unsigned long long)(r + a.row_offset), a.subsample);
     if (a.objective == kSoftprob || a.objective == kSoftmax) {
       const int K = a.K;
       const float* m = a.margin ? a.margin + r * K : nullptr;

@@ -13,5 +13,9 @@ __host__ __device__ __forceinline__ float rng_uniform(unsigned seed, unsigned lo
   const unsigned long long h = splitmix64(splitmix64(((unsigned long long)seed << 32) ^ stream) ^ idx);
   return (float)(h >> 40) * (1.0f / 16777216.0f);
 }
+// subsample's row draw of boosting round `iter`: row `row` (the rank's row offset added) is in the round's sample
+__host__ __device__ __forceinline__ bool row_sampled(unsigned seed, unsigned long long iter, unsigned long long row, float subsample) {
+  return !(subsample < 1.0f) || rng_uniform(seed, 0x2000ull + iter, row) < subsample;
+}
 
 }  // namespace b200

@@ -12,6 +12,18 @@ _FIT_ONLY = {"n_estimators", "early_stopping_rounds", "eval_metric", "callbacks"
              "feature_types", "n_jobs", "random_state", "verbosity", "objective", "kwargs"}
 
 
+def _objective_decorator(func):
+    """A scikit-learn style objective `func(y_true, y_pred) -> (grad, hess)` as train()'s `obj(margin, dtrain)`: y_true is the
+    label, shaped as the margin for a multi-target label.  [UPSTREAM-RECALL: xgboost.sklearn._objective_decorator; whether 3.0
+    also passes sample_weight is not verified]"""
+    def inner(preds, dmatrix):
+        labels = dmatrix.get_label()
+        if preds.ndim == 2 and labels.size == preds.size:
+            labels = labels.reshape(preds.shape)
+        return func(labels, preds)
+    return inner
+
+
 class XGBModel:
     _default_objective = "reg:squarederror"
 
@@ -44,7 +56,8 @@ class XGBModel:
 
     def get_xgb_params(self):
         p = {k: v for k, v in self.get_params().items() if v is not None and k not in _FIT_ONLY}
-        p["objective"] = self.objective or self._default_objective
+        # a callable objective trains through train(obj=) on the default objective's transform (upstream's _objective_decorator)
+        p["objective"] = self._default_objective if self.objective is None or callable(self.objective) else self.objective
         if self.random_state is not None:
             p["seed"] = int(self.random_state)
         if self.eval_metric is not None and not callable(self.eval_metric):
@@ -71,7 +84,8 @@ class XGBModel:
             evals.append((dtrain if (Xe is X and ye is y) else self._dmatrix(Xe, ye, we), "validation_%d" % i))
         self.evals_result_ = {}
         model = xgb_model.get_booster() if isinstance(xgb_model, XGBModel) else xgb_model
-        self._Booster = train(params, dtrain, self.get_num_boosting_rounds(), evals=evals, early_stopping_rounds=self.early_stopping_rounds,
+        obj = _objective_decorator(self.objective) if callable(self.objective) else None
+        self._Booster = train(params, dtrain, self.get_num_boosting_rounds(), evals=evals, obj=obj, early_stopping_rounds=self.early_stopping_rounds,
                               evals_result=self.evals_result_, custom_metric=self.eval_metric if callable(self.eval_metric) else None,
                               verbose_eval=verbose, xgb_model=model, callbacks=self.callbacks)
         self.n_features_in_ = dtrain.num_col()
@@ -175,6 +189,8 @@ class XGBRanker(XGBModel):
 
     def fit(self, X, y, *, group=None, qid=None, sample_weight=None, base_margin=None, eval_set=None, eval_group=None, eval_qid=None,
             verbose=False, xgb_model=None, sample_weight_eval_set=None):
+        if callable(self.objective):
+            raise ValueError("custom objective function not supported by XGBRanker")
         params = self.get_xgb_params()
         if not str(params["objective"]).startswith("rank:"):
             raise ValueError("XGBRanker takes a rank:* objective (got %s)" % params["objective"])
