@@ -126,6 +126,25 @@ XGB_DLL int XGBoosterEvalOneIter(BoosterHandle handle, int iter, DMatrixHandle d
  * serve_utils.py:244-250, serving.py:98, handler_service.py:73, train.py:445 */
 XGB_DLL int XGBoosterPredictFromDMatrix(BoosterHandle handle, DMatrixHandle dmat, const char* config,
                                 bst_ulong const** out_shape, bst_ulong* out_dim, float const** out_result);
+/* In-place prediction (upstream's Booster.inplace_predict): predict from an array without building a DMatrix.  `values` is an
+ * array-interface JSON of a 2-D array (numpy __array_interface__ / __cuda_array_interface__: "data", "shape", "typestr" in
+ * <f4 <f8 <f2 |i1 <i2 <i4 <i8 |u1 <u2 <u4 <u8 |b1, optional byte "strides", negative allowed), read at its own dtype and
+ * strides.  config JSON: {"type": 0 value | 1 margin, "iteration_begin": int, "iteration_end": int, "strict_shape": bool,
+ * "missing": float (default NaN)}.  m / proxy: NULL, or a proxy DMatrix (XGProxyDMatrixCreate) whose "base_margin"
+ * (XGDMatrixSetInfoFromInterface) holds rows x outputs base margins.  The result equals XGBoosterPredictFromDMatrix on a DMatrix
+ * of the same values converted to float32 (round to nearest even), bit for bit.  [UPSTREAM-RECALL: 2.x/3.0 c_api.h signatures]
+ * FromDense: host memory, copied to the device in row chunks at its own dtype; out_result is host memory owned by the booster. */
+XGB_DLL int XGBoosterPredictFromDense(BoosterHandle handle, const char* values, const char* config, DMatrixHandle m,
+                                      bst_ulong const** out_shape, bst_ulong* out_dim, const float** out_result);
+/* host CSR as three array interfaces: indptr (<i8 / <u8), indices (<i4 / <u4, each < ncol), data (<f4).  Absent entries are
+ * missing; `missing` does not apply to stored values; a column repeated in a row keeps its last value */
+XGB_DLL int XGBoosterPredictFromCSR(BoosterHandle handle, const char* indptr, const char* indices, const char* values, bst_ulong ncol,
+                                    const char* config, DMatrixHandle m, bst_ulong const** out_shape, bst_ulong* out_dim,
+                                    const float** out_result);
+/* CUDA memory on the booster's device, read in place; "stream" as in XGBoosterTrainOneIter (the v3 stream is waited on, null:
+ * no wait, no key: a device synchronise).  out_result is DEVICE memory owned by the booster, valid until its next call. */
+XGB_DLL int XGBoosterPredictFromCudaArray(BoosterHandle handle, const char* values, const char* config, DMatrixHandle proxy,
+                                          bst_ulong const** out_shape, bst_ulong* out_dim, const float** out_result);
 /* file name extension picks the format: .json -> JSON text, anything else (incl. none) -> UBJSON  (train.py:480) */
 XGB_DLL int XGBoosterSaveModel(BoosterHandle handle, const char* fname);
 XGB_DLL int XGBoosterLoadModel(BoosterHandle handle, const char* fname);                              /* serve_utils.py:184-185 */
@@ -259,6 +278,10 @@ XGB_DLL int XGB200BuildHistogramEx(BoosterHandle handle, DMatrixHandle dmat, con
  * "lower", "upper"}]}; a candidate is {"loss_chg", "feature", "bin", "dleft", "ord", "GL", "HL"}; every float is its uint32 bits. */
 XGB_DLL int XGB200BoosterEvalRootSplit(BoosterHandle handle, DMatrixHandle dmat, const int64_t* hist, int64_t G, int64_t H, float max_g,
                                float max_h, float lower, float upper, const uint8_t* feat_mask, const char** out_json);
+/* in-place prediction's staging: chunk_rows >= 0 sets the rows per staged chunk (0 = as many as a staging buffer holds; -1 keeps the
+ * setting); *staged_bytes = the most device bytes one chunk of the last in-place call staged or converted (0 when the input was read
+ * where it lies), *staging_capacity = the staging and scratch bytes the booster holds.  Either pointer may be NULL. */
+XGB_DLL int XGB200BoosterInplaceDebug(BoosterHandle handle, int64_t chunk_rows, bst_ulong* staged_bytes, bst_ulong* staging_capacity);
 /* mean device time (CUDA events) of the predictor kernel alone over `repeats` launches on `dmat` */
 XGB_DLL int XGB200BoosterPredictKernelMs(BoosterHandle handle, DMatrixHandle dmat, int repeats, float* out_ms);
 /* the predictor's plan for `dmat` and the rounds [iter_begin, iter_end) (iter_end == 0: all), without running it: JSON

@@ -323,6 +323,67 @@ class CudaBackend:
             return np.zeros(shp, np.float32)
         return np.ctypeslib.as_array(res, shape=(n,)).copy().reshape(shp)
 
+    # ---- in-place prediction (XGBoosterPredictFromDense / FromCSR / FromCudaArray)
+    def _inplace_proxy(self, base_margin):
+        if base_margin is None:
+            return None
+        p = self.proxy_create()
+        try:
+            self._check(self.lib.XGDMatrixSetInfoFromInterface(p, _cstr("base_margin"), _cstr(self._host_iface(np.ascontiguousarray(base_margin, np.float32)))))
+        except Exception:
+            self.dmatrix_free(p)
+            raise
+        return p
+
+    def _inplace_call(self, fn, args, base_margin):
+        shape, dim, res = C.POINTER(c_bst_ulong)(), c_bst_ulong(), C.POINTER(C.c_float)()
+        p = self._inplace_proxy(base_margin)
+        try:
+            self._check(fn(*args(p), C.byref(shape), C.byref(dim), C.byref(res)))
+        finally:
+            if p is not None:
+                self.dmatrix_free(p)
+        return res, tuple(int(shape[i]) for i in range(dim.value))
+
+    @staticmethod
+    def _host_result(res, shp):
+        n = int(np.prod(shp)) if shp else 0
+        return np.zeros(shp, np.float32) if n == 0 else np.ctypeslib.as_array(res, shape=(n,)).copy().reshape(shp)
+
+    def booster_inplace_dense(self, h, arr, cfg, base_margin=None):
+        """arr: a numpy array of any layout and numeric dtype, read at its own dtype and strides"""
+        ai = arr.__array_interface__
+        iface = {"data": [int(ai["data"][0]), True], "shape": [int(d) for d in ai["shape"]], "typestr": ai["typestr"],
+                 "strides": None if ai.get("strides") is None else [int(d) for d in ai["strides"]], "version": 3}
+        res, shp = self._inplace_call(self.lib.XGBoosterPredictFromDense,
+                                      lambda p: (h, _cstr(json.dumps(iface)), _cstr(json.dumps(cfg)), p), base_margin)
+        return self._host_result(res, shp)
+
+    def booster_inplace_csr(self, h, indptr, indices, data, ncol, cfg, base_margin=None):
+        indptr = np.ascontiguousarray(indptr, np.int64)
+        indices = np.ascontiguousarray(indices, np.int32)
+        data = np.ascontiguousarray(data, np.float32)
+        res, shp = self._inplace_call(self.lib.XGBoosterPredictFromCSR,
+                                      lambda p: (h, _cstr(self._host_iface(indptr)), _cstr(self._host_iface(indices)), _cstr(self._host_iface(data)),
+                                                 c_bst_ulong(int(ncol)), _cstr(json.dumps(cfg)), p), base_margin)
+        return self._host_result(res, shp)
+
+    def booster_inplace_cuda(self, h, iface, cfg, base_margin=None):
+        """iface: a __cuda_array_interface__ dict; returns (device pointer owned by the booster, shape)"""
+        doc = {"data": [int(iface["data"][0]), bool(iface["data"][1])], "shape": [int(d) for d in iface["shape"]], "typestr": iface["typestr"],
+               "strides": None if iface.get("strides") is None else [int(d) for d in iface["strides"]], "version": 3}
+        if "stream" in iface:                # absent: the engine synchronises the device before reading the array
+            doc["stream"] = None if iface["stream"] is None else int(iface["stream"])
+        res, shp = self._inplace_call(self.lib.XGBoosterPredictFromCudaArray,
+                                      lambda p: (h, _cstr(json.dumps(doc)), _cstr(json.dumps(cfg)), p), base_margin)
+        return C.cast(res, C.c_void_p).value or 0, shp
+
+    def booster_inplace_debug(self, h, chunk_rows=-1):
+        """(device bytes one chunk of the last in-place call staged, staging bytes held); chunk_rows >= 0 sets the rows per chunk"""
+        a, b = c_bst_ulong(), c_bst_ulong()
+        self._check(self.lib.XGB200BoosterInplaceDebug(h, C.c_int64(int(chunk_rows)), C.byref(a), C.byref(b)))
+        return int(a.value), int(b.value)
+
     def booster_save_raw(self, h, fmt):
         n = c_bst_ulong()
         ptr = C.POINTER(C.c_char)()

@@ -582,6 +582,69 @@ def _gradient_array(a, n, what):
     return np.ascontiguousarray(a)
 
 
+def _host_float32(a):
+    """a host float32 copy of an array or tensor (CUDA memory is copied to the host)"""
+    if hasattr(a, "__cuda_array_interface__"):
+        if type(a).__module__.startswith("torch"):
+            return a.detach().float().cpu().numpy()
+        import cupy
+        return cupy.asnumpy(a).astype(np.float32)
+    return np.asarray(a, dtype=np.float32)
+
+
+def _inplace_cuda_iface(a):
+    """a's __cuda_array_interface__, 1-D as one column; for torch (interface v2, no stream) the tensor's current stream"""
+    iface = dict(a.__cuda_array_interface__)
+    if "stream" not in iface and type(a).__module__.startswith("torch"):
+        import torch
+        iface["stream"] = torch.cuda.current_stream(a.device).cuda_stream or 1
+    shape = tuple(int(d) for d in iface["shape"])
+    strides = iface.get("strides")
+    if len(shape) == 1:
+        shape = (shape[0], 1)
+        if strides is not None:
+            strides = (int(strides[0]), int(strides[0]))
+    iface["shape"] = shape
+    iface["strides"] = None if strides is None else tuple(int(d) for d in strides)
+    return iface
+
+
+class _DeviceResult:
+    """The booster's device result as a __cuda_array_interface__ (valid until the booster's next call: copied at once)."""
+
+    def __init__(self, ptr, shape):
+        self.__cuda_array_interface__ = {"data": (int(ptr), False), "shape": tuple(shape), "typestr": "<f4", "strides": None,
+                                         "version": 3, "stream": None}
+
+
+def _device_result(data, ptr, shape):
+    """A copy of the device result: a torch tensor on data's device for torch, cupy for cupy, else numpy."""
+    mod = type(data).__module__
+    if int(np.prod(shape)) == 0:
+        ptr = 0
+    if mod.startswith("cupy"):
+        import cupy
+        return cupy.array(_DeviceResult(ptr, shape), copy=True) if ptr else cupy.zeros(shape, cupy.float32)
+    import torch
+    dev = data.device if mod.startswith("torch") else torch.device("cuda", torch.cuda.current_device())
+    t = torch.as_tensor(_DeviceResult(ptr, shape), device=dev).clone() if ptr else torch.zeros(shape, dtype=torch.float32, device=dev)
+    return t if mod.startswith("torch") else t.cpu().numpy()
+
+
+def _frame_array(df):
+    """A numeric pandas frame as one 2-D array: its own dtype when the columns share it, else each column rounded to float32 on
+    its own (what DMatrix(df) does per column); other frames as DMatrix(df, missing=...) converts them."""
+    dts = list(df.dtypes)
+    if dts and all(isinstance(t, np.dtype) and t.kind in "fiub" for t in dts):
+        if all(t == dts[0] for t in dts):
+            return df.to_numpy()
+        out = np.empty(df.shape, np.float32, order="F")
+        for j in range(df.shape[1]):
+            out[:, j] = df.iloc[:, j].to_numpy().astype(np.float32)
+        return out
+    return df.to_numpy(dtype=np.float32, na_value=np.nan)
+
+
 class Booster:
     """A gradient-boosted tree model trained / evaluated by the CUDA engine."""
 
@@ -757,12 +820,14 @@ class Booster:
             self.feature_types = ft
 
     def _validate_features(self, data):
-        if data.num_row() == 0:
+        self._check_feature_names(data.feature_names, data.num_row(), data.num_col())
+
+    def _check_feature_names(self, fn, nrow, ncol):
+        if nrow == 0:
             return
-        fn = data.feature_names
         mine = self.feature_names
         if mine is None or fn is None:
-            if mine is not None and fn is None and len(mine) != data.num_col():
+            if mine is not None and fn is None and len(mine) != ncol:
                 raise ValueError("feature_names mismatch: training data did not have the following fields: " + ", ".join(mine))
             return
         if list(mine) != list(fn):
@@ -845,6 +910,49 @@ class Booster:
         cfg = {"type": ptype, "training": bool(training), "iteration_begin": int(iteration_range[0]),
                "iteration_end": int(iteration_range[1]), "strict_shape": bool(strict_shape)}
         return get_backend().booster_predict(self.handle, data.handle, cfg)
+
+    def inplace_predict(self, data, iteration_range=(0, 0), predict_type="value", missing=np.nan, validate_features=True,
+                        base_margin=None, strict_shape=False):
+        """predict(DMatrix(data, missing=missing)) without the DMatrix, bit for bit: `data` is read at its own dtype and strides.
+
+        data: a numpy array (any bool, integer or float dtype, any layout; 1-D is one column), an object with
+        `__cuda_array_interface__` (torch tensors, cupy arrays: read in place after the producer's stream), a scipy CSR / CSC
+        matrix (absent entries are missing, `missing` does not apply to them) or a numeric pandas frame.  predict_type: "value"
+        (predict()) or "margin" (output_margin=True).  base_margin: (n,) or (n, outputs), host or CUDA.  Returns a torch CUDA
+        tensor for a torch CUDA input, a cupy array for a cupy input, numpy otherwise (upstream returns cupy for every device
+        input)."""
+        if predict_type not in ("value", "margin"):
+            raise ValueError("predict_type must be 'value' or 'margin', got %r" % (predict_type,))
+        cfg = {"type": 0 if predict_type == "value" else 1, "iteration_begin": int(iteration_range[0]),
+               "iteration_end": int(iteration_range[1]), "strict_shape": bool(strict_shape),
+               "missing": float(np.nan if missing is None else missing)}
+        be = get_backend()
+        bm = None if base_margin is None else _host_float32(base_margin).reshape(-1)
+        names = None
+        if hasattr(data, "__cuda_array_interface__"):
+            iface = _inplace_cuda_iface(data)
+            shape = iface["shape"]
+            if validate_features and len(shape) == 2:
+                self._check_feature_names(None, shape[0], shape[1])
+            ptr, out_shape = be.booster_inplace_cuda(self.handle, iface, cfg, bm)
+            return _device_result(data, ptr, out_shape)
+        if _is_scipy_sparse(data):
+            csr = data.tocsr()
+            if validate_features:
+                self._check_feature_names(None, csr.shape[0], csr.shape[1])
+            return be.booster_inplace_csr(self.handle, csr.indptr, csr.indices, csr.data, csr.shape[1], cfg, bm)
+        if _is_pandas_df(data):
+            names = [str(c) for c in data.columns]
+            arr = _frame_array(data)
+        else:
+            arr = np.asarray(data)
+            if arr.dtype == object:
+                arr = arr.astype(np.float32)
+            if arr.ndim == 1:
+                arr = arr.reshape(-1, 1)
+        if validate_features and arr.ndim == 2:
+            self._check_feature_names(names, arr.shape[0], arr.shape[1])
+        return be.booster_inplace_dense(self.handle, arr, cfg, bm)
 
     # ---- model IO
     def save_raw(self, raw_format="ubj"):

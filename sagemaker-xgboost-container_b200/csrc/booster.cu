@@ -574,6 +574,12 @@ std::string colsample_mask(unsigned seed, int tree_index, int F, float frac) {
 Booster::Booster() {}
 Booster::~Booster() {
   for (auto& p : pending_) if (p.ready) cudaEventDestroy(p.ready);
+  if (inplace_.copy) {
+    cudaStreamSynchronize(inplace_.copy);
+    cudaStreamDestroy(inplace_.copy);
+    for (int b = 0; b < 2; ++b) { cudaEventDestroy(inplace_.copied[b]); cudaEventDestroy(inplace_.consumed[b]); }
+  }
+  if (inplace_.pinned) cudaFreeHost(inplace_.pinned);
 }
 
 const std::map<std::string, int>& objective_table() {
@@ -1065,17 +1071,24 @@ float* Booster::dart_begin_round(DMatrix* dtrain, PredCache& c, int round) {
   return dart_drop_margin_.p;
 }
 
-void Booster::dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop,
-                          float* m_full, float* m_drop) {
+DartArgs Booster::dart_args(const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop) {
   cudaStream_t s = engine_stream();
   upload_model();
   const size_t m = ids.size();
   dart_ids_.ensure(m); dart_coef_.ensure(2 * m);
   CUDA_OK(cudaMemcpyAsync(dart_ids_.p, ids.data(), sizeof(int) * m, cudaMemcpyHostToDevice, s));
   CUDA_OK(cudaMemcpyAsync(dart_coef_.p, coef_full.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
-  if (m_drop) CUDA_OK(cudaMemcpyAsync(dart_coef_.p + m, coef_drop.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
-  DartArgs a{}; a.X = dm->X.p; a.n = dm->n; a.F = dm->F; a.nodes = d_nodes.p; a.tree_offset = d_tree_offset.p; a.tree_info = d_tree_info.p;
+  if (!coef_drop.empty()) CUDA_OK(cudaMemcpyAsync(dart_coef_.p + m, coef_drop.data(), sizeof(float) * m, cudaMemcpyHostToDevice, s));
+  DartArgs a{}; a.nodes = d_nodes.p; a.tree_offset = d_tree_offset.p; a.tree_info = d_tree_info.p;
   a.trees = dart_ids_.p; a.ntrees = (int)m; a.K = param_.num_outputs(); a.coef_full = dart_coef_.p; a.coef_drop = dart_coef_.p + m;
+  return a;
+}
+
+void Booster::dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop,
+                          float* m_full, float* m_drop) {
+  cudaStream_t s = engine_stream();
+  DartArgs a = dart_args(ids, coef_full, m_drop ? coef_drop : std::vector<float>());
+  a.X = dm->X.p; a.n = dm->n; a.F = dm->F;
   a.m_full = m_full; a.m_drop = m_drop;
   launch_dart_margin(a, s);
   Comm::get().sync_stream(s);            // the host vectors and the list buffers are reused by the next call
@@ -1636,20 +1649,26 @@ static size_t host_span(const GradInput& in) {
 // in's elements as the kernel reads them.  Device memory is read in place once the engine stream is ordered after the
 // producer: an event on the given stream, or with no stream named at all a device synchronise.  Host memory is copied to
 // the staging buffer at staging_offset bytes, which boost_one_iter has sized for the host arrays only.
+// s waits for the work the producer of a device array queued (stream as GradInput::stream): an event on the given stream,
+// nothing for null, a device synchronise when no stream is named at all
+static void wait_for_producer(uint64_t stream, cudaStream_t s) {
+  if (stream == GradInput::kNoStream) CUDA_OK(cudaDeviceSynchronize());
+  else if (stream != 0) {
+    const cudaStream_t ps = stream == 1 ? cudaStreamLegacy : stream == 2 ? cudaStreamPerThread : reinterpret_cast<cudaStream_t>(stream);
+    cudaEvent_t ev; CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    const cudaError_t e1 = cudaEventRecord(ev, ps), e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(s, ev, 0) : e1;
+    cudaEventDestroy(ev);
+    CUDA_OK(e2);
+  }
+}
+
 GradArray Booster::custom_array(const GradInput& in, bool device, size_t staging_offset) {
   const int64_t isz = in.f64 ? 8 : 4;
   GradArray a{}; a.s0 = in.s0 / isz; a.s1 = in.s1 / isz; a.f64 = in.f64 ? 1 : 0; a.data = in.ptr;
   if (in.n == 0 || in.m == 0) return a;
   cudaStream_t s = engine_stream();
   if (device) {
-    if (in.stream == GradInput::kNoStream) CUDA_OK(cudaDeviceSynchronize());
-    else if (in.stream != 0) {
-      const cudaStream_t ps = in.stream == 1 ? cudaStreamLegacy : in.stream == 2 ? cudaStreamPerThread : reinterpret_cast<cudaStream_t>(in.stream);
-      cudaEvent_t ev; CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      const cudaError_t e1 = cudaEventRecord(ev, ps), e2 = e1 == cudaSuccess ? cudaStreamWaitEvent(s, ev, 0) : e1;
-      cudaEventDestroy(ev);
-      CUDA_OK(e2);
-    }
+    wait_for_producer(in.stream, s);
     return a;
   }
   int64_t lo, hi; host_extent(in, &lo, &hi);
@@ -2013,8 +2032,16 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     shape->assign({(uint64_t)n, (uint64_t)nt});
     return;
   }
-  DevBuf<float>& margin = pred_margin_;
   predict_margin(dm, tb, te);
+  finish_predict(n, type, strict_shape, out, shape, nullptr);
+}
+
+// the margins of n rows in pred_margin_ -> predict()'s output of type 0 (the objective's transform) or 1 (margins), shaped; into
+// *out, or with dev_out != nullptr left on the device (*dev_out, valid until the next prediction)
+void Booster::finish_predict(int64_t n, int type, bool strict_shape, std::vector<float>* out, std::vector<uint64_t>* shape, const float** dev_out) {
+  cudaStream_t s = engine_stream();
+  const int K = param_.num_outputs();
+  DevBuf<float>& margin = pred_margin_;
   int out_cols = K;
   DevBuf<float>& cls = pred_cls_;
   if (type == 0) {
@@ -2022,11 +2049,159 @@ void Booster::predict(DMatrix* dm, int type, bool training, int iter_begin, int 
     else if (param_.objective == kSoftprob) launch_transform(margin.p, n, K, param_.objective, nullptr, s);
     else launch_transform(margin.p, n * K, 1, param_.objective, nullptr, s);       // element-wise over the n x K outputs
   }
-  out->resize((size_t)n * out_cols);
-  if (!out->empty()) CUDA_OK(cudaMemcpyAsync(out->data(), (type == 0 && param_.objective == kSoftmax) ? cls.p : margin.p, sizeof(float) * out->size(), cudaMemcpyDeviceToHost, s));
+  const float* src = (type == 0 && param_.objective == kSoftmax) ? cls.p : margin.p;
+  if (dev_out) *dev_out = src;
+  else {
+    out->resize((size_t)n * out_cols);
+    if (!out->empty()) CUDA_OK(cudaMemcpyAsync(out->data(), src, sizeof(float) * out->size(), cudaMemcpyDeviceToHost, s));
+  }
   Comm::get().sync_stream(s);
   if (out_cols == 1 && !strict_shape) shape->assign({(uint64_t)n});
   else shape->assign({(uint64_t)n, (uint64_t)out_cols});
+}
+
+// ---------------------------------------------------------------------------------------------
+// in-place prediction (upstream Booster.inplace_predict -> XGBoosterPredictFromDense / FromCSR / FromCudaArray; DESIGN.md
+// "In-place prediction"): predict(DMatrix(X)) without the DMatrix
+// ---------------------------------------------------------------------------------------------
+void Booster::inplace_predict(const InputDesc& in, bool on_device, uint64_t stream, int type, int iter_begin, int iter_end, bool strict_shape,
+                              const std::vector<float>& base_margin_rows, std::vector<float>* out, std::vector<uint64_t>* shape, const float** dev_out) {
+  configure();
+  cudaStream_t s = engine_stream();
+  const int K = param_.num_outputs();
+  const int rounds = layers();
+  if (iter_end == 0) iter_end = rounds;
+  B200_CHECK(iter_begin >= 0 && iter_begin <= iter_end && iter_end <= rounds, "Invalid iteration range: [" + std::to_string(iter_begin) + ", " + std::to_string(iter_end) + ") for a model with " + std::to_string(rounds) + " rounds");
+  B200_CHECK(type == 0 || type == 1, "inplace_predict: predict type " + std::to_string(type) + " is not supported (0 value, 1 margin)");
+  const int64_t n = in.n; const int F = in.F;
+  B200_CHECK(n >= 0 && F >= 0 && n < (int64_t)0x7fffffff, "inplace_predict: bad shape");
+  B200_CHECK(num_feature_ == 0 || F <= num_feature_, "feature count mismatch: the data has " + std::to_string(F) + " columns, the model was trained on " +
+             std::to_string(num_feature_) + " features");
+  B200_CHECK(in.indptr ? in.type == kInF32 : (in.type >= kInF32 && in.type <= kInBool), "inplace_predict: element type " + std::to_string(in.type) + " is not supported");
+  if (!base_margin_rows.empty()) B200_CHECK(base_margin_rows.size() == (size_t)n * K, "base_margin size does not match rows x groups");
+  if (on_device) {
+    B200_CHECK(!in.indptr, "inplace_predict: CSR input is read from host memory");
+    cudaPointerAttributes attr{};
+    const bool dev = n * F > 0 && cudaPointerGetAttributes(&attr, in.ptr) == cudaSuccess && (attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged);
+    (void)cudaGetLastError();
+    if (n * F > 0) {
+      B200_CHECK(dev, "inplace_predict: the CUDA array interface points at memory that is not CUDA device memory");
+      int d = 0; CUDA_OK(cudaGetDevice(&d));
+      B200_CHECK(attr.device == d, "inplace_predict: the CUDA array is on device " + std::to_string(attr.device) + " but the booster predicts on device " + std::to_string(d));
+    }
+  }
+  const int tb = iteration_indptr_[iter_begin], te = iteration_indptr_[iter_end];
+  upload_model();
+  DevBuf<float>& margin = pred_margin_; margin.ensure((size_t)n * K);
+  if (!base_margin_rows.empty()) { if (n) CUDA_OK(cudaMemcpyAsync(margin.p, base_margin_rows.data(), sizeof(float) * n * K, cudaMemcpyHostToDevice, s)); }
+  else launch_fill(margin.p, n * K, base_margin(), s);
+  DartArgs dart{};
+  if (dart_.on && te > tb) {
+    std::vector<int> ids; std::vector<float> coef;
+    for (int t = tb; t < te; ++t) { ids.push_back(t); coef.push_back(weight_drop_[t]); }
+    dart = dart_args(ids, coef, {});
+  }
+  // margins of chunk d (its rows from r0 on) into margin rows [r0, r0 + d.n)
+  auto run = [&](const InputDesc& d, int64_t r0) {
+    if (dart_.on) {
+      if (te <= tb) return;
+      DartArgs a = dart; a.n = d.n; a.F = d.F; a.m_full = margin.p + r0 * K; a.m_drop = nullptr;
+      launch_dart_margin_inplace(a, d, s);
+      return;
+    }
+    PredictArgs pa = predict_args(nullptr, tb, te);
+    pa.n = d.n; pa.F = d.F; pa.margin = margin.p + r0 * K; pa.has_nan = 1;
+    launch_predict_inplace(pa, d, s);
+  };
+  // a chunk of rows x F float32 in the scratch, C order, NaN = missing
+  auto scratch_desc = [&](int64_t rows) { InputDesc c; c.ptr = inplace_.scratch.p; c.type = kInF32; c.s0 = 4 * (int64_t)F; c.s1 = 4; c.n = rows; c.F = F; return c; };
+  const bool convert = !in.indptr && !in_read_in_place(in.type);
+  const int isz = in_itemsize(in.type);
+  const size_t cap = kInplaceStageBytes;
+  inplace_.staged_bytes = 0;
+  if (n > 0 && on_device) {
+    wait_for_producer(stream, s);
+    if (!convert) run(in, 0);
+    else {
+      const int64_t rows = inplace_chunk_rows(n, 4 * (int64_t)F, cap, inplace_.debug_chunk_rows);
+      inplace_.scratch.ensure((size_t)rows * F);
+      for (int64_t r0 = 0; r0 < n; r0 += rows) {
+        const int64_t m = std::min(rows, n - r0);
+        launch_convert_rows(in, r0, m, inplace_.scratch.p, s);
+        run(scratch_desc(m), r0);
+        inplace_.staged_bytes = std::max<uint64_t>(inplace_.staged_bytes, (uint64_t)m * F * 4);
+      }
+    }
+  } else if (n > 0) {
+    // host input: row chunks at their own dtype through pinned buffer b = chunk & 1 into device buffer b (copy stream), predicted on
+    // the engine stream while the CPU packs and the copy engine moves the next chunk
+    const int64_t row_bytes = (int64_t)F * (convert ? std::max(isz, 4) : isz);
+    B200_CHECK(in.indptr || inplace_row_fits(row_bytes, cap), "inplace_predict: a row of " + std::to_string(row_bytes) + " bytes does not fit the staging buffer");
+    if (!inplace_.copy) {
+      CUDA_OK(cudaHostAlloc(&inplace_.pinned, 2 * cap, cudaHostAllocDefault));
+      CUDA_OK(cudaStreamCreateWithFlags(&inplace_.copy, cudaStreamNonBlocking));
+      for (int b = 0; b < 2; ++b) { CUDA_OK(cudaEventCreateWithFlags(&inplace_.copied[b], cudaEventDisableTiming));
+                                    CUDA_OK(cudaEventCreateWithFlags(&inplace_.consumed[b], cudaEventDisableTiming)); }
+    }
+    inplace_.stage.ensure(2 * cap);
+    const int64_t dense_rows = in.indptr ? 0 : inplace_chunk_rows(n, row_bytes, cap, inplace_.debug_chunk_rows);
+    if (convert) inplace_.scratch.ensure((size_t)dense_rows * F);
+    const unsigned char* base = static_cast<const unsigned char*>(in.ptr);
+    int64_t r0 = 0;
+    for (int c = 0; r0 < n; ++c) {
+      const int b = c & 1;
+      if (c >= 2) { CUDA_OK(cudaEventSynchronize(inplace_.copied[b])); CUDA_OK(cudaStreamWaitEvent(inplace_.copy, inplace_.consumed[b], 0)); }
+      unsigned char* hp = inplace_.pinned + b * cap; unsigned char* dp = inplace_.stage.p + b * cap;
+      int64_t r1; size_t bytes; InputDesc cd = in;
+      if (in.indptr) {
+        r1 = inplace_csr_chunk_end(in.indptr, n, r0, cap, inplace_.debug_chunk_rows);
+        B200_CHECK(r1 > r0, "inplace_predict: CSR row " + std::to_string(r0) + " has more entries than the staging buffer holds");
+        const int64_t e0 = in.indptr[r0], nnz = in.indptr[r1] - e0, rows = r1 - r0;
+        const size_t off_i = inplace_csr_bytes(rows, 0), off_v = off_i + (((size_t)nnz * 4 + 15) & ~size_t(15));
+        memcpy(hp, in.indptr + r0, sizeof(int64_t) * (rows + 1));
+        memcpy(hp + off_i, in.indices + e0, sizeof(int32_t) * nnz);
+        memcpy(hp + off_v, static_cast<const float*>(in.ptr) + e0, sizeof(float) * nnz);
+        bytes = off_v + sizeof(float) * nnz;
+        cd.indptr = reinterpret_cast<const int64_t*>(dp); cd.indices = reinterpret_cast<const int32_t*>(dp + off_i) - e0;
+        cd.ptr = reinterpret_cast<const float*>(dp + off_v) - e0;
+      } else {
+        r1 = std::min(n, r0 + dense_rows);
+        const int64_t rows = r1 - r0, rb = (int64_t)F * isz;
+        if (in.s1 == isz) {                                  // rows of contiguous elements: C order
+          if (in.s0 == rb) memcpy(hp, base + r0 * in.s0, (size_t)(rows * rb));
+          else for (int64_t r = 0; r < rows; ++r) memcpy(hp + r * rb, base + (r0 + r) * in.s0, (size_t)rb);
+          cd.s0 = rb; cd.s1 = isz;
+        } else if (in.s0 == isz) {                           // columns of contiguous elements: F order
+          for (int f = 0; f < F; ++f) memcpy(hp + (int64_t)f * rows * isz, base + r0 * isz + (int64_t)f * in.s1, (size_t)(rows * isz));
+          cd.s0 = isz; cd.s1 = rows * isz;
+        } else {
+          for (int64_t r = 0; r < rows; ++r)
+            for (int f = 0; f < F; ++f) memcpy(hp + r * rb + (int64_t)f * isz, base + (r0 + r) * in.s0 + (int64_t)f * in.s1, (size_t)isz);
+          cd.s0 = rb; cd.s1 = isz;
+        }
+        bytes = (size_t)(rows * rb);
+        cd.ptr = dp;
+      }
+      cd.n = r1 - r0;
+      if (bytes) CUDA_OK(cudaMemcpyAsync(dp, hp, bytes, cudaMemcpyHostToDevice, inplace_.copy));
+      CUDA_OK(cudaEventRecord(inplace_.copied[b], inplace_.copy));
+      CUDA_OK(cudaStreamWaitEvent(s, inplace_.copied[b], 0));
+      uint64_t used = bytes;
+      if (convert) { launch_convert_rows(cd, 0, cd.n, inplace_.scratch.p, s); cd = scratch_desc(cd.n); used += (uint64_t)cd.n * F * 4; }
+      run(cd, r0);
+      CUDA_OK(cudaEventRecord(inplace_.consumed[b], s));
+      inplace_.staged_bytes = std::max(inplace_.staged_bytes, used);
+      r0 = r1;
+    }
+  }
+  finish_predict(n, type, strict_shape, out, shape, dev_out);
+  if (inplace_.copy) CUDA_OK(cudaStreamSynchronize(inplace_.copy));   // the pinned buffers are free again when the call returns
+}
+
+void Booster::inplace_debug(int64_t chunk_rows, uint64_t* staged_bytes, uint64_t* staging_capacity) {
+  if (chunk_rows >= 0) inplace_.debug_chunk_rows = chunk_rows;
+  if (staged_bytes) *staged_bytes = inplace_.staged_bytes;
+  if (staging_capacity) *staging_capacity = (uint64_t)inplace_.stage.n + (uint64_t)inplace_.scratch.n * sizeof(float);
 }
 
 void Booster::debug_build_root_hist(DMatrix* dm, const float* gpair_host, std::vector<long long>* hist_out, float* scales_out,
@@ -2102,9 +2277,10 @@ void Booster::predict_contribs(DMatrix* dm, int tb, int te, std::vector<float>* 
 }
 
 PredictArgs Booster::predict_args(DMatrix* dm, int tree_begin, int tree_end) {
-  PredictArgs pa{}; pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
+  PredictArgs pa{}; if (dm) { pa.X = dm->X.p; pa.n = dm->n; pa.F = dm->F; pa.has_nan = dm->has_missing ? 1 : 0; }
+  pa.nodes = d_nodes.p; pa.tree_offset = d_tree_offset.p; pa.tree_info = d_tree_info.p;
   pa.tree_begin = tree_begin; pa.tree_end = tree_end; pa.K = param_.num_outputs(); pa.margin = nullptr; pa.leaf = nullptr;
-  pa.h_tree_offset = h_tree_offset.data(); pa.has_nan = dm->has_missing ? 1 : 0; pa.children_adjacent = children_adjacent_ ? 1 : 0;
+  pa.h_tree_offset = h_tree_offset.data(); pa.children_adjacent = children_adjacent_ ? 1 : 0;
   pa.model_F = num_feature_;
   return pa;
 }

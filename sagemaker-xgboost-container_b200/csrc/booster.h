@@ -179,6 +179,15 @@ class Booster {
   void predict(DMatrix* dm, int type, bool training, int iter_begin, int iter_end, bool strict_shape,
                std::vector<float>* out, std::vector<uint64_t>* shape);
   void predict_contribs(DMatrix* dm, int tree_begin, int tree_end, std::vector<float>* out, std::vector<uint64_t>* shape);
+  // predict(DMatrix(in)) of type 0 (value) or 1 (margin) without the DMatrix, reading `in` at its own dtype and strides
+  // (DESIGN.md "In-place prediction").  on_device: in is CUDA memory on the booster's device, read in place once the engine stream
+  // is ordered after `stream` (GradInput::stream); else host memory, staged in row chunks.  base_margin_rows: n x outputs or
+  // empty.  The result goes to *out, or with dev_out to *dev_out (device memory owned by the booster, valid until its next call).
+  void inplace_predict(const InputDesc& in, bool on_device, uint64_t stream, int type, int iter_begin, int iter_end, bool strict_shape,
+                       const std::vector<float>& base_margin_rows, std::vector<float>* out, std::vector<uint64_t>* shape, const float** dev_out);
+  // chunk_rows >= 0 sets the rows per chunk of in-place staging (0: as many as the staging buffer holds); *staged_bytes: the
+  // most device bytes one chunk of the last in-place call staged or converted; *staging_capacity: the staging and scratch held
+  void inplace_debug(int64_t chunk_rows, uint64_t* staged_bytes, uint64_t* staging_capacity);
   // model IO
   std::string save_model_buffer(const std::string& format);      // "ubj" | "json"
   void load_model_buffer(const char* buf, size_t len);
@@ -228,6 +237,15 @@ class Booster {
   void run_predict(DMatrix* dm, PredictArgs pa, cudaStream_t s);
   // predict()'s margins of trees [tb, te) on dm into pred_margin_ (base margin, then the trees; booster=dart: fl(w_t * leaf_t))
   void predict_margin(DMatrix* dm, int tb, int te);
+  void finish_predict(int64_t n, int type, bool strict_shape, std::vector<float>* out, std::vector<uint64_t>* shape, const float** dev_out);
+  // in-place prediction's staging (host inputs) and float32 scratch (converted dtypes), reused across calls, bounded whatever n is
+  struct InplaceState {
+    unsigned char* pinned = nullptr;            // 2 x kInplaceStageBytes of pinned host memory
+    DevBuf<unsigned char> stage;                // 2 x kInplaceStageBytes on the device
+    DevBuf<float> scratch;                      // one chunk converted to float32
+    cudaStream_t copy = nullptr; cudaEvent_t copied[2] = {}, consumed[2] = {};
+    int64_t debug_chunk_rows = 0; uint64_t staged_bytes = 0;
+  } inplace_;
   DevBuf<DevNode> bin_nodes_;                   // d_nodes with each split's cond replaced by its bin threshold (run_predict)
   std::map<std::string, std::string> raw_params_;
   std::vector<std::string> eval_metrics_;
@@ -295,6 +313,7 @@ class Booster {
   void append_device_tree(int class_id, size_t device_offset, int max_nodes, PendingTree pt, float weight);
   std::vector<int> dart_drop_set(int round) const;
   float* dart_begin_round(DMatrix* dtrain, PredCache& c, int round);
+  DartArgs dart_args(const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop);   // uploaded list
   void dart_margin(DMatrix* dm, const std::vector<int>& ids, const std::vector<float>& coef_full, const std::vector<float>& coef_drop,
                    float* m_full, float* m_drop);
   void reserve_nodes(size_t count, size_t slack);    // room for `count` more nodes in d_nodes

@@ -469,6 +469,93 @@ int XGBoosterPredictFromDMatrix(BoosterHandle handle, DMatrixHandle dmat, const 
   *out_shape = box->ret_shape.data(); *out_dim = box->ret_shape.size(); *out_result = box->ret_vec.data();
   API_END();
 }
+namespace {
+// an in-place input as an array interface (numpy __array_interface__ / __cuda_array_interface__ as JSON): 2-D, any supported
+// typestr, optional byte "strides" (multiples of the item size, negative allowed), optional v3 "stream" (GradInput::stream)
+InputDesc inplace_desc(const char* json, uint64_t* stream) {
+  JPtr a = parse_json(json);
+  const JValue& shape = a->at("shape");
+  if (shape.length() != 2) throw Error("inplace_predict: expecting a 2-dimensional array, got " + std::to_string(shape.length()) + " dimension(s)");
+  std::string why;
+  InputDesc d;
+  d.type = in_type_of(a->at("typestr").s, &why);
+  if (d.type < 0) throw Error("inplace_predict: " + why);
+  const int64_t isz = in_itemsize(d.type);
+  d.n = (int64_t)shape.num_at(0); d.F = (int)shape.num_at(1);
+  d.s1 = isz; d.s0 = isz * d.F;
+  if (a->has("strides") && a->at("strides").type != JValue::kNull) {
+    const JValue& st = a->at("strides");
+    if (st.length() != 2) throw Error("inplace_predict: strides and shape differ in length");
+    d.s0 = st.arr[0]->as_int(); d.s1 = st.arr[1]->as_int();
+  }
+  d.ptr = reinterpret_cast<const void*>((uintptr_t)a->at("data").arr[0]->as_int());
+  B200_CHECK(d.s0 % isz == 0 && d.s1 % isz == 0 && (uintptr_t)d.ptr % (uintptr_t)isz == 0,
+             "inplace_predict: the data pointer and strides must be multiples of the item size (" + std::to_string(isz) + " bytes)");
+  *stream = !a->has("stream") ? GradInput::kNoStream : a->at("stream").type == JValue::kNull ? 0 : (uint64_t)a->at("stream").as_int();
+  return d;
+}
+// the config of the XGBoosterPredictFrom* entries: {"type": 0 | 1, "iteration_begin", "iteration_end", "strict_shape", "missing"}
+// (other keys upstream passes, e.g. "training", are ignored), then the prediction; the base margin comes from the proxy m
+int inplace_entry(BoosterHandle handle, InputDesc d, bool device, uint64_t stream, const char* config, DMatrixHandle m,
+                  bst_ulong const** out_shape, bst_ulong* out_dim, const float** out_result) {
+  API_BEGIN();
+  BoosterBox* box = static_cast<BoosterBox*>(handle);
+  JPtr cfg = parse_json(config ? config : "{}");
+  auto geti = [&](const char* k, int64_t def) { auto v = cfg->get(k); return v ? v->as_int() : def; };
+  auto getb = [&](const char* k, bool def) { auto v = cfg->get(k); if (!v) return def; return v->type == JValue::kBool ? v->b : v->as_int() != 0; };
+  if (!d.indptr) { auto mv = cfg->get("missing"); d.missing = mv && mv->type != JValue::kNull ? (float)mv->as_double() : std::nanf(""); }
+  static const std::vector<float> none;
+  const std::vector<float>& bm = m ? PROXY(m)->base_margin : none;
+  const float* dev = nullptr;
+  BST(handle)->inplace_predict(d, device, stream, (int)geti("type", 0), (int)geti("iteration_begin", 0), (int)geti("iteration_end", 0),
+                               getb("strict_shape", false), bm, &box->ret_vec, &box->ret_shape, device ? &dev : nullptr);
+  *out_shape = box->ret_shape.data(); *out_dim = box->ret_shape.size(); *out_result = device ? dev : box->ret_vec.data();
+  API_END();
+}
+}  // namespace
+int XGBoosterPredictFromDense(BoosterHandle handle, const char* values, const char* config, DMatrixHandle m, bst_ulong const** out_shape,
+                              bst_ulong* out_dim, const float** out_result) {
+  API_BEGIN();
+  uint64_t stream = 0;
+  const InputDesc d = inplace_desc(values, &stream);
+  return inplace_entry(handle, d, false, 0, config, m, out_shape, out_dim, out_result);
+  API_END();
+}
+int XGBoosterPredictFromCudaArray(BoosterHandle handle, const char* values, const char* config, DMatrixHandle proxy, bst_ulong const** out_shape,
+                                  bst_ulong* out_dim, const float** out_result) {
+  API_BEGIN();
+  uint64_t stream = 0;
+  const InputDesc d = inplace_desc(values, &stream);
+  return inplace_entry(handle, d, true, stream, config, proxy, out_shape, out_dim, out_result);
+  API_END();
+}
+int XGBoosterPredictFromCSR(BoosterHandle handle, const char* indptr, const char* indices, const char* values, bst_ulong ncol, const char* config,
+                            DMatrixHandle m, bst_ulong const** out_shape, bst_ulong* out_dim, const float** out_result) {
+  API_BEGIN();
+  const HostArray ip = parse_array_interface(indptr), ix = parse_array_interface(indices), dv = parse_array_interface(values);
+  B200_CHECK(ip.typestr == "<i8" || ip.typestr == "<u8", "inplace_predict: CSR indptr must be 64-bit integers");
+  B200_CHECK(ix.typestr == "<i4" || ix.typestr == "<u4", "inplace_predict: CSR indices must be 32-bit integers");
+  B200_CHECK(dv.typestr == "<f4", "inplace_predict: CSR data must be float32");
+  B200_CHECK(ip.n >= 1 && ix.n == dv.n, "inplace_predict: CSR indptr must not be empty and indices / data must have the same length");
+  B200_CHECK(ncol < (bst_ulong)0x7fffffff, "inplace_predict: CSR has too many columns");
+  InputDesc d;
+  d.indptr = static_cast<const int64_t*>(ip.ptr); d.indices = static_cast<const int32_t*>(ix.ptr); d.ptr = dv.ptr; d.type = kInF32;
+  d.n = ip.n - 1; d.F = (int)ncol;
+  B200_CHECK(d.indptr[0] == 0 && d.indptr[d.n] <= dv.n, "inplace_predict: CSR indptr must start at 0 and end within the index / value arrays");
+  for (int64_t r = 0; r < d.n; ++r) B200_CHECK(d.indptr[r] <= d.indptr[r + 1], "inplace_predict: CSR indptr is not non-decreasing");
+  for (int64_t j = 0; j < d.indptr[d.n]; ++j)
+    B200_CHECK(d.indices[j] >= 0 && d.indices[j] < d.F, "inplace_predict: CSR column index " + std::to_string(d.indices[j]) + " is outside [0, " + std::to_string(d.F) + ")");
+  return inplace_entry(handle, d, false, 0, config, m, out_shape, out_dim, out_result);
+  API_END();
+}
+int XGB200BoosterInplaceDebug(BoosterHandle handle, int64_t chunk_rows, bst_ulong* staged_bytes, bst_ulong* staging_capacity) {
+  API_BEGIN();
+  uint64_t a = 0, b = 0;
+  BST(handle)->inplace_debug(chunk_rows, &a, &b);
+  if (staged_bytes) *staged_bytes = a;
+  if (staging_capacity) *staging_capacity = b;
+  API_END();
+}
 static bool ends_with(const std::string& s, const char* suf) { size_t n = strlen(suf); return s.size() >= n && s.compare(s.size() - n, n, suf) == 0; }
 int XGBoosterSaveModel(BoosterHandle handle, const char* fname) {
   API_BEGIN();

@@ -8,6 +8,7 @@
 #include "curve.h"
 #include "elementwise.h"
 #include "engine.h"
+#include "inplace.h"
 #include "misc.h"
 #include "predict_tile.h"
 #include "rng.h"
@@ -179,15 +180,15 @@ __global__ void __launch_bounds__(256) replace_missing_kernel(float* X, int64_t 
 // ---------------------------------------------------------------------------------------------
 // predictor: one thread per row, trees in model order, fp32 accumulation
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) predict_kernel(PredictArgs a) {
+template <class Src>
+__global__ void __launch_bounds__(256) predict_kernel(PredictArgs a, Src src) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= a.n) return;
-  const float* x = a.X + r * a.F;
   const int nt = a.tree_end - a.tree_begin;
   float acc = (a.K == 1 && a.margin) ? a.margin[r] : 0.f;
   for (int t = a.tree_begin; t < a.tree_end; ++t) {
     DevNode nd;
-    const int nid = tree_leaf(a.nodes + a.tree_offset[t], x, a.F, &nd);
+    const int nid = tree_leaf_by(a.nodes + a.tree_offset[t], [&](unsigned f) { return src.at(r, (int)f); }, &nd);
     if (a.margin) { if (a.K == 1) acc += nd.cond; else a.margin[r * a.K + a.tree_info[t]] += nd.cond; }
     if (a.leaf) a.leaf[r * nt + (t - a.tree_begin)] = nid;
   }
@@ -198,19 +199,18 @@ __global__ void __launch_bounds__(256) predict_kernel(PredictArgs a) {
 // (the thread-per-row kernel above gathers 4 B at a time from a 4*F-byte row: 1 % of HBM peak in round 1) and keeps the
 // trees there too, 8 B per node, so a traversal step is two LDS.  With T trees of depth D a row costs ~8*T*D instructions
 // against 4*F bytes: beyond T*D ~ 100 the kernel is issue-bound, not HBM-bound (DESIGN.md "predictor").
-template <bool HAS_NAN, bool LEAF_OUT>
-__global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, int tree_lo, int tree_hi, int pitch, int rows_per_tile, int64_t num_tiles) {
+// Src (inplace.h) stages a tile of rows: the DMatrix's float32 matrix, or an in-place input read at its own dtype and strides.
+template <bool HAS_NAN, bool LEAF_OUT, class Src>
+__global__ void __launch_bounds__(1024) predict_tiled_kernel(PredictArgs a, Src src, int tree_lo, int tree_hi, int pitch, int rows_per_tile, int64_t num_tiles) {
   extern __shared__ __align__(16) unsigned char psm[];
   int* s_toff; PNode* s_nodes;
   float* s_x = reinterpret_cast<float*>(stage_tree_chunk(a, tree_lo, tree_hi, psm, &s_toff, &s_nodes));
-  const int F = a.F, nt_chunk = tree_hi - tree_lo;
+  const int nt_chunk = tree_hi - tree_lo;
   for (int64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const int64_t r0 = tile * rows_per_tile;
     const int rows = (int)((a.n - r0 < rows_per_tile) ? a.n - r0 : rows_per_tile);
     __syncthreads();                                                            // trees staged / previous tile consumed
-    const float* src = a.X + r0 * F;
-    const int total = rows * F;
-    for (int i = threadIdx.x; i < total; i += blockDim.x) { const int r = i / F, f = i - r * F; s_x[r * pitch + f] = __ldg(src + i); }
+    src.stage(s_x, pitch, r0, rows);
     __syncthreads();
     for (int rl = threadIdx.x; rl < rows; rl += blockDim.x) {
       const float* x = s_x + rl * pitch;
@@ -327,33 +327,65 @@ PredictPlan plan_for(const PredictArgs& a) {
   return plan_predict(a.h_tree_offset, a.tree_begin, a.tree_end, a.F, a.model_F, a.children_adjacent != 0, legacy);
 }
 
+template <bool HAS_NAN, bool LEAF_OUT, class Src>
+static void launch_tiled(const PredictArgs& a, const Src& src, const PredictPlan& plan, cudaStream_t s) {
+  static bool attr = false;
+  if (!attr) { CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<HAS_NAN, LEAF_OUT, Src>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem)); attr = true; }
+  for (const PredictChunk& ch : plan.chunks) {
+    const int rows = ch.rows, threads = ch.threads;
+    const int64_t tiles = (a.n + rows - 1) / rows;
+    const int grid = (int)std::min<int64_t>(tiles, engine_num_sms() * (threads == 1024 ? 1 : 2048 / threads));
+    predict_tiled_kernel<HAS_NAN, LEAF_OUT, Src><<<grid, threads, ch.smem, s>>>(a, src, ch.tree_lo, ch.tree_hi, plan.pitch, rows, tiles);
+    ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  }
+}
+
 // executes plan_for(a): one tiled launch per tree chunk, or the thread-per-row kernel
 void launch_predict(const PredictArgs& a, cudaStream_t s) {
   if (a.n == 0 || a.tree_end <= a.tree_begin) return;
   const PredictPlan plan = plan_for(a);
+  const RowsF32 src{a.X, a.F};
   if (plan.kernel == PredictKernel::kTiled) {
-    static bool attr = false;
-    if (!attr) {
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
-      CUDA_OK(cudaFuncSetAttribute(predict_tiled_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPredictSmem));
-      attr = true;
-    }
-    const int pitch = plan.pitch;
-    for (const PredictChunk& ch : plan.chunks) {
-      const int rows = ch.rows, threads = ch.threads;
-      const int64_t tiles = (a.n + rows - 1) / rows;
-      const int grid = (int)std::min<int64_t>(tiles, engine_num_sms() * (threads == 1024 ? 1 : 2048 / threads));
-      if (a.leaf) { if (a.has_nan) predict_tiled_kernel<true, true><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles);
-                    else predict_tiled_kernel<false, true><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles); }
-      else { if (a.has_nan) predict_tiled_kernel<true, false><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles);
-             else predict_tiled_kernel<false, false><<<grid, threads, ch.smem, s>>>(a, ch.tree_lo, ch.tree_hi, pitch, rows, tiles); }
-      ++g_kernel_launches; CUDA_OK(cudaGetLastError());
-    }
+    if (a.leaf) { if (a.has_nan) launch_tiled<true, true>(a, src, plan, s); else launch_tiled<false, true>(a, src, plan, s); }
+    else { if (a.has_nan) launch_tiled<true, false>(a, src, plan, s); else launch_tiled<false, false>(a, src, plan, s); }
     return;
   }
-  predict_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, s>>>(a); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+  predict_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, s>>>(a, src); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+
+// plan_for(a) on the in-place input d (a.X unused, a.F == d.F): the NaN-aware tiled kernel, or thread-per-row, reading d
+template <class Src>
+static void launch_predict_src(const PredictArgs& a, const Src& src, cudaStream_t s) {
+  const PredictPlan plan = plan_for(a);
+  if (plan.kernel == PredictKernel::kTiled) { launch_tiled<true, false>(a, src, plan, s); return; }
+  predict_kernel<<<(unsigned)((a.n + 255) / 256), 256, 0, s>>>(a, src); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
+}
+void launch_predict_inplace(const PredictArgs& a, const InputDesc& d, cudaStream_t s) {
+  B200_CHECK(a.leaf == nullptr && a.F == d.F && a.n == d.n, "launch_predict_inplace: margins of the input's rows only");
+  if (a.n == 0 || a.tree_end <= a.tree_begin) return;
+  if (d.indptr) { launch_predict_src(a, CsrSrc{d}, s); return; }
+  switch (d.type) {
+    case kInF32: launch_predict_src(a, StridedSrc<kInF32>{d}, s); return;
+    case kInF64: launch_predict_src(a, StridedSrc<kInF64>{d}, s); return;
+    case kInF16: launch_predict_src(a, StridedSrc<kInF16>{d}, s); return;
+    default: throw Error("launch_predict_inplace: element type " + std::to_string(d.type) + " is converted to float32 first (launch_convert_rows)");
+  }
+}
+
+// rows [r0, r0 + rows) of d as float32 into out (row-major, rows x d.F, NaN = missing)
+__global__ void __launch_bounds__(256) convert_rows_kernel(InputDesc d, int64_t r0, int64_t rows, float* out) {
+  const int F = d.F;
+  const int64_t total = rows * F;
+  const bool rows_fast = (d.s0 < 0 ? -d.s0 : d.s0) < (d.s1 < 0 ? -d.s1 : d.s1);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r; int f;
+    if (rows_fast) { f = (int)(i / rows); r = i - (int64_t)f * rows; } else { r = i / F; f = (int)(i - r * F); }
+    out[r * F + f] = load_x(d, r0 + r, f);
+  }
+}
+void launch_convert_rows(const InputDesc& d, int64_t r0, int64_t rows, float* out, cudaStream_t s) {
+  if (rows * d.F <= 0) return;
+  convert_rows_kernel<<<grid_for(rows * d.F, 256, engine_num_sms() * 16), 256, 0, s>>>(d, r0, rows, out); ++g_kernel_launches; CUDA_OK(cudaGetLastError());
 }
 void launch_transform(float* m, int64_t n, int K, int objective, float* out_class, cudaStream_t s) {
   if (n == 0) return;

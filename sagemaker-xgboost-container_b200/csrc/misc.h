@@ -1,6 +1,7 @@
 // misc.h -- argument blocks and launchers for misc.cu / quantile.cu
 #pragma once
 #include "engine.h"
+#include "inplace.h"
 #include "predict_plan.h"
 
 namespace b200 {
@@ -71,6 +72,8 @@ struct DartArgs {
   float* m_drop;                                // nullptr = no dropped margin; else written as m_full minus the dropped trees
 };
 void launch_dart_margin(const DartArgs& a, cudaStream_t s);
+// the same pass (no dropped margin) reading the in-place input d instead of a.X (d: float32, float64, float16 or CSR)
+void launch_dart_margin_inplace(const DartArgs& a, const InputDesc& d, cudaStream_t s);
 
 // num_parallel_tree > 1 with subsample < 1: one tree's row sample of the round's unsampled gradients (misc.cu)
 struct SampleArgs {
@@ -91,6 +94,12 @@ void launch_count_nan(const float* X, int64_t count, float missing, int use_miss
 void launch_replace_missing(float* X, int64_t count, float missing, cudaStream_t s);
 PredictPlan plan_for(const PredictArgs& a);             // what launch_predict(a) runs
 void launch_predict(const PredictArgs& a, cudaStream_t s);
+// launch_predict's plan on the in-place input d (inplace.h; float32, float64, float16 or CSR) instead of a.X: margins only,
+// always the NaN-aware variant (no pass over the input decides has_nan)
+void launch_predict_inplace(const PredictArgs& a, const InputDesc& d, cudaStream_t s);
+// rows [r0, r0 + rows) of d converted to float32 into out (rows x d.F, row-major, NaN = missing): the element types the
+// predictor does not read itself, a bounded tile at a time
+void launch_convert_rows(const InputDesc& d, int64_t r0, int64_t rows, float* out, cudaStream_t s);
 // Prediction from the bins (predict_bins.cu).  Each value stands at the lower edge of its bin (min_vals[f] for bin 0, else
 // cut_vals[ptr + b - 1]), so `x < cond` becomes `b < t` with t the number of the feature's lower edges below cond.
 // launch_bin_thresholds copies nodes[0, count) to out with each split's cond replaced by t (as int bits); a split on a feature
