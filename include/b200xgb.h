@@ -307,6 +307,12 @@ XGB_DLL int XGB200BoosterGetTreeWeights(BoosterHandle handle, bst_ulong* len, fl
  * trees as they were before the update (trees one after another), 2 int64 per node; the nodes of layers not yet updated are 0.
  * len = 0 before the first update round.  out may be NULL to query len. */
 XGB_DLL int XGB200BoosterGetRefreshSums(BoosterHandle handle, bst_ulong* len, long long* out);
+/* while enabled, the booster keeps the cuts every tree it grows was grown on (tree_method=approx: that tree's hessian cuts);
+ * enabling clears what was kept.  GetTreeCuts returns those of the tree-th tree grown since: num_feature + 1 cut_ptrs, num_cuts
+ * cut_vals and num_feature min_vals; the output pointers may be NULL to query the sizes. */
+XGB_DLL int XGB200BoosterSetRecordCuts(BoosterHandle handle, int enable);
+XGB_DLL int XGB200BoosterGetTreeCuts(BoosterHandle handle, bst_ulong tree, bst_ulong* num_feature, bst_ulong* num_cuts, int* cut_ptrs,
+                                     float* cut_vals, float* min_vals);
 /* the configured objective's gradient pairs on `dmat` at the given margins (n x outputs per row, host), with the row sample of boosting
  * round `round` (subsample < 1: unsampled rows are (0, 0)); out_gpair: n x outputs x 2 floats (g, h).  Under
  * sampling_method=gradient_based that sample is the one tree 0 of each class takes: each class's own threshold over these

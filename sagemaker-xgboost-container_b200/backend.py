@@ -685,6 +685,21 @@ class CudaBackend:
         self._check(self.lib.XGB200BoosterGetRefreshSums(bh, C.byref(n), out.ctypes.data_as(C.POINTER(C.c_longlong))))
         return out.reshape(-1, 2)
 
+    def booster_set_record_cuts(self, bh, enable):
+        """Keep (or stop keeping) the cuts each tree is grown on (include/b200xgb.h XGB200BoosterSetRecordCuts)."""
+        self._check(self.lib.XGB200BoosterSetRecordCuts(bh, C.c_int(1 if enable else 0)))
+
+    def booster_tree_cuts(self, bh, tree):
+        """(cut_ptrs int32 [F + 1], cut_vals float32, min_vals float32 [F]) of the tree-th tree grown since recording began."""
+        nf, nc = c_bst_ulong(), c_bst_ulong()
+        self._check(self.lib.XGB200BoosterGetTreeCuts(bh, c_bst_ulong(int(tree)), C.byref(nf), C.byref(nc), None, None, None))
+        ptrs = np.zeros(nf.value + 1, np.int32)
+        vals = np.zeros(nc.value, np.float32)
+        mins = np.zeros(nf.value, np.float32)
+        self._check(self.lib.XGB200BoosterGetTreeCuts(bh, c_bst_ulong(int(tree)), C.byref(nf), C.byref(nc), ptrs.ctypes.data_as(C.POINTER(C.c_int)),
+                                                      vals.ctypes.data_as(C.POINTER(C.c_float)), mins.ctypes.data_as(C.POINTER(C.c_float))))
+        return ptrs, vals, mins
+
     def timer_start(self):
         self._check(self.lib.XGB200TimerStart())
 

@@ -520,7 +520,7 @@ def _check_unapplied(k, v):
     if k == "max_bin" and _as_float(v, 256) > 256:
         warnings.warn("max_bin=%s exceeds the 256 bins per feature of the uint8 bin codes; using max_bin=256" % v)
         return 256
-    if k == "tree_method" and str(v) in ("exact", "approx"):
+    if k == "tree_method" and str(v) == "exact":
         warnings.warn("tree_method=%s runs the CUDA hist builder (quantile-binned histograms), not xgboost's %s updater" % (v, v))
         return v
     # process_type=update refreshes / prunes the trees of a loaded model (the engine parses process_type, updater and refresh_leaf,

@@ -259,24 +259,114 @@ void DMatrix::finish_bins() {
     // second request per gathered row into the line cost more in the histograms than it saved in the partition (DESIGN §6).
     gather_stride = 128;
     bins_gather.alloc((size_t)n * 128 + 128);
-    launch_pad_rows(bins.p, bins_tail.p, tw == 8 ? 8 : 0, n, 96, bins_gather.p, 128, s);
   }
   bins_col.alloc((size_t)std::max(F, 1) * n);
-  launch_transpose_bins(bins.p, bins_tail.p, n, F, ngroups, tw, bins_col.p, s);
+  launch_bin_copies();
   Comm::get().sync_stream(s);
   binned = true;
+}
+
+void DMatrix::launch_bin_copies() {
+  cudaStream_t s = engine_stream();
+  if (bins_gather.p) launch_pad_rows(bins.p, bins_tail.p, tw == 8 ? 8 : 0, n, ngroups * kSlots, bins_gather.p, gather_stride, s);
+  launch_transpose_bins(bins.p, bins_tail.p, n, F, ngroups, tw, bins_col.p, s);
+}
+
+void DMatrix::rebin_from_hessian(const float2* gp, int max_bin) {
+  require_raw("tree_method=approx");
+  cudaStream_t s = engine_stream();
+  d_cut_vals.ensure((size_t)std::max(F, 1) * kBins);   // room for any tree's cuts: the pointers stay put from tree to tree
+  if (Comm::get().distributed()) {
+    // every rank summarises its shard with the tree's hessian as the weights, and the summaries are merged as the one-time cuts
+    // are (host-synchronising, once per class per round)
+    DevBuf<float> h; h.alloc((size_t)std::max<int64_t>(n, 1));
+    launch_hessian_column(gp, n, h.p, s);
+    HostCuts c;
+    merged_rank_cuts(h.p, max_bin, &c);
+    B200_CHECK(c.ptrs.size() == (size_t)F + 1 && c.vals.size() <= d_cut_vals.n, "tree_method=approx: merged cuts do not fit the cut buffers");
+    CUDA_OK(cudaMemcpyAsync(d_cut_ptrs.p, c.ptrs.data(), sizeof(int) * c.ptrs.size(), cudaMemcpyHostToDevice, s));
+    if (!c.vals.empty()) CUDA_OK(cudaMemcpyAsync(d_cut_vals.p, c.vals.data(), sizeof(float) * c.vals.size(), cudaMemcpyHostToDevice, s));
+    CUDA_OK(cudaMemcpyAsync(d_min_vals.p, c.mins.data(), sizeof(float) * c.mins.size(), cudaMemcpyHostToDevice, s));
+    Comm::get().sync_stream(s);                        // the host cuts and the hessian column die with this scope
+  } else {
+    int nb = std::min(max_bin, kBins);
+    if (has_missing && nb > kMissingBin) nb = kMissingBin;
+    if (!approx || approx->nb != nb) {
+      approx = std::make_unique<ApproxSketch>();
+      approx_sketch_build(X.p, n, F, nb, cuts, approx.get(), s);
+    }
+    approx_sketch_cuts(X.p, *approx, gp, d_cut_ptrs.p, d_cut_vals.p, s);
+  }
+  launch_bin(X.p, n, F, ngroups, tw, d_cut_ptrs.p, d_cut_vals.p, bins.p, bins_tail.p, s);
+  launch_bin_copies();
+  hessian_cuts = true; ++binned_version;
 }
 
 void DMatrix::set_cuts(const HostCuts& c) {
   require_raw("XGB200DMatrixSetCuts (re-binning)");
   B200_CHECK((int)c.ptrs.size() == F + 1 && (int)c.mins.size() == F, "SetCuts: cut_ptrs/min_vals do not match the number of features");
   for (int f = 0; f < F; ++f) B200_CHECK(c.ptrs[f + 1] - c.ptrs[f] >= 1 && c.ptrs[f + 1] - c.ptrs[f] <= (has_missing ? 255 : 256), "SetCuts: 1..256 cuts per feature (255 with missing values)");
-  cuts = c; binned_max_bin = -1;
+  cuts = c; binned_max_bin = -1; hessian_cuts = false;
+  approx.reset();                                     // its fixed cuts came from the cuts replaced here
   bin_with_cuts();
 }
 
-void DMatrix::ensure_binned(int max_bin) {
-  if (binned && (binned_max_bin == max_bin || binned_max_bin == -1)) return;
+// The multi-rank cuts with row weights w (device, nullptr = 1): collective, host-synchronising.
+void DMatrix::merged_rank_cuts(const float* w, int max_bin, HostCuts* out) {
+  cudaStream_t s = engine_stream();
+  Comm& comm = Comm::get();
+  // every rank summarises its shard (exact when a feature has <= cap distinct values), the summaries are
+  // all-gathered and merged, and every rank derives the same cuts.
+  const int cap = kRankSummaryCap;
+  int hm = has_missing ? 1 : 0;
+  {   // has_missing must agree across ranks (bin code 255 reservation)
+    DevBuf<unsigned> flag; flag.alloc(1); unsigned v = (unsigned)hm;
+    CUDA_OK(cudaMemcpyAsync(flag.p, &v, 4, cudaMemcpyHostToDevice, s));
+    comm.allreduce_max_u32(flag.p, 1, s);
+    CUDA_OK(cudaMemcpyAsync(&v, flag.p, 4, cudaMemcpyDeviceToHost, s)); Comm::get().sync_stream(s);
+    has_missing = v != 0;
+  }
+  std::vector<FeatureSummary> local;
+  compute_summaries_device(X.p, n, F, w, cap, &local, s);
+  const size_t per_feat = (size_t)(cap + 2);
+  const size_t rec = per_feat * (sizeof(float) + sizeof(double)) + sizeof(double);   // vals, weights, count
+  std::vector<unsigned char> sendbuf((size_t)F * rec, 0);
+  for (int f = 0; f < F; ++f) {
+    unsigned char* p = sendbuf.data() + (size_t)f * rec;
+    double cntd = (double)local[f].vals.size(); memcpy(p, &cntd, 8);
+    memcpy(p + 8, local[f].vals.data(), sizeof(float) * local[f].vals.size());
+    memcpy(p + 8 + per_feat * sizeof(float), local[f].weights.data(), sizeof(double) * local[f].weights.size());
+  }
+  const int W = comm.world();
+  DevBuf<unsigned char> dsend, drecv; dsend.alloc(sendbuf.size()); drecv.alloc(sendbuf.size() * W);
+  CUDA_OK(cudaMemcpyAsync(dsend.p, sendbuf.data(), sendbuf.size(), cudaMemcpyHostToDevice, s));
+  comm.allgather_bytes(dsend.p, drecv.p, sendbuf.size(), s);
+  std::vector<unsigned char> all(sendbuf.size() * W);
+  CUDA_OK(cudaMemcpyAsync(all.data(), drecv.p, all.size(), cudaMemcpyDeviceToHost, s));
+  Comm::get().sync_stream(s);
+  std::vector<std::vector<FeatureSummary>> per_rank(W, std::vector<FeatureSummary>(F));
+  for (int r = 0; r < W; ++r) {
+    for (int f = 0; f < F; ++f) {
+      const unsigned char* p = all.data() + (size_t)r * sendbuf.size() + (size_t)f * rec;
+      double cntd; memcpy(&cntd, p, 8); size_t c = (size_t)cntd;
+      FeatureSummary& fs = per_rank[r][f];
+      fs.vals.resize(c); fs.weights.resize(c);
+      memcpy(fs.vals.data(), p + 8, sizeof(float) * c);
+      memcpy(fs.weights.data(), p + 8 + per_feat * sizeof(float), sizeof(double) * c);
+    }
+  }
+  std::vector<FeatureSummary> merged;
+  merge_summaries(per_rank, F, &merged);
+  cuts_from_summaries(merged, max_bin, has_missing, out);
+}
+
+void DMatrix::ensure_binned(int max_bin, bool hessian_ok) {
+  if (binned && (!hessian_cuts || hessian_ok) && (binned_max_bin == max_bin || binned_max_bin == -1)) return;
+  if (hessian_cuts) {
+    // back from approx: the matrix's own (or external) cuts are still on the host, and the sketch is no longer needed
+    hessian_cuts = false; approx.reset();
+    if (binned && (binned_max_bin == max_bin || binned_max_bin == -1)) { bin_with_cuts(); return; }
+  }
   B200_CHECK(!quantile, "max_bin=" + std::to_string(max_bin) + " differs from the max_bin=" + std::to_string(quantile_max_bin) +
              " this QuantileDMatrix was built with; pass the training max_bin to QuantileDMatrix(max_bin=...)");
   B200_CHECK(max_bin >= 2, "max_bin must be >= 2");
@@ -295,53 +385,8 @@ void DMatrix::ensure_binned(int max_bin) {
     comm.sync_stream(s);
     w = row_w.p;
   }
-  if (!comm.distributed()) {
-    compute_cuts_device(X.p, n, F, w, max_bin, has_missing, &cuts, s);
-  } else {
-    // every rank summarises its shard (exact when a feature has <= cap distinct values), the summaries are
-    // all-gathered and merged, and every rank derives the same cuts.
-    const int cap = kRankSummaryCap;
-    int hm = has_missing ? 1 : 0;
-    {   // has_missing must agree across ranks (bin code 255 reservation)
-      DevBuf<unsigned> flag; flag.alloc(1); unsigned v = (unsigned)hm;
-      CUDA_OK(cudaMemcpyAsync(flag.p, &v, 4, cudaMemcpyHostToDevice, s));
-      comm.allreduce_max_u32(flag.p, 1, s);
-      CUDA_OK(cudaMemcpyAsync(&v, flag.p, 4, cudaMemcpyDeviceToHost, s)); Comm::get().sync_stream(s);
-      has_missing = v != 0;
-    }
-    std::vector<FeatureSummary> local;
-    compute_summaries_device(X.p, n, F, w, cap, &local, s);
-    const size_t per_feat = (size_t)(cap + 2);
-    const size_t rec = per_feat * (sizeof(float) + sizeof(double)) + sizeof(double);   // vals, weights, count
-    std::vector<unsigned char> sendbuf((size_t)F * rec, 0);
-    for (int f = 0; f < F; ++f) {
-      unsigned char* p = sendbuf.data() + (size_t)f * rec;
-      double cntd = (double)local[f].vals.size(); memcpy(p, &cntd, 8);
-      memcpy(p + 8, local[f].vals.data(), sizeof(float) * local[f].vals.size());
-      memcpy(p + 8 + per_feat * sizeof(float), local[f].weights.data(), sizeof(double) * local[f].weights.size());
-    }
-    const int W = comm.world();
-    DevBuf<unsigned char> dsend, drecv; dsend.alloc(sendbuf.size()); drecv.alloc(sendbuf.size() * W);
-    CUDA_OK(cudaMemcpyAsync(dsend.p, sendbuf.data(), sendbuf.size(), cudaMemcpyHostToDevice, s));
-    comm.allgather_bytes(dsend.p, drecv.p, sendbuf.size(), s);
-    std::vector<unsigned char> all(sendbuf.size() * W);
-    CUDA_OK(cudaMemcpyAsync(all.data(), drecv.p, all.size(), cudaMemcpyDeviceToHost, s));
-    Comm::get().sync_stream(s);
-    std::vector<std::vector<FeatureSummary>> per_rank(W, std::vector<FeatureSummary>(F));
-    for (int r = 0; r < W; ++r) {
-      for (int f = 0; f < F; ++f) {
-        const unsigned char* p = all.data() + (size_t)r * sendbuf.size() + (size_t)f * rec;
-        double cntd; memcpy(&cntd, p, 8); size_t c = (size_t)cntd;
-        FeatureSummary& fs = per_rank[r][f];
-        fs.vals.resize(c); fs.weights.resize(c);
-        memcpy(fs.vals.data(), p + 8, sizeof(float) * c);
-        memcpy(fs.weights.data(), p + 8 + per_feat * sizeof(float), sizeof(double) * c);
-      }
-    }
-    std::vector<FeatureSummary> merged;
-    merge_summaries(per_rank, F, &merged);
-    cuts_from_summaries(merged, max_bin, has_missing, &cuts);
-  }
+  if (!comm.distributed()) compute_cuts_device(X.p, n, F, w, max_bin, has_missing, &cuts, s);
+  else merged_rank_cuts(w, max_bin, &cuts);
   binned_max_bin = max_bin;
   bin_with_cuts();
 }
@@ -710,8 +755,9 @@ void Booster::configure() {
     const std::string& t = tm->second;
     B200_CHECK(t == "hist" || t == "auto" || t == "gpu_hist" || t == "approx" || t == "exact",
                "Unknown tree_method: " + t);
-    // every method maps onto the device hist builder; exact/approx are accepted for hyperparameter compatibility
+    // exact is accepted for hyperparameter compatibility and grows hist trees; approx re-sketches the cuts of every tree
   }
+  approx_ = tm != raw_params_.end() && tm->second == "approx";
   auto bo = raw_params_.find("booster");
   if (bo != raw_params_.end()) B200_CHECK(bo->second == "gbtree" || bo->second == "dart", "Only booster=gbtree and booster=dart are implemented on the CUDA hist path (got " + bo->second + ")");
   dart_ = DartParam{};
@@ -1185,7 +1231,9 @@ void Booster::train_round(DMatrix* dtrain, const CustomGradArgs* custom) {
   if (update_mode_) { dtrain->require_raw("process_type=update"); refresh_one_iter(dtrain); return; }    // reads no bins: no binning, no width limit
   if (dart_.on) dtrain->require_raw("booster=dart");
   check_train_width(dtrain);
-  dtrain->ensure_binned(param_.max_bin);
+  const bool resketch = approx_ && (custom || approx_resketch());
+  if (approx_) dtrain->require_raw("tree_method=approx (it re-sketches the cuts of every tree from the raw features)");
+  dtrain->ensure_binned(param_.max_bin, resketch);
   const int K = param_.num_outputs();
   TreeBuilder& b = builder_for(dtrain);
   if (!custom) { check_label_ranges(dtrain); estimate_base_score(dtrain); }
@@ -1199,7 +1247,9 @@ void Booster::train_round(DMatrix* dtrain, const CustomGradArgs* custom) {
   const int P = param_.num_parallel_tree;
   // a forest with row sampling draws one row sample per tree: the gradients of every row go to a round buffer first, and each
   // tree's masked copy (and its scales) is made before the tree is grown.  Otherwise every tree of the round shares them.
-  const bool per_tree_sample = P > 1 && param_.subsample < 1.0f;
+  // approx re-sketches from the hessian before row sampling, so a re-sketched round with row sampling keeps the unsampled
+  // gradients in the round buffer too (tree 0's copy draws the rows the objective's own sample would have kept)
+  const bool per_tree_sample = (P > 1 || resketch) && param_.subsample < 1.0f;
   // sampling_method=gradient_based: the objective writes every row's pairs, each class's threshold is taken once per round on
   // them (the P trees of a forest share it and differ in their draws), and each tree keeps its rows by it
   const bool gbs = gradient_based_sampling();
@@ -1264,6 +1314,8 @@ void Booster::train_round(DMatrix* dtrain, const CustomGradArgs* custom) {
         CUDA_OK(cudaMemcpyAsync(b.gs.absmax, target_absmax_.p + 2 * k, 2 * sizeof(unsigned), cudaMemcpyDeviceToDevice, s));
         launch_scales(b.gs, grad_bits_for(b.global_n), s);
       }
+      // approx: one sketch per class per round, from the class's unsampled hessian, shared by its P trees
+      if (resketch && j == 0) dtrain->rebin_from_hessian((per_tree_sample ? forest_gpair_.p : b.gpair.p) + (size_t)k * b.gp_stride, param_.max_bin);
       grow_one_tree(dtrain, cache, k, iteration_indptr_[round] + k * P + j);
     }
   iteration_indptr_.push_back((int)trees_.size());
@@ -1425,6 +1477,12 @@ bool Booster::constant_hessian(const DMatrix& dm) const {
          param_.subsample >= 1.0f && param_.scale_pos_weight == 1.0f;
 }
 
+// [UPSTREAM-RECALL: ObjFunction::Task().const_hess, true for reg:squarederror, reg:absoluteerror and reg:quantileerror; GPU approx
+// regenerates the cuts with the hessian as weights only when it is false]
+bool Booster::approx_resketch() const {
+  return !(param_.objective == kSquaredError || param_.objective == kAbsoluteError || param_.objective == kQuantileError);
+}
+
 // The only place TreeInputs are filled.  mask: the tree's column sets (empty = no column sampling), uploaded with its index;
 // the constraints are uploaded here too.
 TreeInputs Booster::tree_inputs(const DMatrix& dm, const std::string& mask, int tree_index, float* margin, int k) {
@@ -1458,6 +1516,16 @@ void Booster::grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_i
     for (int d = 0; d < param_.max_depth; ++d) mask += subset_mask(tm, param_.colsample_bylevel, param_.seed, 0x300000ull + 64ull * (uint64_t)tree_index + (uint64_t)d);
   }
   const TreeInputs in = tree_inputs(*dtrain, mask, tree_index, cache.margin.p, k);
+  if (record_cuts_) {
+    HostCuts c; c.ptrs.resize((size_t)dtrain->F + 1); c.mins.resize((size_t)dtrain->F);
+    CUDA_OK(cudaMemcpyAsync(c.ptrs.data(), in.cut_ptrs, sizeof(int) * c.ptrs.size(), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaMemcpyAsync(c.mins.data(), in.min_vals, sizeof(float) * c.mins.size(), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    c.vals.resize((size_t)c.ptrs.back());
+    CUDA_OK(cudaMemcpyAsync(c.vals.data(), in.cut_vals, sizeof(float) * c.vals.size(), cudaMemcpyDeviceToHost, s));
+    CUDA_OK(cudaStreamSynchronize(s));
+    tree_cuts_.push_back(std::move(c));
+  }
   b.grow(in);
   if (in.root_mode == 1) { b.root_h_valid = true; b.root_h_uid = dtrain->uid; b.root_h_version = dtrain->binned_version; }
 

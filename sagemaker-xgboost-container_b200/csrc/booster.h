@@ -61,6 +61,9 @@ class DMatrix {
   HostCuts cuts; DevBuf<int> d_cut_ptrs; DevBuf<float> d_cut_vals, d_min_vals;
   DevBuf<uint8_t> bins, bins_tail, bins_col, bins_gather; int ngroups = 0, tw = 0, ntail = 0, gather_stride = 0;   // engine.h BinnedMatrix layout
   uint64_t binned_version = 0;                        // bumped by every (re)binning: invalidates captured graphs / cached planes
+  // the bins hold a tree's hessian cuts (tree_method=approx), not the matrix's own: the device cuts differ from `cuts`
+  bool hessian_cuts = false;
+  std::unique_ptr<ApproxSketch> approx;               // tree_method=approx on a training matrix: built on its first approx tree
   uint64_t uid;                                       // identity for prediction caches
 
   DMatrix();
@@ -96,7 +99,11 @@ class DMatrix {
   void set_qid(const int64_t* qid, size_t len);       // groups are the runs of equal consecutive qid; qid must not decrease
   int64_t num_groups() const { return group_ptr.empty() ? 1 : (int64_t)group_ptr.size() - 1; }
   const std::vector<float>& get_float_info(const std::string& field) const;
-  void ensure_binned(int max_bin);
+  // the matrix's own cuts at max_bin (hessian_ok: or the hessian cuts an approx tree left, which its next tree replaces anyway)
+  void ensure_binned(int max_bin, bool hessian_ok = false);
+  // tree_method=approx: the cuts of the tree about to grow, from its hessian gp[r].y, and the bins re-made from them in the same
+  // buffers, in launches only (DESIGN.md "Approx")
+  void rebin_from_hessian(const float2* gp, int max_bin);
   void set_cuts(const HostCuts& c);                   // external cuts (shared with the oracle in tests)
   BinnedMatrix binned_view() const { BinnedMatrix b; b.bins = bins.p; b.bins_tail = tw ? bins_tail.p : nullptr; b.bins_col = bins_col.p; b.n = n; b.F = F;
     b.bins_gather = bins_gather.p ? bins_gather.p : bins.p; b.gather_stride = gather_stride; b.tail_in_gather = bins_gather.p && tw == 8 ? 1 : 0;
@@ -106,6 +113,9 @@ class DMatrix {
   void bin_with_cuts();
   void alloc_bins();                                  // uploads the cuts, allocates the main / tail bins with their pad rows
   void finish_bins();                                 // the aligned and column-major copies of the binned main / tail
+  void launch_bin_copies();                           // finish_bins' two copies into their buffers, launches only
+  // the multi-rank cuts (every rank's capped summary with row weights w, nullptr = 1, merged in rank order): collective
+  void merged_rank_cuts(const float* w, int max_bin, HostCuts* out);
 };
 
 // device half of DMatrix::from_csr (ingest.cu): X (nrow x F) filled with NaN, then row r's entries [d_ptr[r], d_ptr[r + 1]) stored
@@ -218,6 +228,9 @@ class Booster {
   void debug_gradient(DMatrix* dm, const float* margin, int round, float* out);
   // process_type=update: the (G_q, H_q) sums of every node of the trees being updated (include/b200xgb.h XGB200BoosterGetRefreshSums)
   void debug_refresh_sums(std::vector<long long>* out);
+  // while on, the cuts every tree grows on are kept (host copies, in model order; include/b200xgb.h XGB200BoosterGetTreeCuts)
+  void set_record_cuts(bool on) { record_cuts_ = on; if (on) tree_cuts_.clear(); }
+  const std::vector<HostCuts>& tree_cuts() const { return tree_cuts_; }
   std::string get_profile();                      // JSON, see include/b200xgb.h
   // histogram of one node for kernel-level parity tests / the roofline bench
   // mode: 0 = production choice (TMA root kernel), 1 = gather kernel, 2 = G-only TMA root kernel (H plane stays zero);
@@ -253,6 +266,8 @@ class Booster {
   std::vector<std::vector<int>> interaction_;   // parsed interaction_constraints (empty = none)
   bool configured_ = false;
   TrainParam param_;
+  bool approx_ = false;                         // tree_method=approx (DESIGN.md "Approx")
+  bool record_cuts_ = false; std::vector<HostCuts> tree_cuts_;
   std::string objective_name_ = "reg:squarederror";
   bool base_score_set_ = false; float base_score_ = 0.5f; bool base_score_estimated_ = false;
   int num_feature_ = 0;
@@ -322,6 +337,9 @@ class Booster {
   void grow_one_tree(DMatrix* dtrain, PredCache& cache, int k, int tree_index);
   // h == 1 for every row in every round on dm: the gradients are a dense float g and the trees grow on it (TreeInputs root_mode)
   bool constant_hessian(const DMatrix& dm) const;
+  // tree_method=approx re-sketches each tree's cuts from its hessian in a round of an objective whose hessian is not constant
+  // (and in every custom round).  With a constant hessian the weighted cuts are the sample-weighted cuts hist grows on.
+  bool approx_resketch() const;
   // sampling_method=gradient_based applies (subsample < 1): the objective writes every row, the trees sample by threshold
   bool gradient_based_sampling() const { return param_.gradient_based && param_.subsample < 1.0f; }
   // tree j of boosting round `round` keeps rows [0, n) of src by the thresholds in gbs_ (launch_gradient_based_sample)

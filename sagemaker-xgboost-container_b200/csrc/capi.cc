@@ -888,6 +888,21 @@ int XGB200BoosterGetRefreshSums(BoosterHandle handle, bst_ulong* len, long long*
   if (out) memcpy(out, v.data(), sizeof(long long) * v.size());
   API_END();
 }
+int XGB200BoosterSetRecordCuts(BoosterHandle handle, int enable) { API_BEGIN(); BST(handle)->set_record_cuts(enable != 0); API_END(); }
+int XGB200BoosterGetTreeCuts(BoosterHandle handle, bst_ulong tree, bst_ulong* num_feature, bst_ulong* num_cuts, int* cut_ptrs, float* cut_vals,
+                             float* min_vals) {
+  API_BEGIN();
+  const std::vector<HostCuts>& all = BST(handle)->tree_cuts();
+  B200_CHECK(tree < all.size(), "XGB200BoosterGetTreeCuts: tree " + std::to_string(tree) + " was not grown while cuts were recorded (" +
+             std::to_string(all.size()) + " recorded)");
+  const HostCuts& c = all[tree];
+  if (num_feature) *num_feature = c.mins.size();
+  if (num_cuts) *num_cuts = c.vals.size();
+  if (cut_ptrs) memcpy(cut_ptrs, c.ptrs.data(), sizeof(int) * c.ptrs.size());
+  if (cut_vals) memcpy(cut_vals, c.vals.data(), sizeof(float) * c.vals.size());
+  if (min_vals) memcpy(min_vals, c.mins.data(), sizeof(float) * c.mins.size());
+  API_END();
+}
 int XGB200BoosterComputeGradient(BoosterHandle handle, DMatrixHandle dmat, const float* margin, int round, float* out_gpair) {
   API_BEGIN();
   B200_CHECK(round >= 0, "XGB200BoosterComputeGradient: round must be >= 0");

@@ -136,4 +136,27 @@ void merge_summaries(const std::vector<std::vector<FeatureSummary>>& per_rank, i
 void compute_rank_cuts_device(const float* dX, int F, const float* dweights, const int64_t* row_bounds, int nranges, int max_bin,
                               bool has_missing, HostCuts* out, cudaStream_t s);
 
+// tree_method=approx (DESIGN.md "Approx"): what a matrix keeps to re-sketch its cuts before every tree on the device.  Only the
+// A features with more distinct values than bins are kept (the cuts of the others do not depend on the weights): each one's
+// non-missing rows in value order and the runs of equal values in that order.
+struct ApproxSketch {
+  bool valid = false;
+  int64_t n = 0; int F = 0, nb = 0, A = 0; int64_t nruns = 0;
+  DevBuf<int> order;                 // kept feature a: rows [elem_off[a], elem_off[a + 1]) in value order
+  DevBuf<int64_t> elem_off;          // [A + 1]
+  DevBuf<int> run_start;             // [nruns]: a run's first entry, relative to its feature's elem_off
+  DevBuf<int64_t> run_off;           // [A + 1]: feature a's runs
+  DevBuf<int> feat;                  // [A]: the feature id of kept feature a
+  DevBuf<double> run_w;              // [nruns]: per tree, each run's weight, then its inclusive cumulative weight
+  DevBuf<float> stage_vals;          // [F][256]: each feature's cuts before they are packed (the others' fixed cuts from the start)
+  DevBuf<int> stage_cnt;             // [F]
+};
+// out[r] = gp[r].y for r < n: one class's hessian as row weights (the multi-rank re-sketch)
+void launch_hessian_column(const float2* gp, int64_t n, float* out, cudaStream_t s);
+// Built once per matrix (host-synchronising, like the one-time cuts): nb bins per feature, `cuts` the matrix's own cuts.
+void approx_sketch_build(const float* dX, int64_t n, int F, int nb, const HostCuts& cuts, ApproxSketch* sk, cudaStream_t s);
+// The cuts of one tree with weights gp[r].y (the tree's hessian) into cut_ptrs ([F + 1]) and cut_vals ([F][256] capacity),
+// in launches only.  The min values do not change: they depend on each feature's first value alone.
+void approx_sketch_cuts(const float* dX, const ApproxSketch& sk, const float2* gp, int* cut_ptrs, float* cut_vals, cudaStream_t s);
+
 }  // namespace b200

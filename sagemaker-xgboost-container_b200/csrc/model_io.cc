@@ -308,8 +308,8 @@ JPtr Booster::config_to_json() {
   learner->set("generic_param", gp);
   JPtr gb = JValue::Object(); gb->set("name", S("gbtree"));
   JPtr gmp = JValue::Object(); gmp->set("num_parallel_tree", S(std::to_string(param_.num_parallel_tree))); gmp->set("num_trees", S(std::to_string(trees_.size()))); gb->set("gbtree_model_param", gmp);
-  JPtr gtp = JValue::Object(); gtp->set("process_type", S(update_mode_ ? "update" : "default")); gtp->set("tree_method", S("hist"));
-  gtp->set("updater", S(update_mode_ ? update_ops_str_ : "grow_b200_hist")); gb->set("gbtree_train_param", gtp);
+  JPtr gtp = JValue::Object(); gtp->set("process_type", S(update_mode_ ? "update" : "default")); gtp->set("tree_method", S(approx_ ? "approx" : "hist"));
+  gtp->set("updater", S(update_mode_ ? update_ops_str_ : approx_ ? "grow_b200_approx" : "grow_b200_hist")); gb->set("gbtree_train_param", gtp);
   JPtr ttp = JValue::Object();
   auto f = [&](const char* k, float v) { ttp->set(k, S(float_repr(v))); }; auto i = [&](const char* k, int v) { ttp->set(k, S(std::to_string(v))); };
   f("alpha", param_.alpha); f("colsample_bylevel", param_.colsample_bylevel); f("colsample_bynode", param_.colsample_bynode); f("colsample_bytree", param_.colsample_bytree);
@@ -359,6 +359,8 @@ void Booster::config_from_json(const JValue& doc) {
       if (auto inner = gb->get("gbtree")) gb = inner;
     }
     if (auto ttp = gb->get("tree_train_param")) for (auto& kv : ttp->obj) if (kv.second->type == JValue::kString) raw_params_[kv.first] = kv.second->s;
+    if (auto gtp = gb->get("gbtree_train_param")) if (auto tm = gtp->get("tree_method")) if (tm->type == JValue::kString)
+      raw_params_["tree_method"] = tm->s == "approx" ? "approx" : "hist";     // save_config writes exact as hist too
     if (auto gtp = gb->get("gbtree_train_param")) if (auto pt = gtp->get("process_type")) if (pt->type == JValue::kString && pt->s == "update") {
       raw_params_["process_type"] = "update";          // the default mode's gbtree_train_param names this engine's own updater
       if (auto up = gtp->get("updater")) if (up->type == JValue::kString) raw_params_["updater"] = up->s;
